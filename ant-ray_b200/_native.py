@@ -122,7 +122,7 @@ def load():
     if not os.path.exists(path):
         raise ImportError(
             f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  ant_ray_b200 has no CPU or NCCL fallback.")
+            "(nvcc, sm_90a).  ant_ray_b200 has no CPU or NCCL fallback.")
     lib = ctypes.CDLL(path, mode=ctypes.RTLD_LOCAL)
     for name, (restype, argtypes) in SYMBOLS.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree

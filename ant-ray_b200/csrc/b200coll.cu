@@ -127,7 +127,7 @@ struct b200c_comm {
   int rank = 0, world = 1, device = 0;
   CUdevice cudev = 0;
   b200c_config_t cfg{};
-  int sm_count = 148;
+  int sm_count = 132;
   // arena
   size_t arena_bytes = 0, gran = 0;
   size_t off_staging = 0, off_p2p = 0, off_mring = 0, off_ll = 0, ll_words = 0, off_sym = 0, sym_bytes = 0;
@@ -208,23 +208,23 @@ extern "C" void b200c_default_config(b200c_config_t* cfg) {
   cfg->staging_bytes = 256ull << 20;
   cfg->symmetric_bytes = 0;
   cfg->p2p_slot_bytes = 32ull << 10;
-  cfg->p2p_slots = 1024;   // 32 MiB per ordered pair: at ~500 GB/s the ring must hold the ~60 us of data a ready/ack round trip is behind
-  cfg->max_blocks = 296;
+  cfg->p2p_slots = 1024;   // 32 MiB per ordered pair: the ring must hold the data a ready/ack round trip is behind
+  cfg->max_blocks = 264;   // 2 CTAs of 512 threads on each of the 132 SMs of an H100
   cfg->oneshot_max_bytes = 0;  // 0 = pick by world size in b200c_comm_create
   cfg->nvls_min_bytes = (1ull << 20) + 1;
-  cfg->nvls_pipe_min_bytes = 32ull << 20;  // staged NVLS pieces from 32 MiB up run round-pipelined (W=8: 540 vs 505 GB/s at 64 MiB)
+  cfg->nvls_pipe_min_bytes = 32ull << 20;  // staged NVLS pieces from 32 MiB up run round-pipelined
   cfg->timeout_ms = 600000;  // a slow peer (data loading, first-step autotuning skew) is not a dead peer
   cfg->granule_bytes = 32ull << 10;
-  cfg->ll_max_bytes = 64ull << 10;    // W=8: LL 12 us vs one-shot 13 us at 64 KiB, 15 vs 15 at 128 KiB (profiles/r02_sweep8_small.log)
+  cfg->ll_max_bytes = 64ull << 10;
   cfg->bcast_rounds_min_bytes = 4ull << 20;
   cfg->nvls_unroll = 4;
-  cfg->nvls_streams_min_bytes = 768ull << 20;   // W=8, 1 GiB: 737 GB/s vs 704 (rounds kernel) and NCCL 726; 512 MiB: a tie (r02_sweep8_streams.log)
+  cfg->nvls_streams_min_bytes = 768ull << 20;
   cfg->nvls_streams_piece_bytes = 128ull << 20;
   cfg->rounds_order = 0;
   cfg->nvls_lanes = 48;
   cfg->lane_granule_bytes = 64ull << 10;
   cfg->nvls_lanes_min_bytes = 0;   // opt-in until measured on the target box
-  cfg->nvls_blocks = 32;   // zero-copy NVLS saturates the switch with 32 CTAs; more only scatter the access pattern (r02_sweep8_large.log)
+  cfg->nvls_blocks = 32;   // zero-copy NVLS: a few CTAs saturate the switch; more only scatter the access pattern
 }
 
 static int ensure_driver() {
@@ -312,7 +312,7 @@ extern "C" int b200c_comm_create(int rank, int world, int device, const b200c_co
   if (cfg.lane_granule_bytes % 8192) return fail(B200C_EINVAL, "lane_granule_bytes must be a multiple of 8 KiB");
   if (cfg.nvls_streams_piece_bytes == 0) cfg.nvls_streams_piece_bytes = 128ull << 20;
   if (cfg.nvls_streams_piece_bytes % (1u << 20)) return fail(B200C_EINVAL, "nvls_streams_piece_bytes must be a multiple of 1 MiB");
-  // measured crossovers (profiles/r01_sweep_*): W=2 one-shot wins to 8 MiB; W=8 one-shot 23 us vs NVLS 28 us at 1 MiB
+  // one-shot (one flag round, (W-1)*S pushed) pays off for small messages, longer at W=2 where it moves the least
   if (cfg.oneshot_max_bytes == 0) cfg.oneshot_max_bytes = world <= 2 ? (8ull << 20) : (1ull << 20);
 
   int ndev = 0;
@@ -507,8 +507,8 @@ extern "C" int b200c_comm_ready(b200c_comm_t* c) {
   d.mcells = (int)c->mcells;
   d.off_ll = c->off_ll;
   d.ll_words = c->ll_words;
-  // a single multimem.st stream leaves the root at ~340 GB/s (measured), a unicast push at ~690 GB/s:
-  // multicast pays off as soon as there is more than one receiver
+  // multicast: the root's payload leaves it once whatever the number of receivers, so it is chosen as soon as
+  // there is more than one
   c->bcast_mc = c->world > 2;
   if (const char* e = getenv("B200COLL_BCAST_MULTICAST")) c->bcast_mc = e[0] == '1';
   c->ready = true;
@@ -1018,7 +1018,7 @@ static int allreduce_impl(b200c_comm* c, const void* send, void* recv, size_t co
     if (al == B200C_ALGO_AUTO) {
       if (ll_ok && count * esz <= c->cfg.ll_max_bytes) al = B200C_ALGO_LL;
       else if (bytes_left <= c->cfg.oneshot_max_bytes) al = B200C_ALGO_ONESHOT;
-      else if (nvls_ok && W > 2 && bytes_left >= c->cfg.nvls_min_bytes && (W >= 6 || in_sym)) al = B200C_ALGO_NVLS;  // W = 4: two-shot beats STAGED NVLS (r02_sweep4_large.log)
+      else if (nvls_ok && W > 2 && bytes_left >= c->cfg.nvls_min_bytes && (W >= 6 || in_sym)) al = B200C_ALGO_NVLS;  // W = 4: two-shot beats staged NVLS
       else al = B200C_ALGO_TWOSHOT;
     }
     CollArgs a;

@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(kThreads) k_broadcast(const __grid_constant__ 
 //             granules out of its staging into the user buffer.
 // Root egress is ~S (unicast (W-1)/W*S + multicast S/W) instead of (W-1)*S, and — unlike the root-only
 // multicast — the W-1 receivers share the multicast work, so no single multimem.st stream is the bottleneck.
-__global__ void __launch_bounds__(kThreads) k_broadcast_rounds(const __grid_constant__ CollArgs a) {
+__global__ void __launch_bounds__(kThreads, 2) k_broadcast_rounds(const __grid_constant__ CollArgs a) {
   const DevComm& c = a.c;
   const int r = c.rank, W = c.world, root = a.root;
   if (!coll_prologue(a)) return;
@@ -216,8 +216,8 @@ struct P2PArgs {
   int batch;          // pairwise send: cells published per release fence (1..kSendBatch)
 };
 
-// A system-scope release fence costs ~3 us on a quiet SM and ~15 us while the SM's other warps stream
-// stores to the peer (profiles/r02_probe_2gpu_exp.log, E3), so a sender block publishes kSendBatch
+// A system-scope release fence costs far more while the SM's other warps stream stores to the peer than
+// on a quiet SM, so a sender block publishes kSendBatch
 // cells per fence: copy cells i, i+grid, ... , then one __syncthreads + fence and one flag per cell.
 constexpr int kSendBatch = 4;
 

@@ -1,4 +1,4 @@
-// Collective kernels over peer-mapped arenas (hand-written for sm_100a; no NCCL on this path).
+// Collective kernels over peer-mapped arenas (hand-written for sm_90a; no NCCL on this path).
 //
 // Partitioning (SURVEY.md §8e): a piece of n elements is cut into `world` rank chunks of
 // `chunk` elements; each chunk is cut into granules of `tile` elements.  Block b of every rank
@@ -34,7 +34,7 @@ __device__ __forceinline__ size_t clip_count(size_t lo, size_t hi, size_t n) {
 
 // The reducing kernels are compiled once per world size (WT = 2, 4, 8; WT = 0 takes the world size at run time for
 // 3, 5, 6, 7): with the four reduce loops in one kernel the register allocator spilled loop invariants into local
-// memory under the 64-register budget; one loop per kernel compiles without a stack (profiles/*_sass_local_memory.txt).
+// memory under the 64-register budget; one loop per kernel keeps most of them free of a stack (tests/test_sass_hygiene.py).
 // ---------------------------------------------------------------------------------------------
 // one-shot allreduce: push the whole buffer to every peer, reduce locally.  One flag round.
 // staging slot s (n_pad elements of TW) on rank j holds rank s's data.
@@ -175,7 +175,9 @@ __device__ __forceinline__ void ll_allreduce_body(const CollArgs& a) {
 }
 
 constexpr int kLLThreads = 256;
-template <typename T, int OP>
+// one kernel per world size (WT = 2, 4, 8; 0 = the others), like the other reducers: with the four bodies in one
+// kernel the register allocator kept the in-flight vectors of the wider bodies in local memory
+template <typename T, int OP, int WT>
 __global__ void __launch_bounds__(kLLThreads) k_allreduce_ll(const __grid_constant__ CollArgs a) {
   const DevComm& c = a.c;
   const int t = threadIdx.x;
@@ -186,12 +188,7 @@ __global__ void __launch_bounds__(kLLThreads) k_allreduce_ll(const __grid_consta
     unsigned long long tagged = ((unsigned long long)a.seq << 32) | a.sig;
     asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sig), "l"(tagged) : "memory");
   }
-  switch (c.world) {
-    case 2: ll_allreduce_body<T, OP, 2>(a); break;
-    case 4: ll_allreduce_body<T, OP, 4>(a); break;
-    case 8: ll_allreduce_body<T, OP, 8>(a); break;
-    default: ll_allreduce_body<T, OP, 0>(a); break;
-  }
+  ll_allreduce_body<T, OP, WT>(a);
   // arrival (the op after this one may start: arrive rule) goes last so that the fence of the release
   // does not sit in front of the data stores
   if (blockIdx.x == 0 && t < c.world && t != c.rank) {
@@ -340,9 +337,7 @@ __device__ __forceinline__ void multimem_st16(void* p, uint4 v) {
 }
 
 // in-switch reduce of nv 16-byte vectors at multicast address `mc`, broadcast back in place.
-// U = 4 vectors are in flight per thread.  (Eight were tried for the staged kernels, whose bursts between local copies
-// are short: 705-708 GB/s against 705 at 1 GiB, W=8 - profiles/r02_sweep8_unroll_order.log - and the second code path
-// cost the rounds kernel its spill-free register allocation, so it was removed.)
+// U = 4 vectors are in flight per thread.
 template <typename TW, int U>
 __device__ __forceinline__ void nvls_reduce_bcast_u(char* mc, size_t nv, const CollArgs& a, size_t i) {
   constexpr int V = 16 / sizeof(TW);
@@ -510,8 +505,8 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_rounds(const __g
 // 1 + Kc CTAs.  CTA 0 of a lane only talks to the switch (multimem.ld_reduce / multimem.st and the two
 // cross-GPU flags of its lane); the other Kc CTAs only move data locally (user tensor -> ring, ring ->
 // user tensor).  Roles meet through flags in LOCAL memory, so
-//   * the system-scope release fences (3 us on a quiet SM, 15-20 us on an SM that streams stores:
-//     profiles/r02_probe*_exp.log E3) sit in the switch CTAs, where nothing else streams, and never stall
+//   * the system-scope release fences (expensive on an SM that streams stores) sit in the switch CTAs,
+//     where nothing else streams, and never stall
 //     a copy;
 //   * few CTAs issue multimem traffic (the switch saturates with ~32 CTAs; more only scatter the access
 //     pattern) while many CTAs drive the local HBM copies;

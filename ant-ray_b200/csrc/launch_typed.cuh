@@ -14,6 +14,7 @@ static int launch_kind_w(int kind, const CollArgs& a, int grid, cudaStream_t s) 
     case KIND_TWOSHOT: k_allreduce_twoshot<T, T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;
     case KIND_REDUCESCATTER: k_reducescatter<T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;
     case KIND_REDUCE: k_reduce<T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;
+    case KIND_LL: k_allreduce_ll<T, OP, WT><<<grid, kLLThreads, 0, s>>>(a); break;
     default: return B200C_EINVAL;
   }
   return B200C_OK;
@@ -22,10 +23,6 @@ static int launch_kind_w(int kind, const CollArgs& a, int grid, cudaStream_t s) 
 // the reducing kernels exist once per world size 2 / 4 / 8 and once for the other sizes (WT = 0)
 template <typename T, int OP>
 static int launch_kind(int kind, const CollArgs& a, int grid, cudaStream_t s) {
-  if (kind == KIND_LL) {
-    k_allreduce_ll<T, OP><<<grid, kLLThreads, 0, s>>>(a);
-    return B200C_OK;
-  }
   switch (a.c.world) {
     case 2: return launch_kind_w<T, OP, 2>(kind, a, grid, s);
     case 4: return launch_kind_w<T, OP, 4>(kind, a, grid, s);

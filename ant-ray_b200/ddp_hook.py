@@ -106,7 +106,6 @@ def make_grad_state(world_size: Optional[int] = None, rank: Optional[int] = None
         # (the bucket traffic needs a tiny fraction of NVLink), like NCCL's handful of channels.
         from .b200_group import make_config
 
-        # 64 CTAs: 1.07 ms of hook time per ResNet-50 step at 8 GPUs against 2.04 ms with 32 (profiles/r02_bench_8gpu*.json)
         config = make_config(max_blocks=int(os.environ.get("B200COLL_HOOK_MAX_BLOCKS", "64")))
     comm = PeerMemoryComm(world_size, rank, next_comm_key("train/" + name), device, store, config)
     return B200GradState(comm, wire=wire, **kw)

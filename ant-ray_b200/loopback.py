@@ -41,7 +41,7 @@ class LoopbackWorld:
     def __init__(self, world_size: int, device: int = 0, key: str = "loopback", **config_overrides):
         self.world_size, self.device = world_size, device
         sm = torch.cuda.get_device_properties(device).multi_processor_count
-        cfg_kw = dict(max_blocks=max(1, min(296, (2 * sm) // world_size - 2)), staging_bytes=32 << 20)
+        cfg_kw = dict(max_blocks=max(1, min(264, (2 * sm) // world_size - 2)), staging_bytes=32 << 20)
         cfg_kw.update(config_overrides)
         store = _MemStore()
         self.comms: List[Optional[PeerMemoryComm]] = [None] * world_size

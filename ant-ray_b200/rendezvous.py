@@ -175,6 +175,8 @@ def default_store() -> Store:
 # fd passing (SCM_RIGHTS) over an abstract-namespace Unix socket
 # --------------------------------------------------------------------------------------------
 _REQ = struct.Struct("<ii")  # (requester rank, kind) kind: 0 = arena export, 1 = multicast fd
+_LOCAL_SERVERS = {}  # address -> FdServer of this process (see FdServer.take)
+_LOCAL_LOCK = threading.Lock()
 
 
 class FdServer:
@@ -200,6 +202,8 @@ class FdServer:
         self.stop = threading.Event()
         self.thread = threading.Thread(target=self._serve, name="b200coll-fd-server", daemon=True)
         self.thread.start()
+        with _LOCAL_LOCK:
+            _LOCAL_SERVERS[self.address] = self
 
     def offer(self, kind: int, data: bytes, fd: int):
         with self.lock:
@@ -235,6 +239,26 @@ class FdServer:
                 return False
             self.served.add((rank, kind))
         return True
+
+    def take(self, rank: int, kind: int, timeout_s: float):
+        """In-process counterpart of fetch_fd for a peer rank in this very process (a loopback world):
+        (payload bytes, a duplicate of the offered fd).  Same rank / served-once rules as the socket path;
+        no descriptor has to cross a socket, which not every container runtime allows for CUDA's
+        shareable-handle fds."""
+        if self.world is not None and not (0 <= rank < self.world and rank != self.rank):
+            raise OSError(f"rank {rank} may not fetch from rank {self.rank}")
+        deadline = time.monotonic() + timeout_s
+        while True:
+            with self.lock:
+                item = self.payloads.get(kind)
+                if item is not None:
+                    if (rank, kind) in self.served:
+                        raise OSError(f"descriptor {kind} already served to rank {rank}")
+                    self.served.add((rank, kind))
+                    return item[0], os.dup(item[1])
+            if time.monotonic() > deadline or self.stop.is_set():
+                raise RendezvousTimeout(f"peer offered no descriptor {kind} within {timeout_s}s")
+            time.sleep(0.001)
 
     def _serve(self):
         while not self.stop.is_set():
@@ -276,11 +300,22 @@ class FdServer:
 
     def close(self):
         self.stop.set()
+        with _LOCAL_LOCK:
+            _LOCAL_SERVERS.pop(self.address, None)
         try:
             self.sock.close()
         except OSError:
             pass
         self.thread.join(timeout=2)
+
+
+def _fetch_from_peer(address, my_rank: int, kind: int, timeout_s: float):
+    """fetch_fd, or FdServer.take when the serving rank lives in this process."""
+    with _LOCAL_LOCK:
+        local = _LOCAL_SERVERS.get(address.decode() if isinstance(address, bytes) else address)
+    if local is not None:
+        return local.take(my_rank, kind, timeout_s)
+    return fetch_fd(address, my_rank, kind, timeout_s)
 
 
 def fetch_fd(address: str, my_rank: int, kind: int, timeout_s: float):
@@ -402,7 +437,7 @@ def establish(comm: int, store: Store, prefix: str, rank: int, world: int, share
             for peer in range(world):
                 if peer == rank:
                     continue
-                data, fd = fetch_fd(addrs[peer], rank, 0, timeout_s)
+                data, fd = _fetch_from_peer(addrs[peer], rank, 0, timeout_s)
                 try:
                     pe = N.Export.from_buffer_copy(data)
                     pe.fd = fd
@@ -433,7 +468,7 @@ def establish(comm: int, store: Store, prefix: str, rank: int, world: int, share
             ok = flags[0] == b"1"
             if ok and rank != 0:
                 try:
-                    _, fd = fetch_fd(addrs[0], rank, 1, timeout_s)
+                    _, fd = _fetch_from_peer(addrs[0], rank, 1, timeout_s)
                     try:
                         N.check(lib.b200c_comm_mc_import(comm, fd))
                     finally:

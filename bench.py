@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 collective / tensor-transport layer.
+"""bench.py — headline benchmark of the peer-memory collective / tensor-transport layer on H100.
 
-Metric (BASELINE.json): "allreduce bus GB/s vs msg size; Ray Train ResNet-50 img/s at 1/2/4/8 B200".
+Metric: "allreduce bus GB/s vs msg size; Ray Train ResNet-50 img/s at 1/2/4/8 H100".
   value / e2e        ResNet-50 DDP synthetic-image training throughput (whole job, weak scaling),
                      gradients reduced by the fused peer-memory hook (ant_ray_b200.ddp_hook); e2e copies
                      every step's batch from pinned host memory (side stream, double-buffered) and reads
@@ -27,6 +27,10 @@ Launch:  python bench.py --gpus 1 --steps K --warmup W
          python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
              --master-port P bench.py --gpus N --steps K --warmup W
          python bench.py --impl reference ...      (the reference's CPU path, rank 0 only)
+
+--dump-outputs DIR writes what the last timed step computed (its loss and a fixed, seeded sample of the
+updated parameters, float32, with the sampled positions as float64) as .npy files, so that two builds can be
+compared output for output.
 """
 import argparse
 import json
@@ -42,12 +46,11 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 RESNET50_PARAMS = 25_557_032
-NVLINK_PEAK_MEASURED = 770.0   # GB/s per direction per GPU, peer copy (B200_PROFILING.md)
-NVLINK_PEAK_NOMINAL = 900.0
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the N = 1 roofline kernel, from the committed
-# `ncu --set full` capture (profiles/r02_ncu_full_local_scale_tma_details.txt: k_local_scale_tma<float, bf16_t>, 30 MiB bucket):
-# 31.47 MB read; the 31.46 MB written are still dirty in the 126 MB L2 when the kernel ends (ncu: 0.00 MB)
-NCU_TRAFFIC_LOCAL_SCALE_30MIB = 31_465_216 + 1_792_000   # read + write of the second of four captured launches
+# NVIDIA data sheet, H100 SXM (700 W): NVLink 4 at 450 GB/s per direction per GPU, HBM3 at 3.35 TB/s.
+# Data-sheet bounds for the roofline fractions, not rates measured on this code.
+NVLINK_PEAK_NOMINAL = 450.0
+HBM_PEAK_NOMINAL = 3350.0
+DUMP_PARAM_SAMPLE = 1 << 20   # parameters sampled into --dump-outputs (4 MiB of float32)
 
 
 def log(msg):
@@ -70,7 +73,12 @@ def parse():
     p.add_argument("--no-p2p", action="store_true")
     p.add_argument("--no-comm-bound", action="store_true")
     p.add_argument("--sweep-max-bytes", type=int, default=int(os.environ.get("BENCH_SWEEP_MAX", 1 << 30)))
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write the last timed step's loss and a seeded sample of the updated parameters as DIR/<name>.npy")
+    args = p.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        p.error("--dump-outputs needs --steps >= 1: it writes what the last timed step computed")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------
@@ -176,19 +184,36 @@ def max_over_ranks(value, dist, world):
 
 
 def timed_steps(step, x, y, steps, dist, world):
-    """Device-resident inputs: exactly `steps` steps between two fences, CUDA events, max over ranks."""
+    """Device-resident inputs: exactly `steps` steps between two fences, CUDA events, max over ranks.
+    Also returns the loss tensor of the last step."""
     import torch
 
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     fence(dist, world)
     t0 = time.time()
     e0.record()
+    loss = None
     for _ in range(steps):
-        step(x, y)
+        loss = step(x, y)
     e1.record()
     fence(dist, world)
     t1 = time.time()
-    return max_over_ranks(e0.elapsed_time(e1), dist, world), (t0, t1)
+    return max_over_ranks(e0.elapsed_time(e1), dist, world), (t0, t1), loss
+
+
+def dump_outputs(out_dir, loss, model):
+    """What the last timed step computed: its loss and the parameters the optimizer step left behind.  The
+    parameters (25.6 M floats) are sampled at DUMP_PARAM_SAMPLE fixed, seeded positions of their flat concatenation."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    with torch.no_grad():
+        flat = torch.cat([p.detach().float().reshape(-1) for p in model.parameters()])
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_PARAM_SAMPLE].sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample_index.npy"), idx.numpy().astype(np.float64))
 
 
 def timed_steps_e2e(step, x_host, y_host, steps, dist, world, device):
@@ -290,8 +315,8 @@ def time_back_to_back(fn, bufs, iters, dist, world, rounds=3):
 
 def time_torch_copy_same_size(nbytes, dist, world):
     """torch's own out-of-place copy of the same number of bytes, back to back (read nbytes + write nbytes): what a
-    plain STREAM-style kernel reaches at THIS size — the driver's MEASURED_PEAKS figure is a 2 GiB copy, whose
-    ramp-up and launch gap are amortised over ~650 us instead of ~10 us."""
+    plain STREAM-style kernel reaches at THIS size, where ramp-up and launch gap weigh on ~10 us of work instead of
+    being amortised as in a multi-GiB copy."""
     import torch
 
     n = nbytes // 4
@@ -746,7 +771,7 @@ def run_comm_bound(args, dist, world, device, steps=30, warmup=8):
 
 
 # ------------------------------------------------------------------------------------------------
-# RLlib-shaped learner update (BASELINE config 5): KB-scale gradients, latency-bound
+# RLlib-shaped learner update: KB-scale gradients, latency-bound
 # ------------------------------------------------------------------------------------------------
 def run_ppo_shape(dist, world, rank, device, steps=200, warmup=30):
     """RLlib's TorchLearner wraps the RLModule in DistributedDataParallel when num_learners > 1
@@ -936,7 +961,7 @@ def workload_config(B, world, wire):
                         "synthetic randn(B,3,224,224), SGD momentum, bf16 autocast, fp32 grads",
             "model": "torchvision.resnet50", "per_gpu_batch": B, "global_batch": B * world, "parallelism": f"dp{world}",
             "grad_wire": wire, "grad_bytes_per_step": RESNET50_PARAMS * 4,
-            "l2": "per-step working set (activations of the batch) is far larger than the 126 MB L2; "
+            "l2": "per-step working set (activations of the batch) is far larger than the 50 MB L2; "
                   "the sweeps rotate buffers totalling >= 256 MB"}
 
 
@@ -987,13 +1012,20 @@ def main():
     assert world == args.gpus, f"--gpus {args.gpus} but WORLD_SIZE={world}: launch with torchrun for N > 1"
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs CUDA devices (the b200 path has no CPU fallback)")
+    # Same arguments, same result: two runs must compute the same bits, so that two builds can be compared output
+    # for output.  cuDNN autotuning (cudnn.benchmark) times candidate convolution algorithms on every run and may
+    # pick a different one - with different rounding - each time, which 35 SGD steps amplify far beyond rounding.
+    # The heuristic choice is fixed, as fast on an H100 as the autotuned one, and gives identical outputs run after
+    # run (DESIGN.md §4).  The cuBLAS workspace setting (which must precede cuBLAS's start) keeps its reductions in
+    # a fixed order too.
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     os.environ.setdefault("MASTER_PORT", "29533")
     os.environ.setdefault("B200COLL_TIMEOUT_MS", "60000")  # a benchmark should fail fast, not wait out the production default
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
-    torch.backends.cudnn.benchmark = True
+    torch.backends.cudnn.benchmark = False
     N.load()
     optional_errors = {}
 
@@ -1020,19 +1052,21 @@ def main():
     l0 = N.launch_count()
     if os.environ.get("BENCH_CUDA_PROFILER") == "1":  # ncu --profile-from-start off: capture the timed region only
         torch.cuda.profiler.start()
-    ms, win1 = timed_steps(step, x, y, args.steps, dist, world)
+    ms, win1, last_loss_dev = timed_steps(step, x, y, args.steps, dist, world)
     if os.environ.get("BENCH_CUDA_PROFILER") == "1":
         torch.cuda.profiler.stop()
     launches = N.launch_count() - l0
     ktimes = state.kernel_times_ms()
     state.time_kernels = False
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss_dev, model)
     log("timing end-to-end steps")
     # ---- end to end: inputs from pinned host memory every step, loss read back every step
     ms_e2e, win2, last_loss = timed_steps_e2e(step, x_host, y_host, args.steps, dist, world, device)
     value = world * B * args.steps / (ms / 1e3)
     e2e = world * B * args.steps / (ms_e2e / 1e3)
 
-    # ---- stock DDP reducer over NCCL on the same box (B-DDP baseline, BASELINE.md section 3)
+    # ---- stock DDP reducer over NCCL on the same box (baseline)
     nccl_ddp = None
     log("stock NCCL DDP baseline")
     if not args.no_nccl_ddp:
@@ -1047,7 +1081,7 @@ def main():
             s2 = make_step(m2, o2, use_autocast=True, device=device)
             for _ in range(max(3, args.warmup)):
                 s2(x, y)
-            ms2, _ = timed_steps(s2, x, y, args.steps, dist, world)
+            ms2, _, _ = timed_steps(s2, x, y, args.steps, dist, world)
             nccl_ddp = world * B * args.steps / (ms2 / 1e3)
             del m2, o2, s2
         except Exception as e:  # noqa: BLE001
@@ -1123,34 +1157,26 @@ def main():
             by_size.setdefault(nbytes, []).append(t_ms)
         big = max(by_size) if by_size else 0
         t_big = statistics.mean(by_size[big]) if by_size else None
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except OSError:
-            pass
-
         def roofline_for(t_us, nelem, where):
             if world > 1:
                 alg = 2 * (world - 1) / world * nelem * wire_b  # NVLink bytes in (== out) per GPU per launch
                 ach = alg / (t_us * 1e-6) / 1e9
                 return {"bound": "nvlink", "kernel": f"fused gradient allreduce ({args.wire} wire, fp32 accumulate, x1/W), "
                                                      f"{nelem * 4 >> 20} MiB fp32 bucket, {where}",
-                        "achieved": round(ach, 1), "peak": NVLINK_PEAK_MEASURED, "peak_nominal": NVLINK_PEAK_NOMINAL, "unit": "GB/s",
-                        "frac": round(ach / NVLINK_PEAK_MEASURED, 3), "traffic": None, "launch_us": round(t_us, 2),
+                        "achieved": round(ach, 1), "peak": NVLINK_PEAK_NOMINAL, "unit": "GB/s",
+                        "frac": round(ach / NVLINK_PEAK_NOMINAL, 3), "traffic": None, "launch_us": round(t_us, 2),
                         "algorithmic_bytes": int(alg),
-                        "peak_source": "measured peer copy per direction (B200_PROFILING.md), of measured; nominal 900"}
+                        "peak_source": "H100 SXM data sheet, NVLink per direction per GPU"}
             alg = nelem * 8  # read fp32 + write fp32
             ach = alg / (t_us * 1e-6) / 1e9
-            peak = peaks.get("hbm_gbs", 6650.0)
+            peak = HBM_PEAK_NOMINAL
             return {"bound": "hbm", "kernel": f"k_local_scale_tma<float, {args.wire}>: fused gradient scale / wire rounding (world=1), {nelem * 4 >> 20} MiB fp32 bucket, {where}",
                     "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 3),
-                    "traffic": NCU_TRAFFIC_LOCAL_SCALE_30MIB if nelem == (30 << 18) else None,
-                    "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture "
-                                    "(profiles/r02_ncu_full_local_scale_tma_details.txt); the written half is still dirty in L2 at kernel end",
+                    "traffic": None,
                     "launch_us": round(t_us, 2), "algorithmic_bytes": int(alg),
                     "torch_copy_same_bytes_gbs": round(copy_same_size, 1) if copy_same_size else None,
                     "frac_of_torch_copy_same_bytes": round(ach / copy_same_size, 3) if copy_same_size else None,
-                    "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)"}
+                    "peak_source": "H100 SXM data sheet, HBM3"}
 
         # `roofline`: the kernel timed alone, back to back (what the burst peak is comparable with);
         # `roofline_in_step`: the same kernel inside the training step, where it shares the GPU with the

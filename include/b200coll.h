@@ -1,7 +1,7 @@
 /*
  * b200coll.h — C-ABI of the B200 peer-memory collective / tensor-transport library.
  *
- * This is the drop-in boundary for the hot path named in BASELINE.json (SURVEY.md §8b).
+ * This is the drop-in boundary for the hot path (SURVEY.md §8b).
  * The reference has no C seam of its own on this path: its only native boundary is
  * cupy's NcclCommunicator, which takes raw integer device pointers, element counts,
  * NCCL dtype / redop enums and a raw stream pointer.  Every entry point below replaces

@@ -173,9 +173,12 @@ def test_basic_apis(workers):
     with pytest.raises(RuntimeError):  # initialising the same group twice
         get(actors[0].init_group.remote(2, 0, "gloo", "default"))
     assert get(actors[0].report_gloo_availability.remote()) is True
-    assert get(actors[0].report_nccl_availability.remote()) is False  # no GPU here -> B200 backend unavailable
-    with pytest.raises(RuntimeError):
-        get(actors[0].init_group.remote(2, 0, Backend.B200, "gpu_group"))
+    # the B200 backend is available exactly where a CUDA device is (the workers are forked from this process)
+    has_gpu = torch.cuda.is_available()
+    assert get(actors[0].report_nccl_availability.remote()) is has_gpu
+    if not has_gpu:
+        with pytest.raises(RuntimeError):
+            get(actors[0].init_group.remote(2, 0, Backend.B200, "gpu_group"))
 
 
 def test_backend_names():

@@ -213,22 +213,24 @@ def test_multi_reader_channel_sends_once(pair, world):
             if r == 0:
                 chans[0].write(ts)
                 return None
-            return [g.cpu() for g in chans[r].read(30)]
+            return chans[r].read(30)
 
+        # results are copied to the host after every rank joined: a reader's device -> host copy must not queue
+        # behind a peer's kernel that is still waiting
         res = e.run(step)
         for r in readers:
-            assert torch.equal(res[r][0], torch.full((70_000 + i,), float(i))) and torch.equal(res[r][1], torch.arange(5 + i))
+            assert torch.equal(res[r][0].cpu(), torch.full((70_000 + i,), float(i))) and torch.equal(res[r][1].cpu(), torch.arange(5 + i))
     # 2 tensors per message: 1 send_multi + (world-1) recvs each
     assert N.launch_count() - launches0 == n_msgs * 2 * (1 + len(readers))
     # ring wrap: a message of 3 x 64 cells goes through the 64-cell multi-reader ring with per-reader acks
     big = torch.randint(0, 255, (3 * 64 * (32 << 10) + 17,), dtype=torch.uint8, device="cuda")
-    res = e.run(lambda r: chans[0].write([big]) if r == 0 else chans[r].read(30)[0].cpu())
+    res = e.run(lambda r: chans[0].write([big]) if r == 0 else chans[r].read(30)[0])
     for r in readers:
-        assert torch.equal(res[r], big.cpu())
+        assert torch.equal(res[r].cpu(), big.cpu())
     # a second reader set from the same writer is refused by the native layer, and served by per-reader sends
     other = [TensorListChannel(e.comms[r], 0, [1], QueueMeta([1]).for_rank(r)) for r in range(2)]
-    got = e.run(lambda r: other[0].write([torch.ones(4, device="cuda")]) if r == 0 else other[1].read(30)[0].cpu(), ranks=[0, 1])[1]
-    assert torch.equal(got, torch.ones(4))
+    got = e.run(lambda r: other[0].write([torch.ones(4, device="cuda")]) if r == 0 else other[1].read(30)[0], ranks=[0, 1])[1]
+    assert torch.equal(got.cpu(), torch.ones(4))
     if world > 3:
         bad = TensorListChannel(e.comms[0], 0, [1, 2], QueueMeta([1, 2]).for_rank(0))
         from ant_ray_b200.communicator import RayChannelError
@@ -250,38 +252,27 @@ def test_collectives_match_torch(pair, world, dtype):
     expect = {"MIN": stacked.min(0).values, "MAX": stacked.max(0).values}
     if world == 2:  # order-independent: exact (test_torch_tensor_dag.py:1340-1450)
         expect.update({"SUM": stacked.sum(0), "PRODUCT": stacked.prod(0), "AVG": (stacked.float().sum(0) / 2).to(dtype)})
+    # inputs and outputs are placed on the device before the ranks start, results are read after they joined: a
+    # rank's host <-> device copy must not queue behind a peer's kernel that is already waiting for this rank
+    dev = [t.cuda() for t in ins]
+
+    def run(fn, out_numel):
+        outs = [torch.empty(out_numel, dtype=dtype, device="cuda") for _ in range(world)]
+        e.run(lambda r: fn(r, outs[r]))
+        return [o.cpu() for o in outs]
+
     for op, want in expect.items():
-        def step(r):
-            x = ins[r].cuda()
-            out = torch.empty_like(x)
-            e.comms[r].allreduce(x, out, getattr(DagReduceOp, op))
-            return out.cpu()
-        for o in e.run(step):
+        for o in run(lambda r, out: e.comms[r].allreduce(dev[r], out, getattr(DagReduceOp, op)), n):
             assert torch.equal(o, want), op
     if world > 2:  # the kernels fold ranks 0..W-1 in order with fp32 accumulation: compare with exactly that
         from oracle import oracle as O
-        def step(r):
-            x = ins[r].cuda()
-            out = torch.empty_like(x)
-            e.comms[r].allreduce(x, out, DagReduceOp.SUM)
-            return out.cpu()
-        for o in e.run(step):
+        for o in run(lambda r, out: e.comms[r].allreduce(dev[r], out, DagReduceOp.SUM), n):
             assert torch.equal(o, O.allreduce(ins))
 
-    def gather(r):
-        x = ins[r].cuda()
-        out = torch.empty(n * world, dtype=dtype, device="cuda")
-        e.comms[r].allgather(x, out)
-        return out.cpu()
-    for o in e.run(gather):
+    for o in run(lambda r, out: e.comms[r].allgather(dev[r], out), n * world):
         assert torch.equal(o, torch.cat(ins))
 
-    def rs(r):
-        x = ins[r].cuda()
-        out = torch.empty(n // world, dtype=dtype, device="cuda")
-        e.comms[r].reducescatter(x, out, DagReduceOp.MAX)
-        return out.cpu()
-    for r, o in enumerate(e.run(rs)):
+    for r, o in enumerate(run(lambda r, out: e.comms[r].reducescatter(dev[r], out, DagReduceOp.MAX), n // world)):
         assert torch.equal(o, stacked.max(0).values[r * (n // world):(r + 1) * (n // world)])
 
 

@@ -249,7 +249,7 @@ class RawWorker:
         return x.cpu()
 
     def big_properties(self, n):
-        """Size-independent checks at BASELINE's largest message (1 GiB): see test_full_size_properties."""
+        """Size-independent checks at the sweep's largest message (1 GiB): see test_full_size_properties."""
         from ant_ray_b200 import _native as N
 
         g = torch.Generator(device="cuda").manual_seed(4321 + self.rank)
@@ -406,7 +406,7 @@ def test_broadcast_all_gpus(raw_world):
 
 
 def test_full_size_properties(raw_world):
-    """BASELINE.json's largest message (1 GiB, 2^28 elements) is too big to check element by element
+    """The sweep's largest message (1 GiB, 2^28 elements) is too big to check element by element
     against the CPU oracle in seconds, so it is checked through size-independent properties:
       * int32 SUM wraps modulo 2^32, hence  sum_i result[i] == sum_r sum_i x_r[i]  (mod 2^32)
         -- a checksum of checksums computed on the GPUs in int64;

@@ -45,7 +45,7 @@ def test_load_and_host_side_calls():
     assert [lib.b200c_dtype_size(d) for d in range(10)] == [1, 1, 4, 4, 8, 8, 2, 4, 8, 2]
     assert lib.b200c_dtype_size(99) == 0
     cfg = N.default_config()
-    assert cfg.struct_size == ctypes.sizeof(N.Config) and cfg.staging_bytes == 256 << 20 and cfg.max_blocks == 296
+    assert cfg.struct_size == ctypes.sizeof(N.Config) and cfg.staging_bytes == 256 << 20 and cfg.max_blocks == 264
     assert ctypes.sizeof(N.Export) == 96
     assert lib.b200c_status_string(N.ETIMEOUT).decode() == "timed out waiting for a peer"
 

@@ -127,6 +127,38 @@ def test_epoch_of_a_dead_incarnation_is_ignored(tmp_path):
     assert got == [fresh] and fresh != "stale-epoch"
 
 
+def test_in_process_fetch_takes_the_descriptor_directly():
+    """Ranks in one process (a loopback world) take the offered fd from the serving FdServer (a duplicate), with
+    the socket path's rules: rank in range and not the server's own, each (rank, kind) served once."""
+    server = R.FdServer(world=3, rank=0)
+    r, w = os.pipe()
+    try:
+        server.offer(0, b"x", r)
+        with pytest.raises(OSError):
+            R._fetch_from_peer(server.address.encode(), 5, 0, 2)   # rank out of range
+        with pytest.raises(OSError):
+            R._fetch_from_peer(server.address, 0, 0, 2)            # the server's own rank
+        data, fd = R._fetch_from_peer(server.address.encode(), 1, 0, 5)
+        assert data == b"x" and fd != r
+        os.write(w, b"dup")
+        assert os.read(fd, 10) == b"dup"
+        os.close(fd)
+        with pytest.raises(OSError):
+            R._fetch_from_peer(server.address, 1, 0, 2)            # already served
+        with pytest.raises(R.RendezvousTimeout):
+            server.take(2, 1, 0.05)                                # nothing offered under kind 1
+        data, fd = server.take(2, 0, 5)                            # another rank is still served
+        os.close(fd)
+        assert server.rejected == 0                                # nothing went through the socket
+    finally:
+        server.close()
+        os.close(r)
+        os.close(w)
+    # a closed server is no longer reachable in-process: the socket path is tried (and nobody listens)
+    with pytest.raises(R.RendezvousTimeout):
+        R._fetch_from_peer(server.address, 1, 0, 0.2)
+
+
 def test_fd_server_authenticates_requests():
     """The abstract socket has no file permissions: requests are checked (peer uid, rank in range, pid of
     the published group member, one fd per (rank, kind))."""

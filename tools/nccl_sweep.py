@@ -1,4 +1,4 @@
-"""Stock-NCCL allreduce sweep (baseline B-NCCL, BASELINE.md section 3).
+"""Stock-NCCL allreduce sweep (the NCCL baseline).
 
 Launch: python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/nccl_sweep.py
 The reference drives ncclAllReduce through cupy (nccl_collective_group.py:181-188);

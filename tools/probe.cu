@@ -1,6 +1,6 @@
 // Capability + bandwidth probe for the B200 peer-memory transport.
 // Forks one process per GPU; parent relays messages/fds (star topology).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probe tools/probe.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probe tools/probe.cu -lcuda
 // Run:   tools/probe <ngpus> [isolate]
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -445,7 +445,7 @@ static int child_main(int isolate) {
       }
       if (g_exp) {
         // ---- E1: how many CTAs does NVLS need? (fused ld_reduce+st of the own 1/W slice)
-        for (int g2 : {8, 16, 32, 64, 148, 296}) {
+        for (int g2 : {8, 16, 32, 64, 132, 264}) {
           if (barrier()) return -1;
           CK(cudaEventRecord(e0)); for (int it = 0; it < 5; it++) mc_allreduce_kernel<<<g2, 512>>>((float4*)mcva, g_rank * sl16, sl16);
           CK(cudaEventRecord(e1)); CK(cudaDeviceSynchronize());
@@ -475,7 +475,7 @@ static int child_main(int isolate) {
                                     c.nv ? half16 * 16.0 / ms / 1e6 : 0.0, half16 * 16 >> 20, c.np ? c.np * 16.0 / ms / 1e6 : 0.0);
           }
         }
-        // ---- E3: fence cost with and without a concurrent store stream to the peer (148 CTAs)
+        // ---- E3: fence cost with and without a concurrent store stream to the peer (one CTA per SM)
         {
           long long* d_cyc; CK(cudaMalloc(&d_cyc, 8));
           unsigned* pflag = (unsigned*)((char*)peers[peer].va + (BYTES / 2));   // scratch words inside the landing zone

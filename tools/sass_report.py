@@ -1,6 +1,6 @@
 """Per-kernel registers / stack / local-memory instruction report of libb200coll.so (no GPU needed).
 
-    python tools/sass_report.py > profiles/rNN_sass_local_memory.txt
+    python tools/sass_report.py
 
 Reads `cuobjdump -res-usage` (REG, STACK) and `cuobjdump -sass` (LDL/STL count per function, plus the
 mnemonics that prove the TMA / mbarrier / multimem paths are in the binary) and prints one line per kernel.
@@ -64,7 +64,7 @@ def main():
         tree = run("git", "-C", ROOT, "rev-parse", "--short", "HEAD").strip()
     except Exception:
         tree = "?"
-    print(f"# {os.path.basename(lib)} (sm_100a), tree {tree}: registers, stack bytes (cuobjdump -res-usage) and LDL/STL "
+    print(f"# {os.path.basename(lib)} (sm_90a), tree {tree}: registers, stack bytes (cuobjdump -res-usage) and LDL/STL "
           "instruction count (cuobjdump -sass) per kernel")
     print("# stack 0 = no local memory at all; produced by tools/sass_report.py")
     print()

@@ -38,16 +38,26 @@ _incarnations = {}
 _incarnations_lock = threading.Lock()
 
 
-def native_reduce_op(op) -> int:
+def native_reduce_op(op, is_bool: bool = False) -> int:
+    """ncclRedOp_t for a reduce op.  Bool tensors travel as bytes, so SUM becomes MAX (a logical OR
+    that keeps every byte 0 or 1) and AVG is refused, as torch's NCCL backend does; PROD, MIN and
+    MAX are already logical AND / AND / OR on 0/1 bytes."""
     if isinstance(op, ReduceOp):
-        return _REDUCE_OP_MAP[op]
-    if isinstance(op, DagReduceOp):
-        return op.value
-    # ray's own enums when running inside ray: match by name
-    name = getattr(op, "name", None)
-    if name in ("SUM", "PRODUCT", "MIN", "MAX", "AVG"):
-        return {"SUM": N.SUM, "PRODUCT": N.PROD, "MIN": N.MIN, "MAX": N.MAX, "AVG": N.AVG}[name]
-    raise RuntimeError("B200 backend does not support reduce op: '{}'.".format(op))
+        nat = _REDUCE_OP_MAP[op]
+    elif isinstance(op, DagReduceOp):
+        nat = op.value
+    else:
+        # ray's own enums when running inside ray: match by name
+        name = getattr(op, "name", None)
+        if name not in ("SUM", "PRODUCT", "MIN", "MAX", "AVG"):
+            raise RuntimeError("B200 backend does not support reduce op: '{}'.".format(op))
+        nat = {"SUM": N.SUM, "PRODUCT": N.PROD, "MIN": N.MIN, "MAX": N.MAX, "AVG": N.AVG}[name]
+    if is_bool:
+        if nat == N.AVG:
+            raise RuntimeError("AVG is not defined for bool tensors.")
+        if nat == N.SUM:
+            return N.MAX
+    return nat
 
 
 def _torch_dtype_map():
@@ -68,7 +78,7 @@ _TYPESTR = {"|i1": N.INT8, "|u1": N.UINT8, "<i4": N.INT32, "<u4": N.UINT32, "<i8
 class TensorView:
     """Pointer-level view of a GPU tensor (torch.Tensor or any __cuda_array_interface__ object)."""
 
-    __slots__ = ("ptr", "numel", "dtype", "shape", "device", "itemsize")
+    __slots__ = ("ptr", "numel", "dtype", "shape", "device", "itemsize", "is_bool")
 
     def __init__(self, t):
         global _TORCH_DTYPES
@@ -88,6 +98,7 @@ class TensorView:
             self.ptr = t.data_ptr()
             self.numel = t.numel()
             self.dtype = _TORCH_DTYPES[t.dtype]
+            self.is_bool = t.dtype == torch.bool
             self.shape = list(t.shape)
             self.device = t.device.index
             self.itemsize = t.element_size()
@@ -105,6 +116,7 @@ class TensorView:
                 n *= s
             self.numel = n
             self.dtype = _TYPESTR[cai["typestr"]]
+            self.is_bool = cai["typestr"] == "|b1"
             self.itemsize = int(cai["typestr"][2:])
             dev = getattr(getattr(t, "device", None), "id", None)
             self.device = dev if isinstance(dev, int) else None
@@ -420,7 +432,7 @@ class B200Group:
 
     def allreduce(self, tensors, allreduce_options=AllReduceOptions()):
         v = self._single(tensors)
-        op = native_reduce_op(allreduce_options.reduceOp)
+        op = native_reduce_op(allreduce_options.reduceOp, v.is_bool)
         self.comm(v.device).allreduce(v.ptr, v.ptr, v.numel, v.dtype, op)
 
     def barrier(self, barrier_options=BarrierOptions()):
@@ -430,7 +442,7 @@ class B200Group:
 
     def reduce(self, tensors, reduce_options=ReduceOptions()):
         v = self._single(tensors)
-        op = native_reduce_op(reduce_options.reduceOp)
+        op = native_reduce_op(reduce_options.reduceOp, v.is_bool)
         self.comm(v.device).reduce(v.ptr, v.ptr, v.numel, v.dtype, op, reduce_options.root_rank)
 
     def broadcast(self, tensors, broadcast_options=BroadcastOptions()):
@@ -445,7 +457,7 @@ class B200Group:
     def reducescatter(self, tensors, tensor_lists, reducescatter_options=ReduceScatterOptions()):
         v = self._single(tensors)
         ins = self._list(tensor_lists, v)
-        op = native_reduce_op(reducescatter_options.reduceOp)
+        op = native_reduce_op(reducescatter_options.reduceOp, v.is_bool)
         self.comm(v.device).reducescatter([i.ptr for i in ins], v.ptr, v.numel, v.dtype, op)
 
     def send(self, tensors, send_options=SendOptions()):

@@ -325,17 +325,19 @@ class B200Communicator(Communicator):
         s, r = TensorView(send_buf), TensorView(recv_buf)
         if r.numel != s.numel:
             raise RayChannelError(f"allreduce recv_buf has {r.numel} elements, expected {s.numel}")
+        nat = native_reduce_op(op, s.is_bool)
         self._exec_collective(send_buf, recv_buf, "allreduce",
-                              lambda: self._comm.allreduce(s.ptr, r.ptr, s.numel, s.dtype, native_reduce_op(op)))
+                              lambda: self._comm.allreduce(s.ptr, r.ptr, s.numel, s.dtype, nat))
 
     def reducescatter(self, send_buf, recv_buf, op=ReduceOp.SUM) -> None:
         s, r = TensorView(send_buf), TensorView(recv_buf)
         if s.numel != r.numel * self._world_size:
             raise RayChannelError(f"reducescatter send_buf has {s.numel} elements, expected {r.numel * self._world_size}")
         step = r.numel * r.itemsize
+        nat = native_reduce_op(op, s.is_bool)
         self._exec_collective(send_buf, recv_buf, "reducescatter",
                               lambda: self._comm.reducescatter([s.ptr + j * step for j in range(self._world_size)], r.ptr, r.numel,
-                                                               r.dtype, native_reduce_op(op)))
+                                                               r.dtype, nat))
 
     # -- streams / teardown -------------------------------------------------------------------
     @property

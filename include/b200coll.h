@@ -46,7 +46,19 @@ typedef enum {
 
 /* ncclRedOp_t numbering.  ray.experimental.util.types.ReduceOp passes its .value raw
  * (nccl_group.py:304,325); ray.util.collective.types.ReduceOp goes through
- * NCCL_REDUCE_OP_MAP (nccl_util.py:22-27). */
+ * NCCL_REDUCE_OP_MAP (nccl_util.py:22-27).
+ *
+ * Semantics at the edges (pinned by tests/test_oracle.py and tests/test_gpu_value_edges.py):
+ *  - Ranks are folded in order 0..W-1.  MIN / MAX fold with `acc = a < b ? a : b` /
+ *    `acc = a > b ? a : b` (a = the fold so far, b = the next rank).  That rule decides NaN and
+ *    signed zeros: whenever the comparison is false (a NaN on either side, or +0 against -0) the
+ *    next rank's value is taken, so MAX over ranks [NaN, 1] is 1, over [1, NaN] is NaN, and over
+ *    [+0, -0] is -0.
+ *  - Integer SUM / PROD wrap around (two's complement, modulo 2^bits).  Integer AVG is that
+ *    wrapped sum divided by W with truncation toward zero (ncclAvg).
+ *  - f16 / bf16 accumulate in fp32.  A scaled sum (AVG, b200c_allreduce_scaled) multiplies the
+ *    fp32 accumulator by the scale and rounds once, after the scale, to the element (or wire) type;
+ *    f64 AVG divides in fp64.  A contribution is rounded to the wire type before it is summed. */
 typedef enum {
   B200C_SUM = 0,
   B200C_PROD = 1,

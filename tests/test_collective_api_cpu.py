@@ -186,3 +186,18 @@ def test_backend_names():
     assert Backend("torch_gloo") == Backend.GLOO == Backend("gloo")
     with pytest.raises(ValueError):
         Backend("mpi")
+
+
+def test_bool_reduce_op_mapping():
+    """Bool tensors travel as bytes: SUM maps to MAX (a logical OR that keeps bytes 0/1), AVG is refused,
+    PRODUCT / MIN / MAX (AND / AND / OR on 0/1 bytes) are unchanged; other dtypes keep every op."""
+    from ant_ray_b200 import _native as N
+    from ant_ray_b200.b200_group import native_reduce_op
+    from ant_ray_b200.types import DagReduceOp
+
+    assert native_reduce_op(ReduceOp.SUM, True) == N.MAX
+    assert native_reduce_op(DagReduceOp.SUM, True) == N.MAX
+    assert [native_reduce_op(op, True) for op in (ReduceOp.PRODUCT, ReduceOp.MIN, ReduceOp.MAX)] == [N.PROD, N.MIN, N.MAX]
+    with pytest.raises(RuntimeError):
+        native_reduce_op(DagReduceOp.AVG, True)
+    assert [native_reduce_op(op) for op in DagReduceOp] == [N.SUM, N.PROD, N.MAX, N.MIN, N.AVG]

@@ -54,7 +54,8 @@ def test_allreduce_sum_all_dtypes(world, dtype, algo):
 
 @pytest.mark.parametrize("algo", [N.ALGO_ONESHOT, N.ALGO_TWOSHOT])
 @pytest.mark.parametrize("opname", ["prod", "max", "min", "avg"])
-@pytest.mark.parametrize("dtype", [torch.int32, torch.int64, torch.uint8, torch.float32, torch.bfloat16, torch.float16, torch.float64])
+@pytest.mark.parametrize("dtype", [torch.int32, torch.int64, torch.uint8, torch.float32, torch.bfloat16, torch.float16, torch.float64,
+                                   torch.uint32, torch.uint64])
 def test_allreduce_ops(world, dtype, opname, algo):
     for n in (7, 5000):
         _run_allreduce(world, dtype, n, opname, algo)
@@ -72,7 +73,8 @@ def test_allreduce_ll_all_dtypes(world, dtype):
 
 
 @pytest.mark.parametrize("opname", ["prod", "max", "min", "avg"])
-@pytest.mark.parametrize("dtype", [torch.int32, torch.int64, torch.uint8, torch.float32, torch.bfloat16, torch.float64])
+@pytest.mark.parametrize("dtype", [torch.int32, torch.int64, torch.uint8, torch.float32, torch.bfloat16, torch.float64,
+                                   torch.uint32, torch.uint64])
 def test_allreduce_ll_ops(world, dtype, opname):
     for n in (7, 3001):
         _run_allreduce(world, dtype, n, opname, N.ALGO_LL)
@@ -168,21 +170,23 @@ def test_fused_gradient_mean(world, wire, algo):
         assert torch.allclose(dev[0].cpu(), ref, rtol=tol, atol=tol)
 
 
-@pytest.mark.parametrize("dtype", [torch.int32, torch.float32, torch.bfloat16, torch.uint8])
+@pytest.mark.parametrize("dtype", [torch.int32, torch.float32, torch.bfloat16, torch.uint8, torch.int8, torch.int64, torch.uint32,
+                                   torch.uint64, torch.float16, torch.float64])
 def test_reducescatter(world, dtype):
     W = world.world_size
-    for n in (6, 20_001):
-        lists = [[make_input(dtype, n, r * 16 + j) for j in range(W)] for r in range(W)]
-        dev = [[t.cuda() for t in row] for row in lists]
-        outs = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(W)]
-        world.run(lambda r, c: c.reducescatter([t.data_ptr() for t in dev[r]], outs[r].data_ptr(), n, NATIVE[dtype], N.SUM))
-        torch.cuda.synchronize()
-        world.check()
-        want = O.reducescatter(lists)
-        for r in range(W):
-            assert_equal_bits(outs[r], want[r], f"reducescatter {dtype} n={n} rank={r}")
-            for j in range(W):
-                assert_equal_bits(dev[r][j], lists[r][j], "inputs must be untouched")
+    for opname, (nat, orc) in OPS.items():
+        for n in (6, 20_001):
+            lists = [[make_input(dtype, n, r * 16 + j, opname) for j in range(W)] for r in range(W)]
+            dev = [[t.cuda() for t in row] for row in lists]
+            outs = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(W)]
+            world.run(lambda r, c: c.reducescatter([t.data_ptr() for t in dev[r]], outs[r].data_ptr(), n, NATIVE[dtype], nat))
+            torch.cuda.synchronize()
+            world.check()
+            want = O.reducescatter(lists, orc)
+            for r in range(W):
+                assert_equal_bits(outs[r], want[r], f"reducescatter {dtype} {opname} n={n} rank={r}")
+                for j in range(W):
+                    assert_equal_bits(dev[r][j], lists[r][j], "inputs must be untouched")
 
 
 @pytest.mark.parametrize("dtype", [torch.int64, torch.float16, torch.uint8])
@@ -210,13 +214,16 @@ def test_broadcast_and_reduce(world):
             torch.cuda.synchronize()
             for r in range(W):
                 assert_equal_bits(dev[r], ins[root], f"broadcast root={root} rank={r}")
-            dev = [t.cuda() for t in ins]
-            world.run(lambda r, c: c.reduce(dev[r].data_ptr(), dev[r].data_ptr(), n, N.FLOAT32, N.SUM, root))
-            torch.cuda.synchronize()
-            world.check()
-            want = O.reduce(ins)
-            for r in range(W):
-                assert_equal_bits(dev[r], want if r == root else ins[r], f"reduce root={root} rank={r}")
+            for dtype in INT_DTYPES + FLOAT_DTYPES:
+                for opname, (nat, orc) in OPS.items():
+                    ins = [make_input(dtype, n, r, opname) for r in range(W)]
+                    dev = [t.cuda() for t in ins]
+                    world.run(lambda r, c: c.reduce(dev[r].data_ptr(), dev[r].data_ptr(), n, NATIVE[dtype], nat, root))
+                    torch.cuda.synchronize()
+                    world.check()
+                    want = O.reduce(ins, orc)
+                    for r in range(W):
+                        assert_equal_bits(dev[r], want if r == root else ins[r], f"reduce {dtype} {opname} n={n} root={root} rank={r}")
 
 
 def test_send_recv(world):

@@ -501,3 +501,107 @@ def test_rdt_transport_loopback():
             os.environ["B200COLL_MULTICAST"] = prev
         for name in names:
             col._group_mgr.destroy_collective_group(name)
+
+
+def _bool_cases(W, n):
+    """All-True, all-False and mixed bool tensors, one per rank."""
+    g = torch.Generator().manual_seed(21)
+    return {"all_true": [torch.ones(n, dtype=torch.bool) for _ in range(W)],
+            "all_false": [torch.zeros(n, dtype=torch.bool) for _ in range(W)],
+            "mixed": [torch.rand(n, generator=g) < 0.5 for _ in range(W)]}
+
+
+def _bool_want(ins, opname):
+    """Logical OR for SUM / MAX, AND for PRODUCT / MIN, as the bytes 0 and 1."""
+    st = torch.stack([t.to(torch.uint8) for t in ins])
+    return st.max(0).values if opname in ("SUM", "MAX") else st.min(0).values
+
+
+def test_bool_reductions_stay_boolean(pair):
+    """Bool tensors travel as bytes: SUM must not leave bytes 2..W in a torch.bool tensor, and AVG is refused
+    (torch's NCCL backend does the same), through B200Communicator and through B200Group."""
+    from ant_ray_b200.b200_group import B200Group, make_config
+    from ant_ray_b200.loopback import _MemStore
+    from ant_ray_b200.types import AllReduceOptions, DagReduceOp, ReduceOptions, ReduceScatterOptions
+
+    W, n = 3, 1000
+    e = pair(W)
+    for case, ins in _bool_cases(W, n).items():
+        dev = [t.cuda() for t in ins]
+        for opname in ("SUM", "PRODUCT", "MIN", "MAX"):
+            op = getattr(DagReduceOp, opname)
+            want = _bool_want(ins, opname)
+            outs = [torch.empty(n, dtype=torch.bool, device="cuda") for _ in range(W)]
+            e.run(lambda r: e.comms[r].allreduce(dev[r], outs[r], op))
+            for r in range(W):
+                assert torch.equal(outs[r].cpu().view(torch.uint8), want), f"communicator allreduce {case} {opname} rank={r}"
+            flat = [torch.cat([ins[r]] * W).cuda() for r in range(W)]   # rank r contributes ins[r] to every slot
+            outs = [torch.empty(n, dtype=torch.bool, device="cuda") for _ in range(W)]
+            e.run(lambda r: e.comms[r].reducescatter(flat[r], outs[r], op))
+            for r in range(W):
+                assert torch.equal(outs[r].cpu().view(torch.uint8), want), f"communicator reducescatter {case} {opname} rank={r}"
+    x = torch.ones(n, dtype=torch.bool, device="cuda")
+    with pytest.raises(RuntimeError):
+        e.comms[0].allreduce(x, torch.empty_like(x), DagReduceOp.AVG)
+    with pytest.raises(RuntimeError):
+        e.comms[0].reducescatter(torch.cat([x] * W), x, DagReduceOp.AVG)
+
+    store = _MemStore()
+    prev = os.environ.get("B200COLL_MULTICAST")
+    os.environ["B200COLL_MULTICAST"] = "0"
+    groups = [B200Group(W, r, "bool-lb", store=store, device=0, config=make_config(max_blocks=64, staging_bytes=4 << 20, timeout_ms=15000))
+              for r in range(W)]
+    streams = [torch.cuda.Stream() for _ in range(W)]
+
+    def run(fn):
+        errs = []
+
+        def body(r):
+            try:
+                torch.cuda.set_device(0)
+                with torch.cuda.stream(streams[r]):
+                    fn(r)
+                    streams[r].synchronize()
+            except BaseException as ex:  # noqa: BLE001
+                errs.append(ex)
+
+        ts = [threading.Thread(target=body, args=(r,)) for r in range(W)]
+        [t.start() for t in ts]
+        [t.join(60) for t in ts]
+        assert not any(t.is_alive() for t in ts), "a rank thread is stuck"
+        assert not errs, errs
+
+    try:
+        for case, ins in _bool_cases(W, n).items():
+            for opname in ("SUM", "PRODUCT", "MIN", "MAX"):
+                want = _bool_want(ins, opname)
+                ar, rd, rs = AllReduceOptions(), ReduceOptions(), ReduceScatterOptions()
+                ar.reduceOp = rd.reduceOp = rs.reduceOp = getattr(DagReduceOp, opname)
+                rd.root_rank = W - 1
+                dev = [t.cuda() for t in ins]
+                run(lambda r: groups[r].allreduce([dev[r]], ar))
+                for r in range(W):
+                    assert torch.equal(dev[r].cpu().view(torch.uint8), want), f"group allreduce {case} {opname} rank={r}"
+                dev = [t.cuda() for t in ins]
+                run(lambda r: groups[r].reduce([dev[r]], rd))
+                assert torch.equal(dev[W - 1].cpu().view(torch.uint8), want), f"group reduce {case} {opname}"
+                for r in range(W - 1):
+                    assert torch.equal(dev[r].cpu(), ins[r]), "non-root ranks keep their input"
+                lists = [[ins[r].cuda() for _ in range(W)] for r in range(W)]
+                outs = [torch.empty(n, dtype=torch.bool, device="cuda") for _ in range(W)]
+                run(lambda r: groups[r].reducescatter([outs[r]], [lists[r]], rs))
+                for r in range(W):
+                    assert torch.equal(outs[r].cpu().view(torch.uint8), want), f"group reducescatter {case} {opname} rank={r}"
+        avg = AllReduceOptions()
+        avg.reduceOp = DagReduceOp.AVG
+        with pytest.raises(RuntimeError):
+            groups[0].allreduce([torch.ones(n, dtype=torch.bool, device="cuda")], avg)
+        for g in groups:
+            g.check(synchronize=True)
+    finally:
+        if prev is None:
+            os.environ.pop("B200COLL_MULTICAST", None)
+        else:
+            os.environ["B200COLL_MULTICAST"] = prev
+        for g in groups:
+            g.destroy_group()

@@ -10,13 +10,17 @@
     differ from gloo in association order only, so they are held to the north-star tolerance
     (1e-5 relative in fp32; half types one rounding step).
 (c) The oracle's half-precision conversions against torch's.
+(d) The oracle at value edges (tests/gpu_common.py::make_edge_inputs: NaN, +-Inf, +-0, subnormals,
+    overflow, rounding ties, integer wrap-around and high words) against a restatement written here:
+    Python integers modulo 2^bits, and for floats a rank-order fold with torch CPU ops in fp32 (fp64
+    for f64) whose MIN / MAX spell out the `a > b ? a : b` rule.
 """
 import os
 
 import pytest
 import torch
 
-from gpu_common import make_input
+from gpu_common import FLOAT_DTYPES, INT_DTYPES, _from_bits, _int_range, assert_same_values, bits_of, make_edge_inputs, make_input
 
 from oracle import oracle as O
 
@@ -159,3 +163,101 @@ def test_integer_wraparound_and_avg():
     assert O.allreduce([a, b], O.PROD).tolist() == [127, -128, 16]
     assert O.allreduce([torch.tensor([7, -7], dtype=torch.int32)] * 3, O.AVG).tolist() == [7, -7]
     assert O.allreduce([torch.tensor([1.0]), torch.tensor([2.0]), torch.tensor([4.0])], O.AVG).item() == pytest.approx(7 / 3, rel=1e-6)
+
+
+# ---- (d) value edges ------------------------------------------------------------------------------
+EDGE_N = 2 * 31 + 2 * 31 * 31 + 101   # the fixed blocks of the longest pattern (f32, 31 values) and a random tail
+
+
+def _ints_of(t):
+    bits, lo, _ = _int_range(t.dtype)
+    return [(v - lo) % 2 ** bits + lo for v in bits_of(t).tolist()]
+
+
+def _restate_int(ins, op):
+    bits, lo, _ = _int_range(ins[0].dtype)
+    cols = list(zip(*[_ints_of(t) for t in ins]))
+    wrap = lambda v: (v - lo) % 2 ** bits + lo  # noqa: E731
+    out = []
+    for col in cols:
+        acc = col[0]
+        for x in col[1:]:
+            if op in (O.SUM, O.AVG):
+                acc = wrap(acc + x)
+            elif op == O.PROD:
+                acc = wrap(acc * x)
+            elif op == O.MAX:
+                acc = acc if acc > x else x
+            else:
+                acc = acc if acc < x else x
+        if op == O.AVG:  # the wrapped sum, divided with truncation toward zero
+            acc = abs(acc) // len(cols[0]) * (1 if acc >= 0 else -1)
+        out.append(acc)
+    return _from_bits(out, ins[0].dtype)
+
+
+def _restate_float(ins, op, wire=None, scale=None):
+    dt = ins[0].dtype
+    acc_t = torch.float64 if dt == torch.float64 else torch.float32
+    xs = [t.to(acc_t) if wire is None else t.to(wire).to(acc_t) for t in ins]
+    acc = xs[0]
+    for x in xs[1:]:
+        if op in (O.SUM, O.AVG):
+            acc = acc + x
+        elif op == O.PROD:
+            acc = acc * x
+        elif op == O.MAX:
+            acc = torch.where(acc > x, acc, x)
+        else:
+            acc = torch.where(acc < x, acc, x)
+    if op == O.AVG and dt == torch.float64:
+        acc = acc / len(ins)
+    elif op == O.AVG or scale is not None:
+        acc = acc * torch.tensor(1.0 / len(ins) if scale is None else scale, dtype=torch.float32)
+    if wire is not None:
+        acc = acc.to(wire).to(acc_t)
+    return acc.to(dt)
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 8])
+@pytest.mark.parametrize("dtype", INT_DTYPES + FLOAT_DTYPES, ids=str)
+def test_oracle_at_value_edges(dtype, world):
+    ins = make_edge_inputs(dtype, EDGE_N, world, seed=world)
+    for name, op in (("sum", O.SUM), ("prod", O.PROD), ("max", O.MAX), ("min", O.MIN), ("avg", O.AVG)):
+        want = _restate_int(ins, op) if not dtype.is_floating_point else _restate_float(ins, op)
+        assert_same_values(O.allreduce(ins, op), want, f"{dtype} {name} W={world}")
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 8])
+def test_oracle_fused_mean_at_value_edges(world):
+    """Wire rounding of every contribution, fp32 sum, the scale, then ONE rounding to the wire."""
+    ins = make_edge_inputs(torch.float32, EDGE_N, world, seed=100 + world)
+    for wire in (None, torch.bfloat16, torch.float16):
+        assert_same_values(O.allreduce_scaled(ins, wire, 1.0 / world), _restate_float(ins, O.SUM, wire, 1.0 / world),
+                           f"fused mean wire={wire} W={world}")
+    for dt in (torch.bfloat16, torch.float16):
+        ins = make_edge_inputs(dt, EDGE_N, world, seed=200 + world)
+        assert_same_values(O.allreduce_scaled(ins, None, 1.0 / 3), _restate_float(ins, O.SUM, None, 1.0 / 3), f"{dt} scaled W={world}")
+
+
+def test_oracle_edge_table():
+    """Single cases that decide the documented semantics (include/b200coll.h, b200c_redop_t)."""
+    nan, inf = float("nan"), float("inf")
+    f = lambda *v: torch.tensor(v, dtype=torch.float32)  # noqa: E731
+    assert O.allreduce([f(nan), f(1.0)], O.MAX).item() == 1.0                   # a NaN in the fold is replaced ...
+    assert O.allreduce([f(1.0), f(nan)], O.MAX).isnan().all()                  # ... a NaN at the next rank is taken
+    assert bits_of(O.allreduce([f(0.0), f(-0.0)], O.MAX)).item() == bits_of(f(-0.0)).item()
+    assert bits_of(O.allreduce([f(-0.0), f(0.0)], O.MAX)).item() == 0
+    assert bits_of(O.allreduce([f(-0.0), f(-0.0)])).item() == bits_of(f(-0.0)).item()   # no +0 start value
+    assert O.allreduce([f(inf), f(-inf)]).isnan().all()
+    i32 = lambda *v: torch.tensor(v, dtype=torch.int32)  # noqa: E731
+    assert O.allreduce([i32(2**31 - 1), i32(1)], O.AVG).item() == -(2**30)     # wrapped sum, truncating divide
+    assert O.allreduce([i32(-3), i32(0)], O.AVG).item() == -1
+    # fused mean, f16 wire, W = 2, scale 0.5: the contribution overflows before the scale, the sum does not
+    got = O.allreduce_scaled([f(70000.0, 60000.0, 1e-8, 3e-5), f(0.0, 60000.0, 0.0, 3e-5)], torch.float16, 0.5)
+    assert got[0].item() == inf and got[1].item() == 60000.0 and got[2].item() == 0.0
+    assert got[3].item() == torch.tensor(3e-5).half().float().item()
+    u64 = torch.tensor([-1], dtype=torch.int64).view(torch.uint64)              # 2^64 - 1
+    two = torch.tensor([2], dtype=torch.int64).view(torch.uint64)
+    assert bits_of(O.allreduce([u64, two], O.AVG)).item() == 0                  # (2^64 - 1 + 2) mod 2^64 = 1, / 2 = 0
+    assert bits_of(O.allreduce([u64, u64], O.AVG)).item() == 2**63 - 1         # unsigned: (2^64 - 2) / 2

@@ -96,6 +96,7 @@ SYMBOLS = {
     "b200c_broadcast": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
     "b200c_allgather": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), c_size_t, c_int, c_void_p]),
     "b200c_reducescatter": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_size_t, c_int, c_int, c_void_p]),
+    "b200c_reducescatter_scaled": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_size_t, c_int, c_int, c_float, c_void_p]),
     "b200c_send": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "b200c_recv": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "b200c_send_multi": (c_int, [c_void_p, c_void_p, c_size_t, POINTER(c_int), c_int, c_void_p]),

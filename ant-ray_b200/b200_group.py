@@ -296,6 +296,11 @@ class PeerMemoryComm:
         arr = (ctypes.c_void_p * len(send_ptrs))(*send_ptrs)
         N.check(self.lib.b200c_reducescatter(self._h(), arr, recv_ptr, count, dtype, op, s.cuda_stream))
 
+    def reducescatter_scaled(self, send_ptrs: List[int], recv_ptr, count, dtype, wire_dtype, scale):
+        s = self.stream()
+        arr = (ctypes.c_void_p * len(send_ptrs))(*send_ptrs)
+        N.check(self.lib.b200c_reducescatter_scaled(self._h(), arr, recv_ptr, count, dtype, wire_dtype, scale, s.cuda_stream))
+
     def send(self, ptr, nbytes, peer, stream=None):
         s = self.stream() if stream is None else stream
         N.check(self.lib.b200c_send(self._h(), ptr, nbytes, peer, s.cuda_stream))

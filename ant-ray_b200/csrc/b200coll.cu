@@ -765,6 +765,15 @@ static void launch_mixed(int algo, const CollArgs& a, int grid, cudaStream_t s) 
   }
 }
 template <typename TI, typename TW>
+static void launch_rs_scaled(const CollArgs& a, int grid, cudaStream_t s) {
+  switch (a.c.world) {
+    case 2: k_reducescatter_scaled<TI, TW, 2><<<grid, kThreads, 0, s>>>(a); break;
+    case 4: k_reducescatter_scaled<TI, TW, 4><<<grid, kThreads, 0, s>>>(a); break;
+    case 8: k_reducescatter_scaled<TI, TW, 8><<<grid, kThreads, 0, s>>>(a); break;
+    default: k_reducescatter_scaled<TI, TW, 0><<<grid, kThreads, 0, s>>>(a); break;
+  }
+}
+template <typename TI, typename TW>
 static void launch_nvls(const CollArgs& a, int grid, cudaStream_t s, bool pipe, bool lanes = false) {
   if (lanes) k_allreduce_nvls_lanes<TI, TW><<<grid, kThreads, 0, s>>>(a);
   else if (pipe) k_allreduce_nvls_rounds<TI, TW><<<grid, kThreads, 0, s>>>(a);
@@ -1203,6 +1212,53 @@ extern "C" int b200c_reducescatter(b200c_comm_t* c, const void* const* send_ptrs
     rc = launch_same_type(dtype, KIND_REDUCESCATTER, op, a, grid, s);
     if (rc) return rc;
     rc = launch_check(c, "reducescatter");
+    if (rc) return rc;
+    commit_args(c, a);
+    done += n;
+  }
+  return B200C_OK;
+}
+
+extern "C" int b200c_reducescatter_scaled(b200c_comm_t* c, const void* const* send_ptrs, void* recv, size_t count, int dtype,
+                                          int wire_dtype, float scale, b200c_stream_t stream) {
+  int rc = check_ready(c);
+  if (rc) return rc;
+  if (dtype != B200C_FLOAT32 && dtype != B200C_BFLOAT16 && dtype != B200C_FLOAT16)
+    return fail(B200C_EUNSUPPORTED, "scaled reducescatter supports f32/bf16/f16 buffers, got %d", dtype);
+  const size_t esz = b200c_dtype_size(dtype), wsz = b200c_dtype_size(wire_dtype);
+  if (!wsz) return fail(B200C_EINVAL, "bad wire dtype %d", wire_dtype);
+  if (wire_dtype != dtype && !(dtype == B200C_FLOAT32 && (wire_dtype == B200C_BFLOAT16 || wire_dtype == B200C_FLOAT16)))
+    return fail(B200C_EUNSUPPORTED, "wire dtype %d for buffer dtype %d", wire_dtype, dtype);
+  if (count == 0) return B200C_OK;
+  if (!send_ptrs || !recv) return fail(B200C_EINVAL, "null buffer");
+  for (int j = 0; j < c->world; j++) if (!send_ptrs[j]) return fail(B200C_EINVAL, "send_ptrs[%d] is null", j);
+  cudaStream_t s = (cudaStream_t)stream;
+  // one rank: only the wire rounding and the scale remain, which is the one-rank scaled allreduce
+  if (c->world == 1) return allreduce_impl(c, send_ptrs[0], recv, count, dtype, wire_dtype, B200C_SUM, scale, 1, B200C_ALGO_AUTO, s);
+  DeviceGuard g(c->device);
+  const size_t vec = 16 / wsz;
+  size_t cap = c->cfg.staging_bytes / c->world / wsz / vec * vec;   // pieces are sized in wire bytes
+  size_t done = 0;
+  while (done < count) {
+    size_t n = count - done < cap ? count - done : cap;
+    CollArgs a;
+    base_args(c, &a);
+    for (int j = 0; j < c->world; j++) a.in_ptrs[j] = static_cast<const char*>(send_ptrs[j]) + done * esz;
+    a.out = static_cast<char*>(recv) + done * esz;
+    a.n = n; a.chunk = round_up(n, vec);
+    a.has_scale = 1; a.scale = scale;
+    int grid;
+    plan_tiles(n, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+    // the wire is part of the signature: a peer in a plain reducescatter (or on another wire) is a mismatch
+    a.sig = make_sig(OPC_REDUCESCATTER, dtype, B200C_SUM, n, -1, 16 + wire_dtype);
+    switch (dtype * 16 + wire_dtype) {
+      case B200C_FLOAT32 * 16 + B200C_FLOAT32: launch_rs_scaled<float, float>(a, grid, s); break;
+      case B200C_FLOAT32 * 16 + B200C_BFLOAT16: launch_rs_scaled<float, bf16_t>(a, grid, s); break;
+      case B200C_FLOAT32 * 16 + B200C_FLOAT16: launch_rs_scaled<float, f16_t>(a, grid, s); break;
+      case B200C_BFLOAT16 * 16 + B200C_BFLOAT16: launch_rs_scaled<bf16_t, bf16_t>(a, grid, s); break;
+      default: launch_rs_scaled<f16_t, f16_t>(a, grid, s); break;
+    }
+    rc = launch_check(c, "reducescatter_scaled");
     if (rc) return rc;
     commit_args(c, a);
     done += n;

@@ -278,6 +278,34 @@ __global__ void __launch_bounds__(kThreads, 2) k_reducescatter(const __grid_cons
   }
 }
 
+// Fused gradient mean as a reducescatter (FSDP): phases A+B of two-shot reading in_ptrs[j].  Each contribution
+// travels as TW, the fold accumulates in fp32 in rank order and scales once, the result is stored as TI.
+// At W = 8 with a wire narrower than the buffer the fold also writes the TW result into the rank's own staging
+// slot, which no peer writes in a reducescatter.  That store is not needed for the result; it is the form of the
+// W = 8 fold that sm_90a allocates without a stack under the 64-register budget (tests/test_sass_hygiene.py), like
+// the phase B of two-shot, and costs 2 bytes of local HBM writes per element.  The other world sizes fit without it.
+template <typename TI, typename TW, int WT>
+__global__ void __launch_bounds__(kThreads, 2) k_reducescatter_scaled(const __grid_constant__ CollArgs a) {
+  const DevComm& c = a.c;
+  const int r = c.rank, W = c.world;
+  if (!coll_prologue(a)) return;
+  const size_t slot_bytes = a.chunk * sizeof(TW);
+  B200C_FOR_GRANULES(t0, t1, a, a.n) {
+    for (int k = 1; k < W; k++) {
+      int j = r + k; if (j >= W) j -= W;
+      move_tile<TI, TW, false>(staging_ptr<TW>(c, j, a.seq, (size_t)r * slot_bytes) + t0, static_cast<const TI*>(a.in_ptrs[j]) + t0, t1 - t0);
+    }
+  }
+  block_signal_all(kOffFlagA, a.seq, c);
+  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  check_signature(a);
+  B200C_FOR_GRANULES(t0, t1, a, a.n) {
+    TW* own_slot = WT == 8 && sizeof(TI) > sizeof(TW) ? staging_ptr<TW>(c, r, a.seq, (size_t)r * slot_bytes) + t0 : nullptr;
+    reduce_tile<TI, TW, B200C_SUM, WT>(a, staging_ptr<TW>(c, r, a.seq, 0) + t0, a.chunk, r, static_cast<const TI*>(a.in_ptrs[r]) + t0, own_slot,
+                                       static_cast<TI*>(a.out) + t0, t1 - t0);
+  }
+}
+
 template <typename T, int OP, int WT>
 __global__ void __launch_bounds__(kThreads, 2) k_reduce(const __grid_constant__ CollArgs a) {
   const DevComm& c = a.c;

@@ -14,6 +14,7 @@ Attachment point: `DistributedDataParallel.register_comm_hook(state, hook)` with
 mean.  The kernel is enqueued on a dedicated communication stream so it overlaps the rest of the
 backward pass, like the NCCL stream of the default reducer.
 """
+import logging
 import os
 from typing import Optional
 
@@ -21,6 +22,8 @@ import torch
 
 from . import _native as N
 from .b200_group import PeerMemoryComm, next_comm_key
+
+logger = logging.getLogger(__name__)
 
 _WIRE = {None: None, "fp32": None, "bf16": N.BFLOAT16, "fp16": N.FLOAT16,
          torch.float32: None, torch.bfloat16: N.BFLOAT16, torch.float16: N.FLOAT16}
@@ -50,6 +53,16 @@ class B200GradState:
         out = [(s.elapsed_time(e), n) for s, e, n in self.events]
         self.events = []
         return out
+
+
+def resolve_wire(wire: Optional[str] = None) -> str:
+    """The gradient wire type: `wire`, else B200COLL_GRAD_WIRE (set from B200TorchConfig.grad_wire), else fp32."""
+    wire = wire or os.environ.get("B200COLL_GRAD_WIRE", "fp32")
+    if wire != "fp32":
+        logger.warning("B200 gradient reduction uses a %s wire (fp32 accumulate): gradients are rounded to %s on the "
+                       "way across NVLink, like torch's %s_compress_hook. Use grad_wire='fp32' for the exact "
+                       "default-reducer numerics.", wire, wire, wire)
+    return wire
 
 
 SMALL_BUCKET_BYTES = 1 << 20

@@ -10,9 +10,11 @@ Train when Ray is installed and into any stand-in worker group otherwise (tests,
 
 What changes against the reference: torch.distributed is still initialised (DDP needs a process
 group for its one-off parameter broadcast), but every per-step gradient reduction goes through
-the fused peer-memory kernel registered as DDP's comm hook — NCCL is off the hot path.
+the fused peer-memory kernel registered as DDP's comm hook — NCCL is off the hot path.  With
+parallel_strategy="fsdp" the model is wrapped in FullyShardedDataParallel as in the reference and
+the gradient reduce-scatter runs in a comm hook on the same kernels (fsdp.py); FSDP1's parameter
+all-gathers stay on the process group.
 """
-import logging
 import os
 import socket
 from dataclasses import dataclass
@@ -23,8 +25,6 @@ import torch
 import torch.distributed as dist
 
 from . import ddp_hook
-
-logger = logging.getLogger(__name__)
 
 
 @dataclass
@@ -123,8 +123,8 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     """ray.train.torch.prepare_model with the fused gradient reduction attached.
 
     Same arguments as the reference (v2/torch/train_loop_utils.py:166-248); `grad_wire` overrides
-    the backend config's wire type, `wrap_single` wraps in DDP even at world size 1 (the reference
-    returns the bare model there).  The returned module carries `.b200_grad_state`.
+    the backend config's wire type, `wrap_single` wraps in DDP / FSDP even at world size 1 (the
+    reference returns the bare model there).  The returned module carries `.b200_grad_state`.
     """
     parallel_strategy_kwargs = dict(parallel_strategy_kwargs or {})
     device = move_to_device if isinstance(move_to_device, torch.device) else get_device()
@@ -134,18 +134,24 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
         model = model.to(device)
     world_size = dist.get_world_size() if dist.is_initialized() else 1
     if parallel_strategy and (world_size > 1 or wrap_single):
-        if parallel_strategy != "ddp":
-            raise RuntimeError("The B200 backend accelerates the DDP gradient path; use parallel_strategy='ddp'.")
+        if parallel_strategy not in ("ddp", "fsdp"):
+            raise RuntimeError(f"Unknown parallel_strategy {parallel_strategy!r}: the B200 backend supports 'ddp' and 'fsdp'.")
         if device.type != "cuda":
             raise RuntimeError("The B200 backend needs CUDA devices; there is no CPU fallback.")
-        from torch.nn.parallel import DistributedDataParallel
+        wire = ddp_hook.resolve_wire(grad_wire)
+        if parallel_strategy == "ddp":
+            from torch.nn.parallel import DistributedDataParallel
 
-        kwargs = {"device_ids": [device], "output_device": device, **parallel_strategy_kwargs}
-        model = DistributedDataParallel(model, **kwargs)
-        wire = grad_wire or os.environ.get("B200COLL_GRAD_WIRE", "fp32")
-        if wire not in ("fp32", None):
-            logger.warning("B200 gradient reduction uses a %s wire (fp32 accumulate): gradients are rounded to %s on the "
-                           "way across NVLink, like torch's %s_compress_hook. Use grad_wire='fp32' for the exact "
-                           "default-reducer numerics.", wire, wire, wire)
-        model.b200_grad_state = ddp_hook.register(model, wire=wire)
+            kwargs = {"device_ids": [device], "output_device": device, **parallel_strategy_kwargs}
+            model = DistributedDataParallel(model, **kwargs)
+            model.b200_grad_state = ddp_hook.register(model, wire=wire)
+        else:
+            # the gradient reduce-scatter (or, for NO_SHARD, allreduce) runs in the comm hook; FSDP1 has no seam
+            # for the parameter all-gather, which stays on the torch process group
+            from torch.distributed.fsdp import FullyShardedDataParallel
+
+            from . import fsdp
+
+            model = FullyShardedDataParallel(model, **parallel_strategy_kwargs)
+            model.b200_grad_state = fsdp.register_fsdp1(model, wire=wire)
     return model

@@ -242,6 +242,18 @@ int b200c_allgather(b200c_comm_t* comm, const void* send, void* const* recv_ptrs
 int b200c_reducescatter(b200c_comm_t* comm, const void* const* send_ptrs, void* recv, size_t count,
                         int dtype, int op, b200c_stream_t stream);
 
+/* Fused gradient mean as a reduceScatter (the FSDP gradient reduce-scatter, K13): `send_ptrs[j]`
+ * is this rank's contribution to rank j (`count` elements of `dtype` each).  Every contribution is
+ * rounded to `wire_dtype` and moved as `wire_dtype` (FLOAT32 buffers + BFLOAT16 / FLOAT16 wire, or
+ * wire == dtype), the W contributions are summed in fp32 in rank order, multiplied once by `scale`
+ * (1/world for the mean), rounded to `wire_dtype` and written to `recv` as `dtype`.  Buffers are
+ * f32 / bf16 / f16, anything else is B200C_EUNSUPPORTED.  `recv` may alias send_ptrs[rank].
+ * Pieces are sized by the staging capacity in wire bytes.  The wire is part of the op signature:
+ * a peer that entered b200c_reducescatter (or another wire) instead gets B200C_EMISMATCH.  With one
+ * rank only the wire rounding and the scale are applied. */
+int b200c_reducescatter_scaled(b200c_comm_t* comm, const void* const* send_ptrs, void* recv, size_t count,
+                               int dtype, int wire_dtype, float scale, b200c_stream_t stream);
+
 /* send / recv: nccl_collective_group.py:355-363, 381-389; nccl_group.py:178-184, 217-237.
  * Sender writes the receiver's HBM (ring of slots) and raises a flag; receiver copies out. */
 int b200c_send(b200c_comm_t* comm, const void* buf, size_t bytes, int peer, b200c_stream_t stream);

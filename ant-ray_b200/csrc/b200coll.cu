@@ -16,6 +16,7 @@
 
 #include "byte_kernels.cuh"
 #include "launch_typed.cuh"
+#include "norm_launch.h"
 
 using namespace b200c;
 
@@ -200,6 +201,48 @@ extern "C" size_t b200c_dtype_size(int dtype) {
   }
 }
 extern "C" uint64_t b200c_launch_count(void) { return g_launches.load(); }
+
+// ------------------------------------------------------------------------------------------------
+// fused batch norm (norm_kernels.cuh)
+// ------------------------------------------------------------------------------------------------
+static int check_bn_shape(int m, int c, const void* scratch) {
+  if (m < 1 || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX)
+    return fail(B200C_EINVAL, "batch norm: bad shape m=%d c=%d", m, c);
+  if (!scratch) return fail(B200C_EINVAL, "batch norm: null scratch");
+  return B200C_OK;
+}
+
+extern "C" size_t b200c_bn_scratch_bytes(int channels) {
+  return channels < 1 || channels > bn::kMaxChannels ? 0 : bn::scratch_bytes(channels);
+}
+
+extern "C" int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
+                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
+                                b200c_stream_t stream) {
+  int rc = check_bn_shape(m, channels, scratch);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
+    return fail(B200C_EINVAL, "batch norm forward: null buffer");
+  bn::FwdArgs a{x, identity, y, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
+                save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  RT(bn::forward(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
+                                 const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
+                                 int channels, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn_shape(m, channels, scratch);
+  if (rc) return rc;
+  if (!dy || !y || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias)
+    return fail(B200C_EINVAL, "batch norm backward: null buffer");
+  bn::BwdArgs a{dy, y, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
+  RT(bn::backward(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
 
 extern "C" void b200c_default_config(b200c_config_t* cfg) {
   memset(cfg, 0, sizeof *cfg);

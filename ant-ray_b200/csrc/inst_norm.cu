@@ -1,0 +1,130 @@
+// Launchers of the fused batch-norm kernels (norm_kernels.cuh); argument checking lives in b200coll.cu.
+#include <algorithm>
+
+#include "norm_kernels.cuh"
+#include "norm_launch.h"
+
+namespace b200c {
+namespace bn {
+
+static int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// torch's lastPow2 (ATen/native/cuda/LaunchUtils.h)
+static int last_pow2(unsigned n) {
+  n |= (n >> 1);
+  n |= (n >> 2);
+  n |= (n >> 4);
+  n |= (n >> 8);
+  n |= (n >> 16);
+  return std::max<int>(1, n - (n >> 1));
+}
+
+// torch's flexible_launch_configs with coop_flag = true: the statistics and backward-reduce kernels must run
+// with exactly this block and grid, because the per-channel reduction order follows from them.
+static void reduce_config(int reduction, int stride, dim3* block, dim3* grid) {
+  int block_x = std::min(last_pow2(stride), kTileW);
+  int block_y = std::min(last_pow2(ceil_div(reduction, kElemsPerThread)), kMaxBlock / block_x);
+  if (block_x * block_y != kMaxBlock) block_x = std::min(last_pow2(stride), kMaxBlock / block_y);
+  int grid_y = std::min(ceil_div(reduction, block_y * kElemsPerThread), kMaxHBlock);
+  *block = dim3(block_x, block_y, 1);
+  *grid = dim3(ceil_div(stride, block_x), grid_y < 8 ? 1 : grid_y, 1);
+}
+
+// Elementwise kernels: 8 channels (16 bytes) per thread when the rows allow it, `rows` rows per block, and
+// enough blocks for a few waves on the GPU (each thread then strides over the rows).
+static bool vec_ok(int stride, const void* const* ptrs, int n) {
+  if (stride % kEwVec) return false;
+  for (int i = 0; i < n; i++)
+    if (reinterpret_cast<uintptr_t>(ptrs[i]) % 16) return false;
+  return true;
+}
+
+static void ew_config(int reduction, int stride, int vec, dim3* block, dim3* grid) {
+  const int groups = stride / vec;
+  const int bx = std::min(groups, kEwThreads);
+  const int by = kEwThreads / bx;
+  const int gx = ceil_div(groups, bx);
+  const int gy = std::max(1, std::min(ceil_div(reduction, by), 4096 / gx));
+  *block = dim3(bx, by, 1);
+  *grid = dim3(gx, gy, 1);
+}
+
+// One scratch buffer serves sites of every channel count, so the semaphores sit in a fixed region at its start
+// that no call's staging overlaps: each call finds zeros there and leaves zeros.  For c >= kTileW the reducing
+// kernels' grid.x is at most c / kTileW (block.x >= kTileW), below that it is at most 2.
+constexpr int kSemaphores = kMaxChannels / kTileW;
+constexpr size_t kSemaphoreBytes = (size_t)kSemaphores * 4;
+
+size_t scratch_bytes(int stride) {
+  // semaphores [kSemaphores] ints | staging 3 * stride * kMaxHBlock floats | sum_dy, sum_dy_xmu [stride] floats each
+  return kSemaphoreBytes + (size_t)3 * stride * kMaxHBlock * 4 + (size_t)2 * stride * 4;
+}
+
+struct Scratch {
+  int* semaphores;
+  float* staging;
+  float* sums;
+};
+static Scratch carve(void* scratch, int stride) {
+  char* p = static_cast<char*>(scratch);
+  Scratch s;
+  s.semaphores = reinterpret_cast<int*>(p);
+  s.staging = reinterpret_cast<float*>(p + kSemaphoreBytes);
+  s.sums = s.staging + (size_t)3 * stride * kMaxHBlock;
+  return s;
+}
+
+cudaError_t forward(const FwdArgs& a, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
+             (float)((double)a.m / (double)(a.m - 1)), a.eps};
+  k_bn_stats<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), o, s.staging, s.semaphores, a.m, a.c);
+  const void* ptrs[3] = {a.x, a.y, a.identity ? a.identity : a.x};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const bf16* x = static_cast<const bf16*>(a.x);
+  const bf16* id = static_cast<const bf16*>(a.identity);
+  bf16* y = static_cast<bf16*>(a.y);
+#define B200C_BN_TRANSFORM(V, R) k_bn_transform<V, R><<<grid, block, 0, st>>>(x, id, y, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c)
+  if (vec == kEwVec) {
+    if (id) B200C_BN_TRANSFORM(kEwVec, true); else B200C_BN_TRANSFORM(kEwVec, false);
+  } else {
+    if (id) B200C_BN_TRANSFORM(1, true); else B200C_BN_TRANSFORM(1, false);
+  }
+#undef B200C_BN_TRANSFORM
+  return cudaGetLastError();
+}
+
+cudaError_t backward(const BwdArgs& a, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  float* sum_dy = s.sums;
+  float* sum_dy_xmu = s.sums + a.c;
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const bf16* x = static_cast<const bf16*>(a.x);
+  const bf16* dy = static_cast<const bf16*>(a.dy);
+  const bf16* y = static_cast<const bf16*>(a.y);
+  bf16* masked = static_cast<bf16*>(a.dy_masked);
+  k_bn_bwd_reduce<<<grid, block, 0, st>>>(x, dy, y, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu, a.grad_weight,
+                                          a.grad_bias, s.staging, s.semaphores, a.m, a.c);
+  const void* ptrs[4] = {a.x, a.dy, a.y, a.dx};
+  const void* mptrs[3] = {a.x, a.dy_masked, a.dx};
+  const int vec = (masked ? vec_ok(a.c, mptrs, 3) : vec_ok(a.c, ptrs, 4)) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const float norm_fct = (float)(1.0 / a.m);
+  bf16* dx = static_cast<bf16*>(a.dx);
+#define B200C_BN_ELEMT(V, M, G) \
+  k_bn_bwd_elemt<V, M><<<grid, block, 0, st>>>(G, y, x, dx, a.save_mean, a.save_invstd, a.weight, sum_dy, sum_dy_xmu, norm_fct, a.m, a.c)
+  if (vec == kEwVec) {
+    if (masked) B200C_BN_ELEMT(kEwVec, true, masked); else B200C_BN_ELEMT(kEwVec, false, dy);
+  } else {
+    if (masked) B200C_BN_ELEMT(1, true, masked); else B200C_BN_ELEMT(1, false, dy);
+  }
+#undef B200C_BN_ELEMT
+  return cudaGetLastError();
+}
+
+}  // namespace bn
+}  // namespace b200c

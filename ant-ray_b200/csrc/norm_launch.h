@@ -1,0 +1,48 @@
+// Host-side interface between the C-ABI (b200coll.cu) and the fused batch-norm launchers (inst_norm.cu).
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+
+namespace b200c {
+namespace bn {
+
+struct FwdArgs {
+  const void* x;         // bf16 [m][c]
+  const void* identity;  // bf16 [m][c], or null: no residual add
+  void* y;               // bf16 [m][c]
+  const float* weight;
+  const float* bias;
+  float* running_mean;
+  float* running_var;
+  long long* num_batches_tracked;  // may be null
+  float* save_mean;
+  float* save_invstd;
+  int m, c;
+  float momentum, eps;
+  void* scratch;
+};
+
+struct BwdArgs {
+  const void* dy;        // bf16 [m][c], gradient of the ReLU's output
+  const void* y;         // bf16 [m][c], the ReLU's output
+  const void* x;         // bf16 [m][c], the batch norm's input
+  void* dy_masked;       // bf16 [m][c], or null: receives the ReLU's input gradient (residual site)
+  void* dx;              // bf16 [m][c]
+  const float* weight;
+  const float* save_mean;
+  const float* save_invstd;
+  float* grad_weight;
+  float* grad_bias;
+  int m, c;
+  void* scratch;
+};
+
+// Largest channel count the kernels take: it bounds the semaphore region at the start of every scratch buffer.
+constexpr int kMaxChannels = 1 << 17;
+
+size_t scratch_bytes(int c);
+cudaError_t forward(const FwdArgs& a, cudaStream_t s);   // 2 kernels
+cudaError_t backward(const BwdArgs& a, cudaStream_t s);  // 2 kernels
+
+}  // namespace bn
+}  // namespace b200c

@@ -1,0 +1,180 @@
+"""Fused batch norm for the ResNet training step (libb200coll.so, norm_kernels.cuh).
+
+Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
+by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
+passes: batch norm, ReLU and the residual add forward; threshold_backward and batch norm backward.
+`fuse_resnet` swaps a model's torchvision `ResNet`, `Bottleneck` and `BasicBlock` classes for subclasses whose
+forward runs each such site as one native call per direction, which writes its output once and folds the ReLU
+mask into the backward.  The kernels reproduce torch's own channels-last kernels, reduction order included, so
+outputs, gradients and running statistics are bit-identical to eager torch.
+
+A site runs fused when it is in training mode, its input is a bf16 channels-last CUDA tensor with more than one
+value per channel and at most 131072 channels, its batch norm is
+a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum, and
+torch would run it on its native kernels (`torch._C._select_batch_norm_backend`).  Otherwise the block runs the
+parent class's ops, so the choice never changes a result.
+"""
+import numbers
+
+import torch
+import torch.nn as nn
+from torch.autograd.function import once_differentiable
+
+from . import _native as N
+
+_lib = None
+# (device index, stream) -> (bytes, pointer, zero-initialised uint8 tensor).  One buffer per stream serves every
+# channel count (the library keeps its semaphores in a region no call's staging overlaps); calls on one stream
+# are ordered.
+_scratch = {}
+_scratch_need = {}   # channels -> b200c_bn_scratch_bytes(channels); 0: more channels than the kernels take
+_NATIVE = torch._C._BatchNormBackend.Native
+
+
+def _native_lib():
+    global _lib
+    if _lib is None:
+        _lib = N.load()
+    return _lib
+
+
+def _scratch_bytes(channels):
+    need = _scratch_need.get(channels)
+    if need is None:
+        need = _scratch_need[channels] = int(_native_lib().b200c_bn_scratch_bytes(channels))
+    return need
+
+
+def _scratch_ptr(device, stream, channels):
+    key = (device.index, stream)
+    entry = _scratch.get(key)
+    need = _scratch_need[channels]   # filled by _fusable
+    if entry is None or entry[0] < need:
+        buf = torch.zeros(need, dtype=torch.uint8, device=device)
+        entry = _scratch[key] = (need, buf.data_ptr(), buf)
+    return entry[1]
+
+
+class _FusedBatchNorm(torch.autograd.Function):
+    """relu(bn(x)) or, with `identity`, relu(bn(x) + identity) in training mode."""
+
+    @staticmethod
+    def forward(ctx, x, identity, weight, bias, bn):
+        lib = _native_lib()
+        c = x.shape[1]
+        m = x.numel() // c
+        y = torch.empty_like(x)
+        stats = torch.empty(2, c, dtype=torch.float32, device=x.device)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        nbt = bn.num_batches_tracked
+        N.check(lib.b200c_bn_forward(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
+                                     weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                     nbt.data_ptr() if nbt is not None else None, stats[0].data_ptr(), stats[1].data_ptr(),
+                                     m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, c), stream))
+        ctx.save_for_backward(x, y, weight, stats)
+        ctx.residual = identity is not None
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        lib = _native_lib()
+        x, y, weight, stats = ctx.saved_tensors
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        c = x.shape[1]
+        m = x.numel() // c
+        dx = torch.empty_like(x)
+        d_identity = torch.empty_like(x) if ctx.residual else None
+        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
+        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        N.check(lib.b200c_bn_backward(dy.data_ptr(), y.data_ptr(), x.data_ptr(),
+                                      d_identity.data_ptr() if d_identity is not None else None, dx.data_ptr(),
+                                      weight.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), grad_weight.data_ptr(),
+                                      grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, c), stream))
+        return dx, d_identity, grad_weight, grad_bias, None
+
+
+def _activation(t):
+    return t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last)
+
+
+def _fusable(bn, relu, x):
+    """Whether this site can run fused: the conditions of the module docstring."""
+    if type(bn) is not nn.BatchNorm2d or type(relu) is not nn.ReLU or not bn.training or not bn.track_running_stats:
+        return False
+    w, b, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
+    if w is None or b is None or rm is None or bn._forward_hooks or bn._forward_pre_hooks:
+        return False
+    if not isinstance(bn.momentum, numbers.Real) or not _activation(x) or x.numel() >= 2 ** 31:
+        return False
+    # one value per channel: torch's batch_norm raises ("Expected more than 1 value per channel"), so must we
+    if x.numel() // x.shape[1] <= 1 or not _scratch_bytes(x.shape[1]):
+        return False
+    if any(t.dtype != torch.float32 or not t.is_contiguous() for t in (w, b, rm, rv)):
+        return False
+    return torch._C._select_batch_norm_backend(x, w, b, rm, rv, True, bn.eps) == _NATIVE
+
+
+def bn_relu(bn, relu, x):
+    """relu(bn(x)), fused when the site allows it."""
+    if _fusable(bn, relu, x):
+        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn)
+    return relu(bn(x))
+
+
+def bn_add_relu(bn, relu, x, identity):
+    """`out = bn(x); out += identity; relu(out)`, fused when the site allows it."""
+    if _fusable(bn, relu, x) and _activation(identity) and identity.shape == x.shape:
+        return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn)
+    out = bn(x)
+    out += identity
+    return relu(out)
+
+
+try:
+    from torchvision.models.resnet import BasicBlock, Bottleneck, ResNet
+except ImportError:  # without torchvision there is nothing to rewrite
+    _SWAP = {}
+else:
+
+    class FusedBasicBlock(BasicBlock):
+        def forward(self, x):
+            if not self.training:
+                return super().forward(x)
+            out = bn_relu(self.bn1, self.relu, self.conv1(x))
+            out = self.conv2(out)
+            identity = self.downsample(x) if self.downsample is not None else x
+            return bn_add_relu(self.bn2, self.relu, out, identity)
+
+    class FusedBottleneck(Bottleneck):
+        def forward(self, x):
+            if not self.training:
+                return super().forward(x)
+            out = bn_relu(self.bn1, self.relu, self.conv1(x))
+            out = bn_relu(self.bn2, self.relu, self.conv2(out))
+            out = self.conv3(out)
+            identity = self.downsample(x) if self.downsample is not None else x
+            return bn_add_relu(self.bn3, self.relu, out, identity)
+
+    class FusedResNet(ResNet):
+        def forward(self, x):
+            if not self.training:
+                return super().forward(x)
+            x = bn_relu(self.bn1, self.relu, self.conv1(x))
+            x = self.maxpool(x)
+            x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+            x = torch.flatten(self.avgpool(x), 1)
+            return self.fc(x)
+
+    _SWAP = {ResNet: FusedResNet, Bottleneck: FusedBottleneck, BasicBlock: FusedBasicBlock}
+
+
+def fuse_resnet(model):
+    """Rewrite `model` in place: every module whose class is exactly torchvision's ResNet, Bottleneck or BasicBlock
+    gets the fused subclass.  Parameters, buffers, state_dict keys, hooks and the object itself are unchanged."""
+    for mod in model.modules():
+        cls = _SWAP.get(type(mod))
+        if cls is not None:
+            mod.__class__ = cls
+    return model

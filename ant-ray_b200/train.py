@@ -124,7 +124,8 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
 
     Same arguments as the reference (v2/torch/train_loop_utils.py:166-248); `grad_wire` overrides
     the backend config's wire type, `wrap_single` wraps in DDP / FSDP even at world size 1 (the
-    reference returns the bare model there).  The returned module carries `.b200_grad_state`.
+    reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
+    torchvision ResNet is first rewritten in place by `fused_norm.fuse_resnet`.
     """
     parallel_strategy_kwargs = dict(parallel_strategy_kwargs or {})
     device = move_to_device if isinstance(move_to_device, torch.device) else get_device()
@@ -132,6 +133,11 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
         torch.cuda.set_device(device)
     if move_to_device:
         model = model.to(device)
+    if device.type == "cuda":
+        # batch norm + ReLU (+ residual add) of torchvision ResNets as fused native sites; same bits as eager torch
+        from . import fused_norm
+
+        fused_norm.fuse_resnet(model)
     world_size = dist.get_world_size() if dist.is_initialized() else 1
     if parallel_strategy and (world_size > 1 or wrap_single):
         if parallel_strategy not in ("ddp", "fsdp"):

@@ -281,6 +281,31 @@ int b200c_barrier(b200c_comm_t* comm, b200c_stream_t stream);
  * flag of the next LL op (one LL launch per call).  Never call it on a live group. */
 int b200c_debug_fill_flags(b200c_comm_t* comm, uint32_t value);
 
+/* ---- fused batch norm (training) over channels-last bf16 activations ----
+ * A ResNet block's batch norm and what follows it, in one call per direction: x -> relu(bn(x)), or, with
+ * `identity` set, x -> relu(bn(x) + identity).  Activations are bf16 rows of `channels` values (NHWC memory order,
+ * m = N*H*W rows); weight, bias and the statistics are fp32 [channels].  The results are bit-identical to eager
+ * torch's native channels-last batch norm (its statistics, running-statistics update, transform, backward reduce
+ * and backward elementwise kernels) followed by the bf16 residual add and ReLU, and their backward.
+ * `scratch` holds at least b200c_bn_scratch_bytes(channels) bytes, zero-filled before its first use.  Its
+ * semaphores sit in a fixed region at its start that no call's staging overlaps, and every call leaves them at
+ * zero, so one buffer, sized for the largest channel count, serves calls of any channel count.  Calls sharing a
+ * scratch buffer must be ordered (one stream).  channels <= 131072; b200c_bn_scratch_bytes returns 0 outside
+ * 1..131072.
+ *
+ * Forward: writes y, save_mean, save_invstd (1 / sqrt(biased var + eps)), updates running_mean / running_var
+ * with `momentum` (unbiased variance) and adds 1 to *num_batches_tracked (may be NULL).  2 kernels.
+ * Backward: from dy (the gradient of y), y and x writes dx, grad_weight and grad_bias; `dy_masked` (may be NULL)
+ * receives the gradient of the ReLU's input, the identity branch's gradient.  2 kernels. */
+size_t b200c_bn_scratch_bytes(int channels);
+int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
+                     float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                     float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
+                     b200c_stream_t stream);
+int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
+                      const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
+                      int channels, void* scratch, b200c_stream_t stream);
+
 /* Launch statistics (bench.py's gpu_launches claim). */
 uint64_t b200c_launch_count(void);
 

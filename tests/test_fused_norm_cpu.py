@@ -1,0 +1,54 @@
+"""fused_norm.fuse_resnet rewrites torchvision ResNets in place without changing what they are or compute.
+
+The rewrite keeps the model object, its submodules, parameters and state_dict keys; the rewritten blocks are still
+instances of torchvision's classes.  Inputs that cannot run fused (here: CPU tensors in train and eval mode, fp32,
+NCHW and channels-last) take the parent classes' ops and give the same bits as the untouched model."""
+import copy
+
+import pytest
+import torch
+
+from ant_ray_b200 import fused_norm
+
+torchvision = pytest.importorskip("torchvision")
+from torchvision.models.resnet import BasicBlock, Bottleneck, ResNet  # noqa: E402
+
+
+@pytest.mark.parametrize("arch", ["resnet18", "resnet50"])
+def test_rewrite_keeps_identity_state_and_keys(arch):
+    torch.manual_seed(0)
+    model = getattr(torchvision.models, arch)(weights=None)
+    keys = list(model.state_dict().keys())
+    mods = list(model.modules())
+    params = list(model.parameters())
+    assert fused_norm.fuse_resnet(model) is model
+    assert list(model.state_dict().keys()) == keys
+    assert [id(m) for m in model.modules()] == [id(m) for m in mods]
+    assert all(a is b for a, b in zip(model.parameters(), params)) and len(list(model.parameters())) == len(params)
+    assert type(model) is fused_norm.FusedResNet and isinstance(model, ResNet)
+    blocks = [m for m in model.modules() if isinstance(m, (BasicBlock, Bottleneck))]
+    assert blocks and all(type(m) in (fused_norm.FusedBasicBlock, fused_norm.FusedBottleneck) for m in blocks)
+    assert fused_norm.fuse_resnet(model) is model   # idempotent
+    assert type(model) is fused_norm.FusedResNet
+
+
+@pytest.mark.parametrize("arch", ["resnet18", "resnet50"])
+@pytest.mark.parametrize("mode", ["train", "eval"])
+@pytest.mark.parametrize("fmt", ["nchw", "channels_last"])
+def test_fallback_computes_what_the_parent_classes_compute(arch, mode, fmt):
+    torch.manual_seed(0)
+    ref = getattr(torchvision.models, arch)(weights=None)
+    fused = fused_norm.fuse_resnet(copy.deepcopy(ref))
+    memory_format = torch.channels_last if fmt == "channels_last" else torch.contiguous_format
+    for m in (ref, fused):
+        m.to(memory_format=memory_format).train(mode == "train")
+    x = torch.randn(2, 3, 64, 64, generator=torch.Generator().manual_seed(1)).contiguous(memory_format=memory_format)
+    want, got = ref(x), fused(x)
+    assert torch.equal(got, want)
+    if mode == "train":
+        want.sum().backward()
+        got.sum().backward()
+        for (name, a), b in zip(fused.named_parameters(), ref.parameters()):
+            assert torch.equal(a.grad, b.grad), name
+    for (name, a), b in zip(fused.state_dict().items(), ref.state_dict().values()):
+        assert torch.equal(a, b), name

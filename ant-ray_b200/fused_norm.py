@@ -9,7 +9,7 @@ mask into the backward.  The kernels reproduce torch's own channels-last kernels
 outputs, gradients and running statistics are bit-identical to eager torch.
 
 A site runs fused when it is in training mode, its input is a bf16 channels-last CUDA tensor with more than one
-value per channel and at most 131072 channels, its batch norm is
+value per channel, a channel stride of 1 and at most 131072 channels, its batch norm is
 a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum, and
 torch would run it on its native kernels (`torch._C._select_batch_norm_backend`).  Otherwise the block runs the
 parent class's ops, so the choice never changes a result.
@@ -96,7 +96,10 @@ class _FusedBatchNorm(torch.autograd.Function):
 
 
 def _activation(t):
-    return t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last)
+    # With one channel, NCHW strides also pass the channels-last check, but torch runs its NCHW statistics kernel
+    # unless stride(1) == 1 (batch_norm_choose_impl), so the channel stride must be 1 as well.
+    return (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last)
+            and t.stride(1) == 1)
 
 
 def _fusable(bn, relu, x):

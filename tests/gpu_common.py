@@ -1,4 +1,6 @@
-"""Shared helpers for the GPU parity tests: seeded inputs and dtype tables."""
+"""Shared helpers for the GPU parity tests: seeded inputs, dtype tables and the batch-norm launch shapes."""
+from typing import NamedTuple
+
 import torch
 
 from ant_ray_b200 import _native as N
@@ -23,6 +25,13 @@ def make_input(dtype, n, rank, op="sum"):
     if op == "prod":
         lo, hi = max(info.min, -3), min(info.max, 4)
     return torch.randint(lo, hi, (n,), generator=g, dtype=torch.int64).to(dtype)
+
+
+def same_bits(a, b):
+    """Whether two tensors (or two Nones) have the same dtype, shape and element bits, whatever their layout."""
+    if a is None or b is None:
+        return a is None and b is None
+    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(bits_of(a), bits_of(b))
 
 
 def assert_equal_bits(a: torch.Tensor, b: torch.Tensor, what=""):
@@ -145,6 +154,7 @@ def assert_same_values(a: torch.Tensor, b: torch.Tensor, what=""):
     (x86 and the GPU produce different NaN bits for the same invalid operation)."""
     a, b = a.detach().cpu().contiguous(), b.detach().cpu().contiguous()
     assert a.dtype == b.dtype and a.shape == b.shape, f"{what}: {a.dtype}{tuple(a.shape)} vs {b.dtype}{tuple(b.shape)}"
+    a, b = a.flatten(), b.flatten()   # the first differing element is reported by its flat index
     same = bits_of(a) == bits_of(b)
     if a.dtype.is_floating_point:
         same |= torch.isnan(a) & torch.isnan(b)
@@ -155,3 +165,59 @@ def assert_same_values(a: torch.Tensor, b: torch.Tensor, what=""):
         va, vb = (a[i].item(), b[i].item()) if a.dtype.is_floating_point else ("", "")
         raise AssertionError(f"{what}: {bad.numel()}/{a.numel()} elements differ; first at {i}: "
                              f"{va} (bits {ba:#x}) vs {vb} (bits {bb:#x})")
+
+
+# ---- fused batch norm: launch shapes of the reducing kernels -------------------------------------------
+# torch's MAX_BLOCK_SIZE, ELEMENTS_PER_THREAD, OPTIMAL_TILE_W and MAX_H_BLOCK (norm_kernels.cuh)
+BN_MAX_BLOCK, BN_ELEMS_PER_THREAD, BN_TILE_W, BN_MAX_H_BLOCK = 512, 16, 32, 128
+BN_MAX_CHANNELS = 1 << 17
+BN_SEMAPHORES = BN_MAX_CHANNELS // BN_TILE_W   # the fixed semaphore region at the start of every scratch buffer
+
+
+class BnLaunch(NamedTuple):
+    block_x: int
+    block_y: int
+    grid_x: int
+    grid_y: int   # 1 when the grid merge is collapsed (fewer than 8 rows of blocks)
+
+
+def _last_pow2(n):
+    for s in (1, 2, 4, 8, 16):
+        n |= n >> s
+    return max(1, n - (n >> 1))
+
+
+def bn_launch_config(m, c):
+    """Block and grid of the statistics and backward-reduce kernels for m rows of c channels: reduce_config in
+    inst_norm.cu, which is torch's flexible_launch_configs with coop_flag set.  Each channel's rounding follows
+    from this shape, so it is the map from shapes to the regimes the tests must reach."""
+    block_x = min(_last_pow2(c), BN_TILE_W)
+    block_y = min(_last_pow2(-(-m // BN_ELEMS_PER_THREAD)), BN_MAX_BLOCK // block_x)
+    if block_x * block_y != BN_MAX_BLOCK:
+        block_x = min(_last_pow2(c), BN_MAX_BLOCK // block_y)
+    grid_y = min(-(-m // (block_y * BN_ELEMS_PER_THREAD)), BN_MAX_H_BLOCK)
+    return BnLaunch(block_x, block_y, -(-c // block_x), grid_y if grid_y >= 8 else 1)
+
+
+# (N, C, H, W) -> bn_launch_config(N*H*W, C): one site per launch regime of the reducing kernels.  A partial
+# channel tile is C % block_x != 0 (its threads past C leave the backward reduce early); C % 8 != 0 takes the
+# scalar elementwise kernels.
+BN_REGIME_SHAPES = {
+    (2, 256, 32, 32): BnLaunch(32, 16, 8, 8),          # the smallest merged grid
+    (4, 100, 16, 16): BnLaunch(32, 16, 4, 1),          # 4 rows of blocks collapsed to 1, partial tile
+    (8, 100, 28, 28): BnLaunch(32, 16, 4, 25),         # partial tile with the grid merge
+    (64, 100, 28, 28): BnLaunch(32, 16, 4, 128),
+    (2, 256, 3, 3): BnLaunch(256, 2, 1, 1),            # block.x widened past 32 by a small M
+    (2, 2048, 5, 5): BnLaunch(128, 4, 16, 1),
+    (2, 64, 1, 1): BnLaunch(64, 1, 1, 1),              # M = 2 and M = 3
+    (3, 64, 1, 1): BnLaunch(64, 1, 1, 1),
+    (64, 1, 32, 32): BnLaunch(1, 512, 1, 8),           # C = 1 (with stride(1) == 1: NHWC strides)
+    (64, 3, 32, 32): BnLaunch(2, 256, 2, 16),          # C < 32, not a power of two: partial tiles, merged
+    (64, 7, 32, 32): BnLaunch(4, 128, 2, 32),
+    (64, 17, 32, 32): BnLaunch(16, 32, 2, 128),
+    (64, 8, 32, 32): BnLaunch(8, 64, 1, 64),           # vector elementwise kernels
+    (16, 24, 28, 28): BnLaunch(16, 32, 2, 25),         # vector, partial tile
+    (16, 36, 28, 28): BnLaunch(32, 16, 2, 49),         # scalar elementwise kernels
+    (8, 4104, 8, 8): BnLaunch(32, 16, 129, 1),         # one column past a power of two
+    (2, 131072, 32, 32): BnLaunch(32, 16, 4096, 8),    # the most channels, merged: the last semaphore (512 MiB per tensor)
+}

@@ -52,3 +52,34 @@ def test_fallback_computes_what_the_parent_classes_compute(arch, mode, fmt):
             assert torch.equal(a.grad, b.grad), name
     for (name, a), b in zip(fused.state_dict().items(), ref.state_dict().values()):
         assert torch.equal(a, b), name
+
+
+def test_named_shapes_reach_their_launch_regimes():
+    # The GPU tests run these shapes for the regimes named beside them (gpu_common.BN_REGIME_SHAPES).  A change of
+    # reduce_config or its constants must come with shapes that reach the same regimes.
+    from gpu_common import BN_REGIME_SHAPES, bn_launch_config
+
+    for (n, c, h, w), want in BN_REGIME_SHAPES.items():
+        assert bn_launch_config(n * h * w, c) == want, (n, c, h, w)
+    # the collapsed case has 2..7 rows of blocks before collapsing, and the partial tiles really are partial
+    assert bn_launch_config(4 * 16 * 16, 100).block_y * 16 * 4 == 4 * 16 * 16
+    partial = [(s, cfg) for s, cfg in BN_REGIME_SHAPES.items() if s[1] % cfg.block_x]
+    assert any(cfg.grid_y > 1 for _, cfg in partial) and any(cfg.grid_y == 1 for _, cfg in partial)
+    assert any(cfg.block_x > 32 for cfg in BN_REGIME_SHAPES.values())
+    assert any(s[1] % 8 for s in BN_REGIME_SHAPES) and any(s[1] % 8 == 0 for s in BN_REGIME_SHAPES)
+
+
+def test_merged_grids_fit_the_semaphore_region():
+    # Each column of a merged grid owns one semaphore of the fixed region at the start of the scratch buffer, so no
+    # shape the kernels take may merge over more columns than the region holds.  The largest channel count uses
+    # every semaphore.
+    from gpu_common import BN_MAX_CHANNELS, BN_SEMAPHORES, bn_launch_config
+
+    worst = 0
+    for m in (2, 3, 17, 100, 1000, 2048, 5000, 10 ** 5, 10 ** 6):
+        for c in range(1, min(BN_MAX_CHANNELS, (2 ** 31 - 1) // m) + 1):
+            cfg = bn_launch_config(m, c)
+            assert cfg.block_x * cfg.block_y <= 512 and cfg.grid_y <= 128
+            if cfg.grid_y > 1:
+                worst = max(worst, cfg.grid_x)
+    assert worst == BN_SEMAPHORES == 4096

@@ -4,6 +4,7 @@ import ctypes
 import os
 import re
 import subprocess
+import sys
 
 import pytest
 
@@ -83,3 +84,48 @@ def test_product_never_imports_the_oracle():
                 text = open(os.path.join(dirpath, f)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", text, flags=re.M), f"{f} imports the oracle"
                 assert "liboracle" not in text
+
+
+def test_bn_scratch_bytes_bounds():
+    lib = N.load()
+    assert [lib.b200c_bn_scratch_bytes(c) for c in (-1, 0, 131073, 1 << 30)] == [0, 0, 0, 0]
+    sizes = [lib.b200c_bn_scratch_bytes(c) for c in range(1, 131073)]
+    assert sizes[0] > 0 and all(a <= b for a, b in zip(sizes, sizes[1:]))
+    assert min(sizes) >= 4096 * 4   # the semaphore region comes first in every buffer
+
+
+def test_bn_calls_reject_bad_arguments_before_any_launch():
+    # The calls pass a made-up pointer, which a correct library never dereferences because it rejects each call
+    # first.  They run in a process that sees no CUDA device, so that a library that lost a check fails with a
+    # CUDA error instead of launching kernels on that pointer.
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="", PYTHONPATH=os.pathsep.join([ROOT, os.path.join(ROOT, "tests")]))
+    code = "import test_native_abi as t; t.bn_argument_checks(); print('ok')"
+    out = subprocess.run([sys.executable, "-s", "-c", code], env=env, cwd=ROOT, capture_output=True, text=True)
+    assert out.returncode == 0 and out.stdout.strip() == "ok", out.stdout + out.stderr
+
+
+def bn_argument_checks():
+    lib = N.load()
+    p = ctypes.c_void_p(16)   # never dereferenced: each call is rejected first
+    before = lib.b200c_launch_count()
+
+    def fwd(m=8, c=4, scratch=p, **null):
+        a = {k: None if k in null else p for k in ("x", "id", "y", "w", "b", "rm", "rv", "nbt", "sm", "si")}
+        return lib.b200c_bn_forward(a["x"], a["id"], a["y"], a["w"], a["b"], a["rm"], a["rv"], a["nbt"], a["sm"], a["si"],
+                                    m, c, 0.1, 1e-5, scratch, None)
+
+    def bwd(m=8, c=4, scratch=p, **null):
+        a = {k: None if k in null else p for k in ("dy", "y", "x", "mask", "dx", "w", "sm", "si", "gw", "gb")}
+        return lib.b200c_bn_backward(a["dy"], a["y"], a["x"], a["mask"], a["dx"], a["w"], a["sm"], a["si"], a["gw"], a["gb"],
+                                     m, c, scratch, None)
+
+    for call in (fwd, bwd):
+        for m, c in ((0, 4), (8, 0), (-1, 4), (8, 131073), (2 ** 16, 2 ** 15), (2 ** 14, 2 ** 17)):   # m * c = 2^31 last
+            assert call(m=m, c=c) == N.EINVAL, (call.__name__, m, c)
+        assert call(scratch=None) == N.EINVAL
+    for name in ("x", "y", "w", "b", "rm", "rv", "sm", "si"):
+        assert fwd(**{name: 1}) == N.EINVAL, name
+    for name in ("dy", "y", "x", "dx", "w", "sm", "si", "gw", "gb"):
+        assert bwd(**{name: 1}) == N.EINVAL, name
+    assert "batch norm" in N.last_error()
+    assert lib.b200c_launch_count() == before

@@ -30,8 +30,10 @@ static void reduce_config(int reduction, int stride, dim3* block, dim3* grid) {
   *grid = dim3(ceil_div(stride, block_x), grid_y < 8 ? 1 : grid_y, 1);
 }
 
-// Elementwise kernels: 8 channels (16 bytes) per thread when the rows allow it, `rows` rows per block, and
-// enough blocks for a few waves on the GPU (each thread then strides over the rows).
+// 8 channels (16 bytes) per thread when the rows allow it: C % 8 == 0 and every operand on the 16-byte grid.  The
+// statistics kernel's vector path takes the same condition: C % 8 == 0 also makes its block.x (a power of two, at
+// least 8 when C >= 8) a multiple of kStatsVec, so no group of kStatsVec channels straddles C or a block.
+static_assert(kEwVec % kStatsVec == 0, "vec_ok covers the statistics kernel's vector width");
 static bool vec_ok(int stride, const void* const* ptrs, int n) {
   if (stride % kEwVec) return false;
   for (int i = 0; i < n; i++)
@@ -39,6 +41,8 @@ static bool vec_ok(int stride, const void* const* ptrs, int n) {
   return true;
 }
 
+// Elementwise kernels: `rows` rows per block, and enough blocks for a few waves on the GPU (each thread then
+// strides over the rows).
 static void ew_config(int reduction, int stride, int vec, dim3* block, dim3* grid) {
   const int groups = stride / vec;
   const int bx = std::min(groups, kEwThreads);
@@ -80,11 +84,15 @@ cudaError_t forward(const FwdArgs& a, cudaStream_t st) {
   reduce_config(a.m, a.c, &block, &grid);
   StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
              (float)((double)a.m / (double)(a.m - 1)), a.eps};
-  k_bn_stats<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), o, s.staging, s.semaphores, a.m, a.c);
+  const bf16* x = static_cast<const bf16*>(a.x);
+  if (vec_ok(a.c, &a.x, 1)) {
+    k_bn_stats<kStatsVec><<<grid, dim3(block.x / kStatsVec, block.y), 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
+  } else {
+    k_bn_stats<1><<<grid, block, 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
+  }
   const void* ptrs[3] = {a.x, a.y, a.identity ? a.identity : a.x};
   const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
   ew_config(a.m, a.c, vec, &block, &grid);
-  const bf16* x = static_cast<const bf16*>(a.x);
   const bf16* id = static_cast<const bf16*>(a.identity);
   bf16* y = static_cast<bf16*>(a.y);
 #define B200C_BN_TRANSFORM(V, R) k_bn_transform<V, R><<<grid, block, 0, st>>>(x, id, y, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c)

@@ -6,8 +6,10 @@
 // and its contributors; the kernels originate in NVIDIA Apex).  They keep torch's launch shape, per-thread
 // sequence of rows, block tree and grid merge, and torch's expressions, so that every per-channel sum is rounded
 // exactly as torch rounds it.  That is what makes the outputs bit-identical to eager torch (torch 2.x runs bf16
-// batch norm on these native kernels, not on cuDNN).  The elementwise kernels (transform, backward elementwise)
-// have no cross-element rounding, so they are restructured freely: 16-byte loads of 8 channels per thread.
+// batch norm on these native kernels, not on cuDNN).  Within those constraints the reducing kernels issue all loads
+// of an iteration before using any, and the statistics kernel carries 4 channels per thread.  The elementwise
+// kernels (transform, backward elementwise) have no cross-element rounding, so they are restructured freely: 16-byte
+// loads of 8 channels per thread.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -23,6 +25,9 @@ constexpr int kParallelLoads = 4;
 constexpr int kElemsPerThread = 16;
 constexpr int kTileW = 32;
 constexpr int kMaxHBlock = 128;
+// statistics kernel: channels per hardware thread on its vector path (8-byte loads).  Measured on H100 against 1, 2
+// and 8 (DESIGN.md section 7); the backward reduce is fastest at one channel per thread, so it has no vector path.
+constexpr int kStatsVec = 4;
 // elementwise kernels
 constexpr int kEwThreads = 256;
 constexpr int kEwVec = 8;
@@ -34,33 +39,54 @@ struct alignas(2 * V) BVec {
   bf16 v[V];
 };
 
-// ---- reduction helpers (verbatim from torch) ----
+// ---- reduction helpers (torch's, per channel) ----
+// The statistics kernel runs V adjacent torch threads in one hardware thread: hardware thread (tx, ty) of a block
+// blockDim.x wide holds torch's threads (tx * V + k, ty), k < V, of a block blockDim.x * V wide, i.e. channels
+// c .. c + V - 1.  Every per-channel value is computed by torch's expression in torch's order; V only changes how
+// many channels one instruction stream carries.
+
+// torch's welford_merge_element, with its roundings spelled out.  nvcc contracts `mean_new * count_new + mean *
+// count` into one FMA on either product, and which one depends on the call site: in torch's statistics kernel the
+// merge of a thread's accumulators fuses mean_new * count_new (FUSE_NEW), every other merge fuses mean * count.
+template <bool FUSE_NEW>
 __device__ __forceinline__ void welford_merge_element(int& count, float& mean, float& m2n, const int& count_new,
                                                       const float& mean_new, const float& m2n_new) {
   float factor = float(1.0) / ::max(1, (count + count_new));
   float delta0 = mean - mean_new;
-  mean = (mean_new * count_new + mean * count) * factor;
-  m2n += m2n_new + delta0 * delta0 * count_new * count * factor;
+  const float c = count, c_new = count_new;
+  mean = __fmul_rn(FUSE_NEW ? __fmaf_rn(mean_new, c_new, __fmul_rn(mean, c)) : __fmaf_rn(mean, c, __fmul_rn(mean_new, c_new)),
+                   factor);
+  // m2n += m2n_new + delta0 * delta0 * count_new * count * factor
+  m2n = __fadd_rn(m2n, __fmaf_rn(__fmul_rn(__fmul_rn(__fmul_rn(delta0, delta0), c_new), c), factor, m2n_new));
   count += count_new;
 }
 
-__device__ __forceinline__ void welford_merge_block_vertical(int& count, float& mean, float& m2n, int* shmem_count,
-                                                             float* shmem_mean, float* shmem_m2n) {
-  auto address_base = threadIdx.x + threadIdx.y * blockDim.x;
+// torch's vertical tree over threadIdx.y; shared memory is indexed by torch's thread (tx * V + k, ty)
+template <int V>
+__device__ __forceinline__ void welford_merge_block_vertical(int (&count)[V], float (&mean)[V], float (&m2n)[V],
+                                                             int* shmem_count, float* shmem_mean, float* shmem_m2n) {
+  const int block_x = blockDim.x * V;
+  auto address_base = threadIdx.x * V + threadIdx.y * block_x;
 #pragma unroll
   for (int offset = blockDim.y / 2; offset > 0; offset >>= 1) {
     if (threadIdx.y < offset * 2) {
-      shmem_mean[address_base] = mean;
-      shmem_m2n[address_base] = m2n;
-      shmem_count[address_base] = count;
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        shmem_mean[address_base + k] = mean[k];
+        shmem_m2n[address_base + k] = m2n[k];
+        shmem_count[address_base + k] = count[k];
+      }
     }
     __syncthreads();
     if (threadIdx.y < offset && threadIdx.y + offset < blockDim.y) {
-      auto address = address_base + offset * blockDim.x;
-      auto count_new = shmem_count[address];
-      auto mean_new = shmem_mean[address];
-      auto m2n_new = shmem_m2n[address];
-      welford_merge_element(count, mean, m2n, count_new, mean_new, m2n_new);
+      auto address = address_base + offset * block_x;
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        auto count_new = shmem_count[address + k];
+        auto mean_new = shmem_mean[address + k];
+        auto m2n_new = shmem_m2n[address + k];
+        welford_merge_element<false>(count[k], mean[k], m2n[k], count_new, mean_new, m2n_new);
+      }
     }
   }
 }
@@ -100,24 +126,33 @@ __device__ __forceinline__ void finish_stats(const StatsOut& o, int c, float mea
   const float momentum = o.momentum;
   const float unbiased_var = var * o.bessel;
   o.save_mean[c] = mean;
-  o.running_mean[c] = mean * momentum + (1 - momentum) * o.running_mean[c];
-  o.running_var[c] = unbiased_var * momentum + (1 - momentum) * o.running_var[c];
+  o.running_mean[c] = __fmaf_rn(mean, momentum, __fmul_rn(1 - momentum, o.running_mean[c]));     // mean * momentum + (1 - momentum) * rm
+  o.running_var[c] = __fmaf_rn(unbiased_var, momentum, __fmul_rn(1 - momentum, o.running_var[c]));
   o.save_invstd[c] = rsqrtf(var + o.eps);
 }
 
 // Welford statistics per channel (torch: batch_norm_collect_statistics_channels_last_kernel<Var, ..., 4>), then
 // the running-statistics update and inversion by the thread that owns the channel's final value.  The last block
 // of each column leaves its semaphore at zero for the next call.
-__global__ void k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile float* staging_data, int* semaphores,
-                           const int reduction_size, const int stride) {
+//
+// Each of torch's threads walks rows m_offset + r * inner_loop_stride into PARALLEL_LOADS accumulators, one
+// iteration of PARALLEL_LOADS rows at a time.  Here all rows of an iteration are loaded (V channels in one load)
+// before the first update, so that they are in flight together; torch's kernel waits for each row's value before it
+// loads the next.  The V channels of a thread share each row's validity, hence count[j] and its reciprocal.
+template <int V>
+__global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile float* staging_data,
+                                                            int* semaphores, const int reduction_size, const int stride) {
   constexpr int PARALLEL_LOADS = kParallelLoads;
-  float x_mean[PARALLEL_LOADS];
-  float m_2_n[PARALLEL_LOADS];
+  float x_mean[PARALLEL_LOADS][V];
+  float m_2_n[PARALLEL_LOADS][V];
   int count[PARALLEL_LOADS];
 #pragma unroll
   for (int i = 0; i < PARALLEL_LOADS; i++) {
-    x_mean[i] = 0.f;
-    m_2_n[i] = 0.f;
+#pragma unroll
+    for (int k = 0; k < V; k++) {
+      x_mean[i][k] = 0.f;
+      m_2_n[i][k] = 0.f;
+    }
     count[i] = 0;
   }
   if (o.num_batches_tracked && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0)
@@ -125,59 +160,73 @@ __global__ void k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile 
 
   int inner_loop_stride = blockDim.y * gridDim.y;
   int m_offset = blockIdx.y * blockDim.y + threadIdx.y;
-  int c_offset = blockIdx.x * blockDim.x + threadIdx.x;
+  int c_offset = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   int loop_count = 1 + (reduction_size - 1) / (inner_loop_stride * PARALLEL_LOADS);
-  int address_base = m_offset * stride + c_offset;
-  int address_increment = inner_loop_stride * stride;
+  const bool c_valid = c_offset < stride;
 
   for (int i = 0; i < loop_count; i++) {
-    float x_math[PARALLEL_LOADS];
-    float x_count_inv[PARALLEL_LOADS];
-    float is_valid[PARALLEL_LOADS];
+    // all rows of the iteration are loaded before any update uses one
+    BVec<V> xv[PARALLEL_LOADS];
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
-      if (c_offset < stride && m_offset < reduction_size) {
-        x_math[j] = __bfloat162float(input[address_base]);
+      const int m = m_offset + j * inner_loop_stride;
+      if (c_valid && m < reduction_size) xv[j] = *reinterpret_cast<const BVec<V>*>(input + ((size_t)m * stride + c_offset));
+    }
+#pragma unroll
+    for (int j = 0; j < PARALLEL_LOADS; j++) {
+      float x_math[V];
+      float x_count_inv;
+      float is_valid;
+      if (c_valid && m_offset < reduction_size) {
+#pragma unroll
+        for (int k = 0; k < V; k++) x_math[k] = __bfloat162float(xv[j].v[k]);
         count[j]++;
-        x_count_inv[j] = float(1) / count[j];
-        is_valid[j] = float(1);
+        x_count_inv = float(1) / count[j];
+        is_valid = float(1);
       } else {
-        x_math[j] = float(0);
-        x_count_inv[j] = float(0);
-        is_valid[j] = float(0);
+#pragma unroll
+        for (int k = 0; k < V; k++) x_math[k] = float(0);
+        x_count_inv = float(0);
+        is_valid = float(0);
       }
       m_offset += inner_loop_stride;
-      address_base += address_increment;
-    }
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      float delta0 = x_math[j] - x_mean[j];
-      x_mean[j] += delta0 * x_count_inv[j];
-      float delta1 = x_math[j] - x_mean[j];
-      m_2_n[j] += delta0 * delta1 * is_valid[j];
+      for (int k = 0; k < V; k++) {
+        float delta0 = x_math[k] - x_mean[j][k];
+        x_mean[j][k] = __fmaf_rn(delta0, x_count_inv, x_mean[j][k]);   // x_mean += delta0 * x_count_inv
+        float delta1 = x_math[k] - x_mean[j][k];
+        m_2_n[j][k] = __fmaf_rn(__fmul_rn(delta0, delta1), is_valid, m_2_n[j][k]);   // m_2_n += delta0 * delta1 * is_valid
+      }
     }
   }
+  float mean_th[V], m2_th[V];
+  int count_th[V];
 #pragma unroll
-  for (int j = 1; j < PARALLEL_LOADS; j++) welford_merge_element(count[0], x_mean[0], m_2_n[0], count[j], x_mean[j], m_2_n[j]);
-
-  auto mean_th = x_mean[0];
-  auto m2_th = m_2_n[0];
-  auto count_th = count[0];
+  for (int k = 0; k < V; k++) {
+    count_th[k] = count[0];
+    mean_th[k] = x_mean[0][k];
+    m2_th[k] = m_2_n[0][k];
+#pragma unroll
+    for (int j = 1; j < PARALLEL_LOADS; j++) welford_merge_element<true>(count_th[k], mean_th[k], m2_th[k], count[j], x_mean[j][k], m_2_n[j][k]);
+  }
 
   __shared__ float shmem_mean[kMaxBlock];
   __shared__ float shmem_m2n[kMaxBlock];
   __shared__ int shmem_count[kMaxBlock];
-  welford_merge_block_vertical(count_th, mean_th, m2_th, shmem_count, shmem_mean, shmem_m2n);
+  welford_merge_block_vertical<V>(count_th, mean_th, m2_th, shmem_count, shmem_mean, shmem_m2n);
 
   if (gridDim.y > 1) {
     volatile float* staging_mean = staging_data;
     volatile float* staging_m2n = &staging_data[stride * gridDim.y];
     volatile int* staging_count = reinterpret_cast<volatile int*>(&staging_m2n[stride * gridDim.y]);
-    address_base = c_offset + blockIdx.y * stride;
-    if (threadIdx.y == 0 && c_offset < stride) {
-      staging_mean[address_base] = mean_th;
-      staging_m2n[address_base] = m2_th;
-      staging_count[address_base] = count_th;
+    int address_base = c_offset + blockIdx.y * stride;
+    if (threadIdx.y == 0 && c_valid) {
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        staging_mean[address_base + k] = mean_th[k];
+        staging_m2n[address_base + k] = m2_th[k];
+        staging_count[address_base + k] = count_th[k];
+      }
     }
     __threadfence();
     __syncthreads();
@@ -189,21 +238,31 @@ __global__ void k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile 
     }
     __syncthreads();
     if (is_last_block_done) {
-      count_th = 0;
-      mean_th = float(0.0);
-      m2_th = float(0.0);
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        count_th[k] = 0;
+        mean_th[k] = float(0.0);
+        m2_th[k] = float(0.0);
+      }
       for (int y = threadIdx.y; y < gridDim.y; y += blockDim.y) {
         address_base = c_offset + y * stride;
-        int count_new = c_offset < stride ? staging_count[address_base] : 0;
-        float mean_new = c_offset < stride ? staging_mean[address_base] : float(0.0);
-        float m2n_new = c_offset < stride ? staging_m2n[address_base] : float(0.0);
-        welford_merge_element(count_th, mean_th, m2_th, count_new, mean_new, m2n_new);
+#pragma unroll
+        for (int k = 0; k < V; k++) {
+          int count_new = c_valid ? staging_count[address_base + k] : 0;
+          float mean_new = c_valid ? staging_mean[address_base + k] : float(0.0);
+          float m2n_new = c_valid ? staging_m2n[address_base + k] : float(0.0);
+          welford_merge_element<false>(count_th[k], mean_th[k], m2_th[k], count_new, mean_new, m2n_new);
+        }
       }
-      welford_merge_block_vertical(count_th, mean_th, m2_th, shmem_count, shmem_mean, shmem_m2n);
-      if (threadIdx.y == 0 && c_offset < stride) finish_stats(o, c_offset, mean_th, m2_th, count_th);
+      welford_merge_block_vertical<V>(count_th, mean_th, m2_th, shmem_count, shmem_mean, shmem_m2n);
+      if (threadIdx.y == 0 && c_valid)
+#pragma unroll
+        for (int k = 0; k < V; k++) finish_stats(o, c_offset + k, mean_th[k], m2_th[k], count_th[k]);
     }
   } else {
-    if (blockIdx.y == 0 && threadIdx.y == 0 && c_offset < stride) finish_stats(o, c_offset, mean_th, m2_th, count_th);
+    if (blockIdx.y == 0 && threadIdx.y == 0 && c_valid)
+#pragma unroll
+      for (int k = 0; k < V; k++) finish_stats(o, c_offset + k, mean_th[k], m2_th[k], count_th[k]);
   }
 }
 
@@ -252,7 +311,8 @@ __device__ __forceinline__ bf16 relu_grad(bf16 dy, bf16 y) { return __bfloat162f
 
 // Per-channel sums of g and g * (x - mean) with g = relu_grad(dy, y) (torch:
 // batch_norm_backward_reduce_channels_last_kernel<4>), and dweight / dbias.  With `masked` set (the block tail,
-// where g is also the identity branch's gradient) g is written there as well.
+// where g is also the identity branch's gradient) g is written there as well.  As in k_bn_stats, all rows of an
+// iteration are loaded before the first sum uses one.
 __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output, const bf16* __restrict__ output,
                                 bf16* __restrict__ masked, const float* __restrict__ mean, const float* __restrict__ inv_std,
                                 float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o, float* __restrict__ grad_weight,
@@ -278,14 +338,24 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
   auto factor = inv_std[c_offset];
 
   for (int i = 0; i < loop_count; i++) {
+    bf16 dy_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS];
+#pragma unroll
+    for (int j = 0; j < PARALLEL_LOADS; j++) {
+      if (m_offset + j * inner_loop_stride < reduction_size) {
+        const int a = address_base + j * address_increment;
+        dy_v[j] = grad_output[a];
+        y_v[j] = output[a];
+        x_v[j] = input[a];
+      }
+    }
     float x_input[PARALLEL_LOADS];
     float x_grad_output[PARALLEL_LOADS];
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (c_offset < stride && m_offset < reduction_size) {
-        const bf16 g = relu_grad(grad_output[address_base], output[address_base]);
+        const bf16 g = relu_grad(dy_v[j], y_v[j]);
         if (masked) masked[address_base] = g;
-        x_input[j] = __bfloat162float(input[address_base]);
+        x_input[j] = __bfloat162float(x_v[j]);
         x_grad_output[j] = __bfloat162float(g);
       } else {
         x_input[j] = float(0);
@@ -297,7 +367,7 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       sum_dy[j] += x_grad_output[j];
-      sum_dy_xmu[j] += x_grad_output[j] * (x_input[j] - r_mean);
+      sum_dy_xmu[j] = __fmaf_rn(x_grad_output[j], x_input[j] - r_mean, sum_dy_xmu[j]);   // += g * (x - mean)
     }
   }
 #pragma unroll

@@ -29,10 +29,12 @@ if ROOT not in sys.path:
 # first match wins: convolutions before anything that may share a word with a fused cuDNN kernel name
 FAMILIES = [
     ("hook", r"b200c::k_(local|allreduce)"),
-    ("bn_stats", r"batch_norm_collect_statistics|k_bn_stats"),
+    ("bn_stats", r"k_bn_stats"),                          # ours; torch's kernels (downsample sites, --unfused): *_torch
+    ("bn_stats_torch", r"batch_norm_collect_statistics"),
     ("bn_update_invert", r"batch_norm_update_stats"),
     ("bn_transform", r"batch_norm_transform_input|k_bn_transform"),
-    ("bn_bwd_reduce", r"batch_norm_backward_reduce|k_bn_bwd_reduce"),
+    ("bn_bwd_reduce", r"k_bn_bwd_reduce"),
+    ("bn_bwd_reduce_torch", r"batch_norm_backward_reduce"),
     ("bn_bwd_elemt", r"batch_norm_backward_elemt|k_bn_bwd_elemt"),
     ("conv", r"conv|cudnn|xmma|gemm|nvjet|cutlass|dgrad|wgrad|fprop|implicit_|nhwc|nchw"),
     ("threshold_backward", r"threshold"),
@@ -44,18 +46,20 @@ FAMILIES = [
 # bytes each family's kernels move per element of a batch-norm site, by site kind (relu: BN -> ReLU; tail:
 # BN -> += identity -> ReLU; plain: downsample BN, always torch's kernels)
 TORCH_BYTES = {  # family -> {kind: bytes per element}
-    "bn_stats": {"relu": 2, "tail": 2, "plain": 2},
+    "bn_stats_torch": {"relu": 2, "tail": 2, "plain": 2},
     "bn_transform": {"relu": 4, "tail": 4, "plain": 4},
     "relu": {"relu": 4, "tail": 4},
     "add": {"tail": 6},
     "threshold_backward": {"relu": 6, "tail": 6},
-    "bn_bwd_reduce": {"relu": 4, "tail": 4, "plain": 4},
+    "bn_bwd_reduce_torch": {"relu": 4, "tail": 4, "plain": 4},
     "bn_bwd_elemt": {"relu": 6, "tail": 6, "plain": 6},
 }
 FUSED_BYTES = {
-    "bn_stats": {"relu": 2, "tail": 2, "plain": 2},
+    "bn_stats": {"relu": 2, "tail": 2},
+    "bn_stats_torch": {"plain": 2},
     "bn_transform": {"relu": 4, "tail": 6, "plain": 4},              # tail: x, identity -> y
-    "bn_bwd_reduce": {"relu": 6, "tail": 8, "plain": 4},             # dy, y, x (tail: -> dy')
+    "bn_bwd_reduce": {"relu": 6, "tail": 8},                         # dy, y, x (tail: -> dy')
+    "bn_bwd_reduce_torch": {"plain": 4},
     "bn_bwd_elemt": {"relu": 8, "tail": 6, "plain": 6},              # dy, y, x -> dx (tail: dy', x -> dx)
 }
 

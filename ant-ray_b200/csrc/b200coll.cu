@@ -764,7 +764,7 @@ static uint32_t make_sig(int opcode, int dtype, int op, size_t n, int root, int 
   for (int i = 0; i < 6; i++) { h ^= v[i]; h *= 1099511628211ull; }
   return ((uint32_t)(h ^ (h >> 32)) & 0x7fffffffu) | 1u;  // never 0 and never the 0xFFFFFFFF wildcard
 }
-// The op takes sequence number seq + 1; the counter itself only advances once the launch has succeeded
+// The op takes sequence number seq + 1; the counters only advance once the launch has succeeded
 // (commit_args), so a rejected call (EINVAL / EUNSUPPORTED before any launch) leaves the ranks aligned.
 static void base_args(b200c_comm* c, CollArgs* a) {
   memset(a, 0, sizeof *a);
@@ -772,7 +772,36 @@ static void base_args(b200c_comm* c, CollArgs* a) {
   a->seq = c->seq + 1;
   a->root = -1;
 }
-static void commit_args(b200c_comm* c, const CollArgs& a) { c->seq = a.seq; }
+// the only place where seq, pipe_base (by the op's round count) and ll_seq (LL ops carry the next one) advance
+static void commit_args(b200c_comm* c, const CollArgs& a, uint32_t rounds = 0) {
+  c->seq = a.seq;
+  c->pipe_base += rounds;
+  if (a.ll_seq) c->ll_seq = a.ll_seq;
+}
+// One collective over `total` units (elements, or bytes for the byte kernels), in pieces of at most `cap`.  For
+// each piece, step(a, done, rounds) fills the CollArgs that base_args started (a.n comes in as the piece's extent
+// and may be lowered), sets the round count of a round-pipelined kernel and launches.
+template <typename Step>
+static int run_pieces(b200c_comm* c, size_t total, size_t cap, const char* what, Step&& step) {
+  for (size_t done = 0; done < total;) {
+    CollArgs a;
+    base_args(c, &a);
+    a.n = total - done < cap ? total - done : cap;
+    uint32_t rounds = 0;
+    int rc = step(a, done, rounds);
+    if (rc) return rc;
+    rc = launch_check(c, what);
+    if (rc) return rc;
+    commit_args(c, a, rounds);
+    done += a.n;
+  }
+  return B200C_OK;
+}
+// one rank: the result is the input, copied unless the call is in place
+static int copy_if_distinct(const void* src, void* dst, size_t bytes, cudaStream_t s) {
+  if (src != dst) RT(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+  return B200C_OK;
+}
 static int launch_same_type(int dtype, int kind, int op, const CollArgs& a, int grid, cudaStream_t s) {
   switch (dtype) {
     case B200C_INT8: return launch_i8(kind, op, a, grid, s);
@@ -792,35 +821,48 @@ static int launch_same_type(int dtype, int kind, int op, const CollArgs& a, int 
 enum { OPC_ALLREDUCE = 1, OPC_REDUCE, OPC_BROADCAST, OPC_ALLGATHER, OPC_REDUCESCATTER, OPC_BARRIER };
 constexpr size_t kMinTileBytes = 8192;
 
-// mixed-type (bucket dtype != wire dtype) and NVLS launches live in this TU
-template <typename TI, typename TW, int WT>
-static void launch_mixed_w(int algo, const CollArgs& a, int grid, cudaStream_t s) {
-  if (algo == B200C_ALGO_ONESHOT) k_allreduce_oneshot<TI, TW, B200C_SUM, WT><<<grid, kThreads, 0, s>>>(a);
-  else k_allreduce_twoshot<TI, TW, B200C_SUM, WT><<<grid, kThreads, 0, s>>>(a);
+// The fused-mean family's (buffer dtype, wire dtype) pairs: f32 on an f32, bf16 or f16 wire, and bf16 / f16
+// on their own.  Calls f(Type<TI>{}, Type<TW>{}) for the pair and returns false for any other.
+template <typename T>
+struct Type { using type = T; };
+template <typename F>
+static bool with_scaled_types(int dtype, int wire, F&& f) {
+  switch (dtype * 16 + wire) {
+    case B200C_FLOAT32 * 16 + B200C_FLOAT32: f(Type<float>{}, Type<float>{}); return true;
+    case B200C_FLOAT32 * 16 + B200C_BFLOAT16: f(Type<float>{}, Type<bf16_t>{}); return true;
+    case B200C_FLOAT32 * 16 + B200C_FLOAT16: f(Type<float>{}, Type<f16_t>{}); return true;
+    case B200C_BFLOAT16 * 16 + B200C_BFLOAT16: f(Type<bf16_t>{}, Type<bf16_t>{}); return true;
+    case B200C_FLOAT16 * 16 + B200C_FLOAT16: f(Type<f16_t>{}, Type<f16_t>{}); return true;
+    default: return false;
+  }
 }
+constexpr int kScaledPairs[][2] = {{B200C_FLOAT32, B200C_FLOAT32}, {B200C_FLOAT32, B200C_BFLOAT16}, {B200C_FLOAT32, B200C_FLOAT16},
+                                   {B200C_BFLOAT16, B200C_BFLOAT16}, {B200C_FLOAT16, B200C_FLOAT16}};
+
+// mixed-type (bucket dtype != wire dtype) and NVLS launches live in this TU
 template <typename TI, typename TW>
 static void launch_mixed(int algo, const CollArgs& a, int grid, cudaStream_t s) {
-  switch (a.c.world) {
-    case 2: launch_mixed_w<TI, TW, 2>(algo, a, grid, s); break;
-    case 4: launch_mixed_w<TI, TW, 4>(algo, a, grid, s); break;
-    case 8: launch_mixed_w<TI, TW, 8>(algo, a, grid, s); break;
-    default: launch_mixed_w<TI, TW, 0>(algo, a, grid, s); break;
-  }
+  with_world_t(a.c.world, [&](auto wt) {
+    constexpr int WT = decltype(wt)::value;
+    if (algo == B200C_ALGO_ONESHOT) k_allreduce_oneshot<TI, TW, B200C_SUM, WT><<<grid, kThreads, 0, s>>>(a);
+    else k_allreduce_twoshot<TI, TW, B200C_SUM, WT><<<grid, kThreads, 0, s>>>(a);
+  });
 }
-template <typename TI, typename TW>
-static void launch_rs_scaled(const CollArgs& a, int grid, cudaStream_t s) {
-  switch (a.c.world) {
-    case 2: k_reducescatter_scaled<TI, TW, 2><<<grid, kThreads, 0, s>>>(a); break;
-    case 4: k_reducescatter_scaled<TI, TW, 4><<<grid, kThreads, 0, s>>>(a); break;
-    case 8: k_reducescatter_scaled<TI, TW, 8><<<grid, kThreads, 0, s>>>(a); break;
-    default: k_reducescatter_scaled<TI, TW, 0><<<grid, kThreads, 0, s>>>(a); break;
-  }
+static void launch_rs_scaled(int dtype, int wire, const CollArgs& a, int grid, cudaStream_t s) {
+  with_scaled_types(dtype, wire, [&](auto ti, auto tw) {
+    with_world_t(a.c.world, [&](auto wt) {
+      k_reducescatter_scaled<typename decltype(ti)::type, typename decltype(tw)::type, decltype(wt)::value><<<grid, kThreads, 0, s>>>(a);
+    });
+  });
 }
-template <typename TI, typename TW>
-static void launch_nvls(const CollArgs& a, int grid, cudaStream_t s, bool pipe, bool lanes = false) {
-  if (lanes) k_allreduce_nvls_lanes<TI, TW><<<grid, kThreads, 0, s>>>(a);
-  else if (pipe) k_allreduce_nvls_rounds<TI, TW><<<grid, kThreads, 0, s>>>(a);
-  else k_allreduce_nvls<TI, TW><<<grid, kThreads, 0, s>>>(a);
+static void launch_nvls(int dtype, int wire, const CollArgs& a, int grid, cudaStream_t s, bool pipe, bool lanes = false) {
+  with_scaled_types(dtype, wire, [&](auto ti, auto tw) {
+    using TI = typename decltype(ti)::type;
+    using TW = typename decltype(tw)::type;
+    if (lanes) k_allreduce_nvls_lanes<TI, TW><<<grid, kThreads, 0, s>>>(a);
+    else if (pipe) k_allreduce_nvls_rounds<TI, TW><<<grid, kThreads, 0, s>>>(a);
+    else k_allreduce_nvls<TI, TW><<<grid, kThreads, 0, s>>>(a);
+  });
 }
 template <typename TI, typename TW>
 static int local_scale_grid(b200c_comm* c, size_t bytes) {
@@ -849,12 +891,21 @@ static int local_scale_grid(b200c_comm* c, size_t bytes) {
 // copy-out still reads it).  Region reuse: copy-in(i+R) waits for copy-out(i); every peer finished reducing
 // region i before switch(i) completed (flag B).
 // ------------------------------------------------------------------------------------------------
-template <typename TS, typename TD, bool BYPASS>
-static void launch_stage_copy(const void* src, void* dst, size_t n, int sm_count, cudaStream_t s) {
-  size_t tile = kStageTileBytes / (sizeof(TS) > sizeof(TD) ? sizeof(TS) : sizeof(TD));
-  size_t want = (n + tile - 1) / tile, cap = (size_t)sm_count * 4;
-  int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
-  k_stage_copy<TS, TD, BYPASS><<<grid, kThreads, 0, s>>>(static_cast<const TS*>(src), static_cast<TD*>(dst), n);
+// Copy n elements from the caller's buffer (dtype) into a staging region (wire), or back (OUT, which bypasses
+// L2).  A 2-byte payload on its own wire is a plain copy: the bf16 kernel serves f16 as well.
+template <bool OUT>
+static void launch_stage_copy(int dtype, int wire, const void* src, void* dst, size_t n, int sm_count, cudaStream_t s) {
+  with_scaled_types(dtype, wire, [&](auto ti, auto tw) {
+    constexpr bool plain = sizeof(typename decltype(ti)::type) == 2;
+    using TI = std::conditional_t<plain, bf16_t, typename decltype(ti)::type>;
+    using TW = std::conditional_t<plain, bf16_t, typename decltype(tw)::type>;
+    using TS = std::conditional_t<OUT, TW, TI>;
+    using TD = std::conditional_t<OUT, TI, TW>;
+    size_t tile = kStageTileBytes / (sizeof(TS) > sizeof(TD) ? sizeof(TS) : sizeof(TD));
+    size_t want = (n + tile - 1) / tile, cap = (size_t)sm_count * 4;
+    int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
+    k_stage_copy<TS, TD, OUT><<<grid, kThreads, 0, s>>>(static_cast<const TS*>(src), static_cast<TD*>(dst), n);
+  });
 }
 static int pipeline_setup(b200c_comm* c) {
   if (c->ps_in) return B200C_OK;
@@ -923,11 +974,7 @@ static int allreduce_streams(b200c_comm* c, const void* send, void* recv, size_t
     const char* src = static_cast<const char*>(send) + e0 * esz;
     char* dst = static_cast<char*>(recv) + e0 * esz;
     if (i >= R) RT(cudaStreamWaitEvent(c->ps_in, c->pe_out[reg], 0));   // the region's previous piece has been copied out
-    if (wire == dtype) {
-      if (esz == 4) launch_stage_copy<float, float, false>(src, region, n, c->sm_count, c->ps_in);
-      else launch_stage_copy<bf16_t, bf16_t, false>(src, region, n, c->sm_count, c->ps_in);   // 2-byte payload: a plain copy either way
-    } else if (wire == B200C_BFLOAT16) launch_stage_copy<float, bf16_t, false>(src, region, n, c->sm_count, c->ps_in);
-    else launch_stage_copy<float, f16_t, false>(src, region, n, c->sm_count, c->ps_in);
+    launch_stage_copy<false>(dtype, wire, src, region, n, c->sm_count, c->ps_in);
     rc = launch_check(c, "stage_in");
     if (rc) return rc;
     RT(cudaEventRecord(c->pe_in[reg], c->ps_in));
@@ -943,19 +990,13 @@ static int allreduce_streams(b200c_comm* c, const void* send, void* recv, size_t
     int grid;
     plan_tiles(a.chunk, wsz, vec, cap, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
     a.sig = make_sig(OPC_ALLREDUCE, dtype * 16 + wire, B200C_SUM, n, reg, B200C_ALGO_NVLS_STREAMS * 8 + i % 8);
-    if (wire == B200C_FLOAT32) launch_nvls<float, float>(a, grid, c->ps_nv, false);
-    else if (wire == B200C_BFLOAT16) launch_nvls<bf16_t, bf16_t>(a, grid, c->ps_nv, false);
-    else launch_nvls<f16_t, f16_t>(a, grid, c->ps_nv, false);
+    launch_nvls(wire, wire, a, grid, c->ps_nv, false);
     rc = launch_check(c, "nvls(stream pipeline)");
     if (rc) return rc;
     commit_args(c, a);
     RT(cudaEventRecord(c->pe_nv[reg], c->ps_nv));
     RT(cudaStreamWaitEvent(c->ps_out, c->pe_nv[reg], 0));
-    if (wire == dtype) {
-      if (esz == 4) launch_stage_copy<float, float, true>(region, dst, n, c->sm_count, c->ps_out);
-      else launch_stage_copy<bf16_t, bf16_t, true>(region, dst, n, c->sm_count, c->ps_out);
-    } else if (wire == B200C_BFLOAT16) launch_stage_copy<bf16_t, float, true>(region, dst, n, c->sm_count, c->ps_out);
-    else launch_stage_copy<f16_t, float, true>(region, dst, n, c->sm_count, c->ps_out);
+    launch_stage_copy<true>(dtype, wire, region, dst, n, c->sm_count, c->ps_out);
     rc = launch_check(c, "stage_out");
     if (rc) return rc;
     RT(cudaEventRecord(c->pe_out[reg], c->ps_out));
@@ -964,6 +1005,146 @@ static int allreduce_streams(b200c_comm* c, const void* send, void* recv, size_t
   // close: the caller's stream continues after the last copy-out, and peers only move on after this rank got here
   RT(cudaStreamWaitEvent(user, c->pe_out[last_reg], 0));
   return barrier_op(c, user);
+}
+
+// One rank: no peers, so only the wire rounding and the scale remain.
+static int allreduce_local(b200c_comm* c, const void* send, void* recv, size_t count, int dtype, int wire, float scale, int has_scale,
+                           cudaStream_t s) {
+  const size_t esz = b200c_dtype_size(dtype);
+  if (!has_scale && wire == dtype) return copy_if_distinct(send, recv, count * esz, s);
+  CollArgs a; memset(&a, 0, sizeof a);
+  a.c = c->dev; a.in = send; a.out = recv; a.n = count; a.has_scale = has_scale; a.scale = scale;
+  // Large, 16-byte aligned buffers stream through shared memory with the bulk copy engine (TMA); the
+  // plain LSU kernel takes small buffers, unaligned views and the sub-tile tail.
+  if (count * esz >= (1u << 20) && ((uintptr_t)send & 15) == 0 && ((uintptr_t)recv & 15) == 0 &&
+      (dtype == B200C_FLOAT32 || ((dtype == B200C_BFLOAT16 || dtype == B200C_FLOAT16) && wire == dtype))) {
+    size_t ntiles = count * esz / kTmaTileBytes;
+    size_t tma_elems = ntiles * kTmaTileBytes / esz;
+    if (c->tma_ctas_per_sm == 0) {
+      int nb = 0;
+      for (const auto& p : kScaledPairs)
+        with_scaled_types(p[0], p[1], [](auto ti, auto tw) {
+          cudaFuncSetAttribute(k_local_scale_tma<typename decltype(ti)::type, typename decltype(tw)::type>,
+                               cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
+        });
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_local_scale_tma<float, bf16_t>, kTmaThreads, kTmaSmemBytes) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 1; }
+      c->tma_ctas_per_sm = nb;
+    }
+    // as many CTAs as are resident at once (measured: a smaller "balanced" grid of 384 x 5 tiles is slower, 13.7 vs
+    // 12.9 us per 30 MiB bucket — what counts is how many bulk loads are in flight from the first microsecond)
+    size_t cap = (size_t)c->sm_count * c->tma_ctas_per_sm;
+    int tgrid = (int)(ntiles < cap ? ntiles : cap);
+    with_scaled_types(dtype, wire, [&](auto ti, auto tw) {
+      k_local_scale_tma<typename decltype(ti)::type, typename decltype(tw)::type><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a);
+    });
+    int rc = launch_check(c, "local_scale_tma");
+    if (rc) return rc;
+    if (tma_elems == count) return B200C_OK;
+    a.in = static_cast<const char*>(send) + tma_elems * esz;
+    a.out = static_cast<char*>(recv) + tma_elems * esz;
+    a.n = count - tma_elems;
+  }
+  int grid = local_scale_grid<float, bf16_t>(c, a.n * esz);
+  if (dtype == B200C_FLOAT64) k_local_scale<double, double><<<grid, kThreads, 0, s>>>(a);
+  else if (!with_scaled_types(dtype, wire, [&](auto ti, auto tw) {
+             k_local_scale<typename decltype(ti)::type, typename decltype(tw)::type><<<grid, kThreads, 0, s>>>(a);
+           }))
+    return copy_if_distinct(send, recv, count * esz, s);  // integer AVG over one rank is the identity
+  return launch_check(c, "local_scale");
+}
+
+// AUTO picks per piece, from the bytes left; the NVLS variants are NVLS pieces planned as pipelined or lanes.
+static int choose_algo(b200c_comm* c, int algo, size_t total_bytes, size_t bytes_left, bool ll_ok, bool nvls_ok, bool in_sym,
+                       bool* pipe, bool* lanes) {
+  const int W = c->world;
+  int al = algo;
+  if (al == B200C_ALGO_NVLS_PIPE) { al = B200C_ALGO_NVLS; *pipe = true; }
+  if (al == B200C_ALGO_NVLS_LANES) { al = B200C_ALGO_NVLS; *lanes = true; }
+  if (al == B200C_ALGO_AUTO) {
+    if (ll_ok && total_bytes <= c->cfg.ll_max_bytes) al = B200C_ALGO_LL;
+    else if (bytes_left <= c->cfg.oneshot_max_bytes) al = B200C_ALGO_ONESHOT;
+    else if (nvls_ok && W > 2 && bytes_left >= c->cfg.nvls_min_bytes && (W >= 6 || in_sym)) al = B200C_ALGO_NVLS;  // W = 4: two-shot beats staged NVLS
+    else al = B200C_ALGO_TWOSHOT;
+  }
+  return al;
+}
+
+// The planners below set the piece's extent (a.n, at most `left` elements), chunk, tile and grid.
+static void plan_ll(b200c_comm* c, CollArgs& a, size_t left, size_t esz, size_t vec, int& grid) {
+  size_t n = left;
+  a.chunk = round_up(n, vec);
+  a.tile = vec;
+  a.ll_seq = c->ll_seq + 1;
+  size_t nvec = (n * esz + 15) / 16;
+  size_t nb = (nvec + kLLThreads - 1) / kLLThreads;
+  grid = (int)(nb < 1 ? 1 : (nb > c->cfg.max_blocks ? c->cfg.max_blocks : nb));
+  a.n = n;
+}
+static void plan_oneshot(b200c_comm* c, CollArgs& a, size_t left, size_t wsz, size_t vec, int& grid) {
+  const int W = c->world;
+  size_t cap = c->cfg.staging_bytes / W / wsz / vec * vec;  // elements per slot
+  size_t n = left < cap ? left : cap;
+  a.chunk = round_up(n, vec);
+  plan_tiles(n, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+  a.n = n;
+}
+static void plan_twoshot(b200c_comm* c, CollArgs& a, size_t left, size_t wsz, size_t vec, int& grid) {
+  const int W = c->world;
+  size_t cap_chunk = c->cfg.staging_bytes / W / wsz / vec * vec;
+  size_t cap = cap_chunk * W;
+  size_t n = left < cap ? left : cap;
+  a.chunk = round_up((n + W - 1) / W, vec);
+  plan_tiles(a.chunk, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+  a.n = n;
+}
+// NVLS: zero-copy on a symmetric buffer (`sym`), else staged: plain, round-pipelined (`pipe`) or lanes (`lanes`),
+// the latter two also chosen here for AUTO by size.
+static int plan_nvls(b200c_comm* c, CollArgs& a, size_t left, size_t wsz, size_t vec, bool sym, int algo, bool& pipe, bool& lanes,
+                     int& grid, uint32_t& rounds) {
+  const int W = c->world;
+  // the zero-copy kernel is pure switch traffic (few CTAs are best); the staged kernels also do the local copies
+  const uint32_t nvls_sym_cap = c->cfg.nvls_blocks && c->cfg.nvls_blocks < c->cfg.max_blocks ? c->cfg.nvls_blocks : c->cfg.max_blocks;
+  // symmetric buffers need no staging; pieces of at most 256 MiB keep the peers' TLB reach
+  size_t cap = sym ? ((size_t)256 << 20) / wsz : c->cfg.staging_bytes / wsz / vec * vec;
+  size_t n = left < cap ? left : cap;
+  a.chunk = round_up((n + W - 1) / W, vec);
+  a.symmetric = sym ? 1 : 0;
+  a.sym_off = sym ? (size_t)((const char*)a.in - c->arena[c->rank]) : 0;
+  if (!sym && algo == B200C_ALGO_AUTO && c->cfg.nvls_lanes_min_bytes && left * wsz >= c->cfg.nvls_lanes_min_bytes) lanes = true;
+  if (!sym && !lanes && algo == B200C_ALGO_AUTO && c->cfg.nvls_pipe_min_bytes && n * wsz >= c->cfg.nvls_pipe_min_bytes) pipe = true;
+  if (sym) pipe = lanes = false;  // nothing to overlap: the symmetric path has no staging copies
+  if (lanes) {
+    // the ring is rewritten every three rounds, so the staging capacity does not bound the piece: take it all
+    n = left;
+    a.chunk = round_up((n + W - 1) / W, vec);
+    uint32_t L = c->cfg.nvls_lanes;
+    uint32_t Kc = c->cfg.max_blocks / L - 1;
+    if (Kc > 7) Kc = 7;
+    if (Kc < 1) Kc = 1;
+    // granule: the configured size, smaller for messages that would otherwise give a lane fewer than ~4 rounds
+    size_t tb = c->cfg.lane_granule_bytes, chunk_bytes = a.chunk * wsz;
+    size_t want = chunk_bytes / ((size_t)L * 4) / 8192 * 8192;
+    if (want < 8192) want = 8192;
+    if (tb > want) tb = want;
+    size_t ring = (size_t)L * kLaneSlots * W * tb;
+    while (ring > c->cfg.staging_bytes && tb > 8192) { tb -= 8192; ring = (size_t)L * kLaneSlots * W * tb; }
+    while (ring > c->cfg.staging_bytes && L > 1) { L--; ring = (size_t)L * kLaneSlots * W * tb; }   // a small staging area: fewer lanes
+    if (ring > c->cfg.staging_bytes) return fail(B200C_EINVAL, "staging_bytes too small for the lane kernel's ring (%zu bytes)", ring);
+    a.tile = tb / wsz;
+    a.lane_copy = (int)Kc;
+    size_t ngran = (a.chunk + a.tile - 1) / a.tile;
+    uint32_t used = (uint32_t)(ngran < L ? ngran : L);   // lanes that own at least one granule
+    grid = (int)(used * (1 + Kc));
+    rounds = (uint32_t)((ngran + used - 1) / used);
+    a.pipe_base = c->pipe_base;
+  } else if (pipe) {
+    plan_rounds(a.chunk, wsz, vec, c->cfg.max_blocks, c->cfg.granule_bytes, &a.tile, &grid, &rounds);
+    a.pipe_base = c->pipe_base;
+  } else {
+    plan_tiles(a.chunk, wsz, vec, sym ? nvls_sym_cap : c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+  }
+  a.n = n;
+  return B200C_OK;
 }
 
 static int allreduce_impl(b200c_comm* c, const void* send, void* recv, size_t count, int dtype, int wire, int op, float scale,
@@ -984,70 +1165,13 @@ static int allreduce_impl(b200c_comm* c, const void* send, void* recv, size_t co
   DeviceGuard g(c->device);
   const int W = c->world;
   const size_t vec = 16 / wsz;
-  if (W == 1) {
-    if (send == recv && !has_scale && wire == dtype) return B200C_OK;
-    if (!has_scale && wire == dtype) { RT(cudaMemcpyAsync(recv, send, count * esz, cudaMemcpyDeviceToDevice, s)); return B200C_OK; }
-    CollArgs a; memset(&a, 0, sizeof a);
-    a.c = c->dev; a.in = send; a.out = recv; a.n = count; a.has_scale = has_scale; a.scale = scale;
-    // Large, 16-byte aligned buffers stream through shared memory with the bulk copy engine (TMA); the
-    // plain LSU kernel takes small buffers, unaligned views and the sub-tile tail.
-    static const bool use_tma = [] { const char* e = getenv("B200COLL_LOCAL_SCALE_TMA"); return !e || e[0] != '0'; }();
-    size_t tma_elems = 0;
-    if (use_tma && count * esz >= (1u << 20) && ((uintptr_t)send & 15) == 0 && ((uintptr_t)recv & 15) == 0 &&
-        (dtype == B200C_FLOAT32 || ((dtype == B200C_BFLOAT16 || dtype == B200C_FLOAT16) && wire == dtype))) {
-      size_t ntiles = count * esz / kTmaTileBytes;
-      tma_elems = ntiles * kTmaTileBytes / esz;
-      if (c->tma_ctas_per_sm == 0) {
-        int nb = 0;
-        cudaFuncSetAttribute(k_local_scale_tma<float, bf16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
-        cudaFuncSetAttribute(k_local_scale_tma<float, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
-        cudaFuncSetAttribute(k_local_scale_tma<float, f16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
-        cudaFuncSetAttribute(k_local_scale_tma<bf16_t, bf16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
-        cudaFuncSetAttribute(k_local_scale_tma<f16_t, f16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_local_scale_tma<float, bf16_t>, kTmaThreads, kTmaSmemBytes) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 1; }
-        c->tma_ctas_per_sm = nb;
-      }
-      // as many CTAs as are resident at once (measured: a smaller "balanced" grid of 384 x 5 tiles is slower, 13.7 vs
-      // 12.9 us per 30 MiB bucket — what counts is how many bulk loads are in flight from the first microsecond)
-      size_t cap = (size_t)c->sm_count * c->tma_ctas_per_sm;
-      int tgrid = (int)(ntiles < cap ? ntiles : cap);
-      switch (dtype * 16 + wire) {
-        case B200C_FLOAT32 * 16 + B200C_FLOAT32: k_local_scale_tma<float, float><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a); break;
-        case B200C_FLOAT32 * 16 + B200C_BFLOAT16: k_local_scale_tma<float, bf16_t><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a); break;
-        case B200C_FLOAT32 * 16 + B200C_FLOAT16: k_local_scale_tma<float, f16_t><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a); break;
-        case B200C_BFLOAT16 * 16 + B200C_BFLOAT16: k_local_scale_tma<bf16_t, bf16_t><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a); break;
-        default: k_local_scale_tma<f16_t, f16_t><<<tgrid, kTmaThreads, kTmaSmemBytes, s>>>(a); break;
-      }
-      rc = launch_check(c, "local_scale_tma");
-      if (rc) return rc;
-      if (tma_elems == count) return B200C_OK;
-      a.in = static_cast<const char*>(send) + tma_elems * esz;
-      a.out = static_cast<char*>(recv) + tma_elems * esz;
-      a.n = count - tma_elems;
-    }
-    int grid = local_scale_grid<float, bf16_t>(c, a.n * esz);
-    switch (dtype * 16 + wire) {
-      case B200C_FLOAT32 * 16 + B200C_FLOAT32: k_local_scale<float, float><<<grid, kThreads, 0, s>>>(a); break;
-      case B200C_FLOAT32 * 16 + B200C_BFLOAT16: k_local_scale<float, bf16_t><<<grid, kThreads, 0, s>>>(a); break;
-      case B200C_FLOAT32 * 16 + B200C_FLOAT16: k_local_scale<float, f16_t><<<grid, kThreads, 0, s>>>(a); break;
-      case B200C_BFLOAT16 * 16 + B200C_BFLOAT16: k_local_scale<bf16_t, bf16_t><<<grid, kThreads, 0, s>>>(a); break;
-      case B200C_FLOAT16 * 16 + B200C_FLOAT16: k_local_scale<f16_t, f16_t><<<grid, kThreads, 0, s>>>(a); break;
-      case B200C_FLOAT64 * 16 + B200C_FLOAT64: k_local_scale<double, double><<<grid, kThreads, 0, s>>>(a); break;
-      default:
-        // integer AVG over one rank is the identity
-        if (send != recv) RT(cudaMemcpyAsync(recv, send, count * esz, cudaMemcpyDeviceToDevice, s));
-        return B200C_OK;
-    }
-    return launch_check(c, "local_scale");
-  }
+  if (W == 1) return allreduce_local(c, send, recv, count, dtype, wire, scale, has_scale, s);
 
   const bool nvls_ok = c->mc_arena && (op == B200C_SUM || op == B200C_AVG) &&
                        (wire == B200C_FLOAT32 || wire == B200C_BFLOAT16 || wire == B200C_FLOAT16);
   if ((algo == B200C_ALGO_NVLS || algo == B200C_ALGO_NVLS_PIPE || algo == B200C_ALGO_NVLS_LANES || algo == B200C_ALGO_NVLS_STREAMS) && !nvls_ok) return fail(B200C_EUNSUPPORTED, "NVLS needs a bound multicast object, SUM/AVG and f32/bf16/f16");
   const bool ll_ok = wire == dtype && c->ll_words && count * esz <= c->ll_words * 4;
   if (algo == B200C_ALGO_LL && !ll_ok) return fail(B200C_EUNSUPPORTED, "LL needs wire == dtype and at most %zu bytes (ll_max_bytes)", c->ll_words * 4);
-  // the zero-copy kernel is pure switch traffic (few CTAs are best); the staged kernels also do the local copies
-  const uint32_t nvls_sym_cap = c->cfg.nvls_blocks && c->cfg.nvls_blocks < c->cfg.max_blocks ? c->cfg.nvls_blocks : c->cfg.max_blocks;
   const char* in = static_cast<const char*>(send);
   char* out = static_cast<char*>(recv);
   // in place, same dtype on the wire, inside the symmetric region: eligible for the zero-copy path
@@ -1059,114 +1183,35 @@ static int allreduce_impl(b200c_comm* c, const void* send, void* recv, size_t co
   if (!in_sym && (algo == B200C_ALGO_NVLS_STREAMS ||
                   (algo == B200C_ALGO_AUTO && nvls_ok && W >= 6 && c->cfg.nvls_streams_min_bytes && count * wsz >= c->cfg.nvls_streams_min_bytes)))
     return allreduce_streams(c, send, recv, count, dtype, wire, op, scale, has_scale, s);
-  size_t done = 0;
-  while (done < count) {
-    size_t left = count - done;
-    size_t bytes_left = left * wsz;
-    int al = algo;
+  // each algorithm's planner sizes its own pieces
+  return run_pieces(c, count, count, "allreduce", [&](CollArgs& a, size_t done, uint32_t& rounds) -> int {
+    const size_t left = count - done;
     bool pipe = false, lanes = false;
-    if (al == B200C_ALGO_NVLS_PIPE) { al = B200C_ALGO_NVLS; pipe = true; }
-    if (al == B200C_ALGO_NVLS_LANES) { al = B200C_ALGO_NVLS; lanes = true; }
-    if (al == B200C_ALGO_AUTO) {
-      if (ll_ok && count * esz <= c->cfg.ll_max_bytes) al = B200C_ALGO_LL;
-      else if (bytes_left <= c->cfg.oneshot_max_bytes) al = B200C_ALGO_ONESHOT;
-      else if (nvls_ok && W > 2 && bytes_left >= c->cfg.nvls_min_bytes && (W >= 6 || in_sym)) al = B200C_ALGO_NVLS;  // W = 4: two-shot beats staged NVLS
-      else al = B200C_ALGO_TWOSHOT;
-    }
-    CollArgs a;
-    base_args(c, &a);
+    const int al = choose_algo(c, algo, count * esz, left * wsz, ll_ok, nvls_ok, in_sym, &pipe, &lanes);
     a.in = in + done * esz; a.out = out + done * esz;
     a.has_scale = has_scale; a.scale = scale;
-    size_t n;
-    int grid;
-    uint32_t rounds = 0;
     // symmetric zero-copy NVLS: buffer lives in the symmetric region at the same offset everywhere
     const bool sym = al == B200C_ALGO_NVLS && in_sym;
-    if (al == B200C_ALGO_LL) {
-      n = left;
-      a.chunk = round_up(n, vec);
-      a.tile = vec;
-      a.ll_seq = c->ll_seq + 1;
-      size_t nvec = (n * esz + 15) / 16;
-      size_t nb = (nvec + kLLThreads - 1) / kLLThreads;
-      grid = (int)(nb < 1 ? 1 : (nb > c->cfg.max_blocks ? c->cfg.max_blocks : nb));
-    } else if (al == B200C_ALGO_ONESHOT) {
-      size_t cap = c->cfg.staging_bytes / W / wsz / vec * vec;  // elements per slot
-      n = left < cap ? left : cap;
-      a.chunk = round_up(n, vec);
-      plan_tiles(n, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-    } else if (al == B200C_ALGO_TWOSHOT) {
-      size_t cap_chunk = c->cfg.staging_bytes / W / wsz / vec * vec;
-      size_t cap = cap_chunk * W;
-      n = left < cap ? left : cap;
-      a.chunk = round_up((n + W - 1) / W, vec);
-      plan_tiles(a.chunk, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-    } else {
-      // symmetric buffers need no staging; pieces of at most 256 MiB keep the peers' TLB reach
-      size_t cap = sym ? ((size_t)256 << 20) / wsz : c->cfg.staging_bytes / wsz / vec * vec;
-      n = left < cap ? left : cap;
-      a.chunk = round_up((n + W - 1) / W, vec);
-      a.symmetric = sym ? 1 : 0;
-      a.sym_off = sym ? (size_t)((const char*)a.in - c->arena[c->rank]) : 0;
-      if (!sym && algo == B200C_ALGO_AUTO && c->cfg.nvls_lanes_min_bytes && left * wsz >= c->cfg.nvls_lanes_min_bytes) lanes = true;
-      if (!sym && !lanes && algo == B200C_ALGO_AUTO && c->cfg.nvls_pipe_min_bytes && n * wsz >= c->cfg.nvls_pipe_min_bytes) pipe = true;
-      if (sym) pipe = lanes = false;  // nothing to overlap: the symmetric path has no staging copies
-      if (lanes) {
-        // the ring is rewritten every three rounds, so the staging capacity does not bound the piece: take it all
-        n = left;
-        a.chunk = round_up((n + W - 1) / W, vec);
-        uint32_t L = c->cfg.nvls_lanes;
-        uint32_t Kc = c->cfg.max_blocks / L - 1;
-        if (Kc > 7) Kc = 7;
-        if (Kc < 1) Kc = 1;
-        // granule: the configured size, smaller for messages that would otherwise give a lane fewer than ~4 rounds
-        size_t tb = c->cfg.lane_granule_bytes, chunk_bytes = a.chunk * wsz;
-        size_t want = chunk_bytes / ((size_t)L * 4) / 8192 * 8192;
-        if (want < 8192) want = 8192;
-        if (tb > want) tb = want;
-        size_t ring = (size_t)L * kLaneSlots * W * tb;
-        while (ring > c->cfg.staging_bytes && tb > 8192) { tb -= 8192; ring = (size_t)L * kLaneSlots * W * tb; }
-        while (ring > c->cfg.staging_bytes && L > 1) { L--; ring = (size_t)L * kLaneSlots * W * tb; }   // a small staging area: fewer lanes
-        if (ring > c->cfg.staging_bytes) return fail(B200C_EINVAL, "staging_bytes too small for the lane kernel's ring (%zu bytes)", ring);
-        a.tile = tb / wsz;
-        a.lane_copy = (int)Kc;
-        size_t ngran = (a.chunk + a.tile - 1) / a.tile;
-        uint32_t used = (uint32_t)(ngran < L ? ngran : L);   // lanes that own at least one granule
-        grid = (int)(used * (1 + Kc));
-        rounds = (uint32_t)((ngran + used - 1) / used);
-        a.pipe_base = c->pipe_base;
-      } else if (pipe) {
-        plan_rounds(a.chunk, wsz, vec, c->cfg.max_blocks, c->cfg.granule_bytes, &a.tile, &grid, &rounds);
-        a.pipe_base = c->pipe_base;
-      } else {
-        plan_tiles(a.chunk, wsz, vec, sym ? nvls_sym_cap : c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-      }
+    int grid = 0;  // set by every planner that returns B200C_OK
+    if (al == B200C_ALGO_LL) plan_ll(c, a, left, esz, vec, grid);
+    else if (al == B200C_ALGO_ONESHOT) plan_oneshot(c, a, left, wsz, vec, grid);
+    else if (al == B200C_ALGO_TWOSHOT) plan_twoshot(c, a, left, wsz, vec, grid);
+    else {
+      int rc = plan_nvls(c, a, left, wsz, vec, sym, algo, pipe, lanes, grid, rounds);
+      if (rc) return rc;
     }
-    a.n = n;
     // a symmetric buffer must sit at the same arena offset on every rank: the offset is part of the signature
-    a.sig = make_sig(OPC_ALLREDUCE, dtype * 16 + wire, op, n, sym ? (int)((a.sym_off >> 4) & 0x3fffffff) : -1, al * 8 + (sym ? 1 : 0) + (pipe ? 2 : 0) + (lanes ? 4 : 0));
-    if (al == B200C_ALGO_NVLS) {
-      if (dtype == B200C_FLOAT32 && wire == B200C_FLOAT32) launch_nvls<float, float>(a, grid, s, pipe, lanes);
-      else if (dtype == B200C_BFLOAT16) launch_nvls<bf16_t, bf16_t>(a, grid, s, pipe, lanes);
-      else if (dtype == B200C_FLOAT16) launch_nvls<f16_t, f16_t>(a, grid, s, pipe, lanes);
-      else if (wire == B200C_BFLOAT16) launch_nvls<float, bf16_t>(a, grid, s, pipe, lanes);
-      else launch_nvls<float, f16_t>(a, grid, s, pipe, lanes);
-    } else if (wire != dtype) {
+    a.sig = make_sig(OPC_ALLREDUCE, dtype * 16 + wire, op, a.n, sym ? (int)((a.sym_off >> 4) & 0x3fffffff) : -1, al * 8 + (sym ? 1 : 0) + (pipe ? 2 : 0) + (lanes ? 4 : 0));
+    if (al == B200C_ALGO_NVLS) launch_nvls(dtype, wire, a, grid, s, pipe, lanes);
+    else if (wire != dtype) {
       if (wire == B200C_BFLOAT16) launch_mixed<float, bf16_t>(al, a, grid, s);
       else launch_mixed<float, f16_t>(al, a, grid, s);
     } else {
       int kind = al == B200C_ALGO_LL ? KIND_LL : (al == B200C_ALGO_ONESHOT ? KIND_ONESHOT : KIND_TWOSHOT);
-      rc = launch_same_type(dtype, kind, op, a, grid, s);
-      if (rc) return rc;
+      return launch_same_type(dtype, kind, op, a, grid, s);
     }
-    rc = launch_check(c, "allreduce");
-    if (rc) return rc;
-    commit_args(c, a);
-    c->pipe_base += rounds;
-    if (al == B200C_ALGO_LL) c->ll_seq = a.ll_seq;
-    done += n;
-  }
-  return B200C_OK;
+    return B200C_OK;
+  });
 }
 
 extern "C" int b200c_allreduce(b200c_comm_t* c, const void* send, void* recv, size_t count, int dtype, int op, int algo,
@@ -1194,32 +1239,19 @@ extern "C" int b200c_reduce(b200c_comm_t* c, const void* send, void* recv, size_
   if (!send || (c->rank == root && !recv)) return fail(B200C_EINVAL, "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard g(c->device);
-  if (c->world == 1) {
-    if (send != recv) RT(cudaMemcpyAsync(recv, send, count * esz, cudaMemcpyDeviceToDevice, s));
-    return B200C_OK;
-  }
+  if (c->world == 1) return copy_if_distinct(send, recv, count * esz, s);
   const size_t vec = 16 / esz;
   size_t cap = c->cfg.staging_bytes / c->world / esz / vec * vec;
-  size_t done = 0;
-  while (done < count) {
-    size_t n = count - done < cap ? count - done : cap;
-    CollArgs a;
-    base_args(c, &a);
+  return run_pieces(c, count, cap, "reduce", [&](CollArgs& a, size_t done, uint32_t&) {
     a.in = static_cast<const char*>(send) + done * esz;
     a.out = recv ? static_cast<char*>(recv) + done * esz : nullptr;
-    a.n = n; a.chunk = round_up(n, vec); a.root = root;
+    a.chunk = round_up(a.n, vec); a.root = root;
     if (op == B200C_AVG) { a.has_scale = 1; a.scale = 1.f / c->world; }
     int grid;
-    plan_tiles(n, esz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-    a.sig = make_sig(OPC_REDUCE, dtype, op, n, root, 0);
-    rc = launch_same_type(dtype, KIND_REDUCE, op, a, grid, s);
-    if (rc) return rc;
-    rc = launch_check(c, "reduce");
-    if (rc) return rc;
-    commit_args(c, a);
-    done += n;
-  }
-  return B200C_OK;
+    plan_tiles(a.n, esz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+    a.sig = make_sig(OPC_REDUCE, dtype, op, a.n, root, 0);
+    return launch_same_type(dtype, KIND_REDUCE, op, a, grid, s);
+  });
 }
 
 extern "C" int b200c_reducescatter(b200c_comm_t* c, const void* const* send_ptrs, void* recv, size_t count, int dtype, int op,
@@ -1234,32 +1266,19 @@ extern "C" int b200c_reducescatter(b200c_comm_t* c, const void* const* send_ptrs
   for (int j = 0; j < c->world; j++) if (!send_ptrs[j]) return fail(B200C_EINVAL, "send_ptrs[%d] is null", j);
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard g(c->device);
-  if (c->world == 1) {
-    if (send_ptrs[0] != recv) RT(cudaMemcpyAsync(recv, send_ptrs[0], count * esz, cudaMemcpyDeviceToDevice, s));
-    return B200C_OK;
-  }
+  if (c->world == 1) return copy_if_distinct(send_ptrs[0], recv, count * esz, s);
   const size_t vec = 16 / esz;
   size_t cap = c->cfg.staging_bytes / c->world / esz / vec * vec;
-  size_t done = 0;
-  while (done < count) {
-    size_t n = count - done < cap ? count - done : cap;
-    CollArgs a;
-    base_args(c, &a);
+  return run_pieces(c, count, cap, "reducescatter", [&](CollArgs& a, size_t done, uint32_t&) {
     for (int j = 0; j < c->world; j++) a.in_ptrs[j] = static_cast<const char*>(send_ptrs[j]) + done * esz;
     a.out = static_cast<char*>(recv) + done * esz;
-    a.n = n; a.chunk = round_up(n, vec);
+    a.chunk = round_up(a.n, vec);
     if (op == B200C_AVG) { a.has_scale = 1; a.scale = 1.f / c->world; }
     int grid;
-    plan_tiles(n, esz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-    a.sig = make_sig(OPC_REDUCESCATTER, dtype, op, n, -1, 0);
-    rc = launch_same_type(dtype, KIND_REDUCESCATTER, op, a, grid, s);
-    if (rc) return rc;
-    rc = launch_check(c, "reducescatter");
-    if (rc) return rc;
-    commit_args(c, a);
-    done += n;
-  }
-  return B200C_OK;
+    plan_tiles(a.n, esz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+    a.sig = make_sig(OPC_REDUCESCATTER, dtype, op, a.n, -1, 0);
+    return launch_same_type(dtype, KIND_REDUCESCATTER, op, a, grid, s);
+  });
 }
 
 extern "C" int b200c_reducescatter_scaled(b200c_comm_t* c, const void* const* send_ptrs, void* recv, size_t count, int dtype,
@@ -1281,32 +1300,18 @@ extern "C" int b200c_reducescatter_scaled(b200c_comm_t* c, const void* const* se
   DeviceGuard g(c->device);
   const size_t vec = 16 / wsz;
   size_t cap = c->cfg.staging_bytes / c->world / wsz / vec * vec;   // pieces are sized in wire bytes
-  size_t done = 0;
-  while (done < count) {
-    size_t n = count - done < cap ? count - done : cap;
-    CollArgs a;
-    base_args(c, &a);
+  return run_pieces(c, count, cap, "reducescatter_scaled", [&](CollArgs& a, size_t done, uint32_t&) {
     for (int j = 0; j < c->world; j++) a.in_ptrs[j] = static_cast<const char*>(send_ptrs[j]) + done * esz;
     a.out = static_cast<char*>(recv) + done * esz;
-    a.n = n; a.chunk = round_up(n, vec);
+    a.chunk = round_up(a.n, vec);
     a.has_scale = 1; a.scale = scale;
     int grid;
-    plan_tiles(n, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+    plan_tiles(a.n, wsz, vec, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
     // the wire is part of the signature: a peer in a plain reducescatter (or on another wire) is a mismatch
-    a.sig = make_sig(OPC_REDUCESCATTER, dtype, B200C_SUM, n, -1, 16 + wire_dtype);
-    switch (dtype * 16 + wire_dtype) {
-      case B200C_FLOAT32 * 16 + B200C_FLOAT32: launch_rs_scaled<float, float>(a, grid, s); break;
-      case B200C_FLOAT32 * 16 + B200C_BFLOAT16: launch_rs_scaled<float, bf16_t>(a, grid, s); break;
-      case B200C_FLOAT32 * 16 + B200C_FLOAT16: launch_rs_scaled<float, f16_t>(a, grid, s); break;
-      case B200C_BFLOAT16 * 16 + B200C_BFLOAT16: launch_rs_scaled<bf16_t, bf16_t>(a, grid, s); break;
-      default: launch_rs_scaled<f16_t, f16_t>(a, grid, s); break;
-    }
-    rc = launch_check(c, "reducescatter_scaled");
-    if (rc) return rc;
-    commit_args(c, a);
-    done += n;
-  }
-  return B200C_OK;
+    a.sig = make_sig(OPC_REDUCESCATTER, dtype, B200C_SUM, a.n, -1, 16 + wire_dtype);
+    launch_rs_scaled(dtype, wire_dtype, a, grid, s);
+    return B200C_OK;
+  });
 }
 
 extern "C" int b200c_allgather(b200c_comm_t* c, const void* send, void* const* recv_ptrs, size_t count, int dtype,
@@ -1321,29 +1326,18 @@ extern "C" int b200c_allgather(b200c_comm_t* c, const void* send, void* const* r
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard g(c->device);
   size_t bytes = count * esz;
-  if (c->world == 1) {
-    if (send != recv_ptrs[0]) RT(cudaMemcpyAsync(recv_ptrs[0], send, bytes, cudaMemcpyDeviceToDevice, s));
-    return B200C_OK;
-  }
+  if (c->world == 1) return copy_if_distinct(send, recv_ptrs[0], bytes, s);
   size_t cap = c->cfg.staging_bytes / c->world / 16 * 16;
-  size_t done = 0;
-  while (done < bytes) {
-    size_t n = bytes - done < cap ? bytes - done : cap;
-    CollArgs a;
-    base_args(c, &a);
+  return run_pieces(c, bytes, cap, "allgather", [&](CollArgs& a, size_t done, uint32_t&) {
     a.in = static_cast<const char*>(send) + done;
     for (int j = 0; j < c->world; j++) a.out_ptrs[j] = static_cast<char*>(recv_ptrs[j]) + done;
-    a.n = n; a.chunk = round_up(n, 16);
+    a.chunk = round_up(a.n, 16);
     int grid;
-    plan_tiles(n, 1, 16, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
-    a.sig = make_sig(OPC_ALLGATHER, dtype, 0, n, -1, 0);
+    plan_tiles(a.n, 1, 16, c->cfg.max_blocks, kMinTileBytes, c->cfg.granule_bytes, &a.tile, &grid);
+    a.sig = make_sig(OPC_ALLGATHER, dtype, 0, a.n, -1, 0);
     k_allgather<<<grid, kThreads, 0, s>>>(a);
-    rc = launch_check(c, "allgather");
-    if (rc) return rc;
-    commit_args(c, a);
-    done += n;
-  }
-  return B200C_OK;
+    return B200C_OK;
+  });
 }
 
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {
@@ -1357,15 +1351,11 @@ extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dty
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard g(c->device);
   const int W = c->world;
-  size_t bytes = count * esz, cap = c->cfg.staging_bytes / 16 * 16, done = 0;
-  while (done < bytes) {
-    size_t n = bytes - done < cap ? bytes - done : cap;
-    CollArgs a;
-    base_args(c, &a);
+  return run_pieces(c, count * esz, c->cfg.staging_bytes / 16 * 16, "broadcast", [&](CollArgs& a, size_t done, uint32_t& rounds) -> int {
+    const size_t n = a.n;
     a.in = static_cast<char*>(buf) + done; a.out = static_cast<char*>(buf) + done;
-    a.n = n; a.root = root;
+    a.root = root;
     int grid;
-    uint32_t rounds = 0;
     // every rank takes the same decision from (n, world, multicast)
     const bool mc = c->mc_arena && c->bcast_mc;
     const bool big = c->cfg.bcast_rounds_min_bytes && n >= c->cfg.bcast_rounds_min_bytes;
@@ -1392,13 +1382,8 @@ extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dty
     a.sig = make_sig(OPC_BROADCAST, dtype, 0, n, root, a.symmetric);
     if (rounds_mode) k_broadcast_rounds<<<grid, kThreads, 0, s>>>(a);
     else k_broadcast<<<grid, kThreads, 0, s>>>(a);
-    rc = launch_check(c, "broadcast");
-    if (rc) return rc;
-    commit_args(c, a);
-    c->pipe_base += rounds;
-    done += n;
-  }
-  return B200C_OK;
+    return B200C_OK;
+  });
 }
 
 extern "C" int b200c_barrier(b200c_comm_t* c, b200c_stream_t stream) {
@@ -1406,14 +1391,50 @@ extern "C" int b200c_barrier(b200c_comm_t* c, b200c_stream_t stream) {
   if (rc) return rc;
   if (c->world == 1) return B200C_OK;
   DeviceGuard g(c->device);
-  CollArgs a;
-  base_args(c, &a);
-  a.sig = make_sig(OPC_BARRIER, 0, 0, 0, -1, 0);
-  k_barrier<<<1, 32, 0, (cudaStream_t)stream>>>(a);
-  rc = launch_check(c, "barrier");
+  return barrier_op(c, (cudaStream_t)stream);
+}
+
+// One message over a cell ring: a.buf, a.bytes and the ring's offsets are set by the caller.  *ctr counts the
+// cells this side has moved through the ring and only advances once the kernel is really queued.
+static int launch_cells(b200c_comm* c, P2PArgs& a, uint32_t* ctr, void (*kernel)(P2PArgs), const char* what, cudaStream_t s) {
+  size_t cb = c->cfg.p2p_slot_bytes;
+  size_t ncells = (a.bytes + cb - 1) / cb;
+  if (ncells > 0x7fffffffull) return fail(B200C_EINVAL, "message too large for the cell ring");
+  a.c = c->dev;
+  a.first_cell = *ctr; a.ncells = (uint32_t)ncells;
+  // no block may wait on a cell that one of its own later iterations has to free: grid <= ring size
+  uint32_t grid = (uint32_t)ncells;
+  uint32_t lim = c->cfg.max_blocks < (uint32_t)a.cells ? c->cfg.max_blocks : (uint32_t)a.cells;
+  if (kernel == k_send) {
+    // A sender block publishes `batch` cells per release fence (stride grid).  Small messages keep batch 1
+    // (one cell per block: lowest latency); large ones amortise the fence.  All cells of one pass over the
+    // grid must fit in the ring together, or a block would wait for an ack that only a later cell of its own
+    // pass triggers: grid * batch <= ring cells.
+    uint32_t batch = (uint32_t)((ncells + lim - 1) / lim);
+    if (batch < 1) batch = 1;
+    if (batch > (uint32_t)kSendBatch) batch = kSendBatch;
+    a.batch = (int)batch;
+    uint32_t lim_s = (uint32_t)a.cells / batch;
+    if (lim_s < 1) lim_s = 1;
+    if (lim > lim_s) lim = lim_s;
+    uint32_t want = ((uint32_t)ncells + batch - 1) / batch;
+    grid = want < 1 ? 1 : want;
+  }
+  if (grid > lim) grid = lim;
+  kernel<<<grid, kThreads, 0, s>>>(a);
+  int rc = launch_check(c, what);
   if (rc) return rc;
-  commit_args(c, a);
+  *ctr += (uint32_t)ncells;
   return B200C_OK;
+}
+// the pairwise ring of (this rank, peer), or the multi-reader ring of source rank `peer` (`multi`)
+static P2PArgs ring_args(b200c_comm* c, void* buf, size_t bytes, int peer, bool multi) {
+  P2PArgs a;
+  memset(&a, 0, sizeof a);
+  a.buf = buf; a.bytes = bytes; a.peer = peer;
+  if (multi) { a.off_ring = c->off_mring; a.off_ready = kOffMReady; a.off_ack = kOffMAck; a.cells = (int)c->mcells; }
+  else { a.off_ring = c->off_p2p; a.off_ready = kOffP2PReady; a.off_ack = kOffP2PAck; a.cells = (int)c->cfg.p2p_slots; }
+  return a;
 }
 
 static int p2p_impl(b200c_comm* c, void* buf, size_t bytes, int peer, bool is_send, cudaStream_t s) {
@@ -1424,42 +1445,9 @@ static int p2p_impl(b200c_comm* c, void* buf, size_t bytes, int peer, bool is_se
   if (bytes == 0) return B200C_OK;
   if (!buf) return fail(B200C_EINVAL, "null buffer");
   DeviceGuard g(c->device);
-  P2PArgs a;
-  memset(&a, 0, sizeof a);
-  a.c = c->dev; a.buf = buf; a.bytes = bytes; a.peer = peer;
-  a.off_ring = c->off_p2p; a.off_ready = kOffP2PReady; a.off_ack = kOffP2PAck; a.cells = (int)c->cfg.p2p_slots;
-  size_t cb = c->cfg.p2p_slot_bytes;
-  size_t ncells = (bytes + cb - 1) / cb;
-  if (ncells > 0x7fffffffull) return fail(B200C_EINVAL, "message too large for the cell ring");
-  uint32_t* ctr = is_send ? &c->send_cells[peer] : &c->recv_cells[peer];
-  a.first_cell = *ctr; a.ncells = (uint32_t)ncells;
-  // no block may wait on a cell that one of its own later iterations has to free: grid <= ring size
-  uint32_t grid = (uint32_t)ncells;
-  uint32_t lim = c->cfg.max_blocks < c->cfg.p2p_slots ? c->cfg.max_blocks : c->cfg.p2p_slots;
-  if (is_send) {
-    // A sender block publishes `batch` cells per release fence (stride grid).  Small messages keep batch 1
-    // (one cell per block: lowest latency); large ones amortise the fence.  All cells of one pass over the
-    // grid must fit in the ring together, or a block would wait for an ack that only a later cell of its own
-    // pass triggers: grid * batch <= ring cells.
-    static int env_batch = [] { const char* e = getenv("B200COLL_SEND_BATCH"); return e ? atoi(e) : 0; }();
-    uint32_t batch = (uint32_t)((ncells + lim - 1) / lim);
-    if (env_batch > 0) batch = (uint32_t)env_batch;
-    if (batch < 1) batch = 1;
-    if (batch > (uint32_t)kSendBatch) batch = kSendBatch;
-    a.batch = (int)batch;
-    uint32_t lim_s = c->cfg.p2p_slots / batch;
-    if (lim_s < 1) lim_s = 1;
-    if (lim > lim_s) lim = lim_s;
-    uint32_t want = ((uint32_t)ncells + batch - 1) / batch;
-    grid = want < 1 ? 1 : want;
-  }
-  if (grid > lim) grid = lim;
-  if (is_send) k_send<<<grid, kThreads, 0, s>>>(a);
-  else k_recv<<<grid, kThreads, 0, s>>>(a);
-  rc = launch_check(c, is_send ? "send" : "recv");
-  if (rc) return rc;
-  *ctr += (uint32_t)ncells;  // the ring position only advances once the kernel is really queued
-  return B200C_OK;
+  P2PArgs a = ring_args(c, buf, bytes, peer, false);
+  if (is_send) return launch_cells(c, a, &c->send_cells[peer], k_send, "send", s);
+  return launch_cells(c, a, &c->recv_cells[peer], k_recv, "recv", s);
 }
 extern "C" int b200c_send(b200c_comm_t* c, const void* buf, size_t bytes, int peer, b200c_stream_t stream) {
   return p2p_impl(c, const_cast<void*>(buf), bytes, peer, true, (cudaStream_t)stream);
@@ -1489,21 +1477,10 @@ extern "C" int b200c_send_multi(b200c_comm_t* c, const void* buf, size_t bytes, 
   if (bytes == 0) return B200C_OK;
   if (!buf) return fail(B200C_EINVAL, "null buffer");
   DeviceGuard g(c->device);
-  P2PArgs a;
-  memset(&a, 0, sizeof a);
-  a.c = c->dev; a.buf = const_cast<void*>(buf); a.bytes = bytes; a.peer = -1; a.reader_mask = mask;
-  a.off_ring = c->off_mring; a.off_ready = kOffMReady; a.off_ack = kOffMAck; a.cells = (int)c->mcells;
-  size_t cb = c->cfg.p2p_slot_bytes;
-  size_t ncells = (bytes + cb - 1) / cb;
-  if (ncells > 0x7fffffffull) return fail(B200C_EINVAL, "message too large for the cell ring");
-  a.first_cell = c->msend_cells; a.ncells = (uint32_t)ncells;
-  uint32_t grid = (uint32_t)ncells;
-  uint32_t lim = c->cfg.max_blocks < c->mcells ? c->cfg.max_blocks : c->mcells;
-  if (grid > lim) grid = lim;
-  k_send_multi<<<grid, kThreads, 0, (cudaStream_t)stream>>>(a);
-  rc = launch_check(c, "send_multi");
+  P2PArgs a = ring_args(c, const_cast<void*>(buf), bytes, -1, true);
+  a.reader_mask = mask;
+  rc = launch_cells(c, a, &c->msend_cells, k_send_multi, "send_multi", (cudaStream_t)stream);
   if (rc) return rc;
-  c->msend_cells += (uint32_t)ncells;
   c->msend_mask = mask;
   return B200C_OK;
 }
@@ -1516,20 +1493,6 @@ extern "C" int b200c_recv_multi(b200c_comm_t* c, void* buf, size_t bytes, int sr
   if (bytes == 0) return B200C_OK;
   if (!buf) return fail(B200C_EINVAL, "null buffer");
   DeviceGuard g(c->device);
-  P2PArgs a;
-  memset(&a, 0, sizeof a);
-  a.c = c->dev; a.buf = buf; a.bytes = bytes; a.peer = src;
-  a.off_ring = c->off_mring; a.off_ready = kOffMReady; a.off_ack = kOffMAck; a.cells = (int)c->mcells;
-  size_t cb = c->cfg.p2p_slot_bytes;
-  size_t ncells = (bytes + cb - 1) / cb;
-  if (ncells > 0x7fffffffull) return fail(B200C_EINVAL, "message too large for the cell ring");
-  a.first_cell = c->mrecv_cells[src]; a.ncells = (uint32_t)ncells;
-  uint32_t grid = (uint32_t)ncells;
-  uint32_t lim = c->cfg.max_blocks < c->mcells ? c->cfg.max_blocks : c->mcells;
-  if (grid > lim) grid = lim;
-  k_recv<<<grid, kThreads, 0, (cudaStream_t)stream>>>(a);
-  rc = launch_check(c, "recv_multi");
-  if (rc) return rc;
-  c->mrecv_cells[src] += (uint32_t)ncells;
-  return B200C_OK;
+  P2PArgs a = ring_args(c, buf, bytes, src, true);
+  return launch_cells(c, a, &c->mrecv_cells[src], k_recv, "recv_multi", (cudaStream_t)stream);
 }

@@ -1,9 +1,23 @@
 // Per-dtype launch tables.  Each inst_<dtype>.cu instantiates this for one storage type so the
 // translation units compile in parallel.
 #pragma once
+#include <type_traits>
+
 #include "coll_kernels.cuh"
 
 namespace b200c {
+
+// The reducing kernels exist once per world size 2 / 4 / 8 and once for the other sizes (WT = 0):
+// calls f(std::integral_constant<int, WT>) for the communicator's world size.
+template <typename F>
+static auto with_world_t(int world, F&& f) {
+  switch (world) {
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    default: return f(std::integral_constant<int, 0>{});
+  }
+}
 
 enum Kind { KIND_ONESHOT = 0, KIND_TWOSHOT = 1, KIND_REDUCESCATTER = 2, KIND_REDUCE = 3, KIND_LL = 4 };
 
@@ -20,15 +34,9 @@ static int launch_kind_w(int kind, const CollArgs& a, int grid, cudaStream_t s) 
   return B200C_OK;
 }
 
-// the reducing kernels exist once per world size 2 / 4 / 8 and once for the other sizes (WT = 0)
 template <typename T, int OP>
 static int launch_kind(int kind, const CollArgs& a, int grid, cudaStream_t s) {
-  switch (a.c.world) {
-    case 2: return launch_kind_w<T, OP, 2>(kind, a, grid, s);
-    case 4: return launch_kind_w<T, OP, 4>(kind, a, grid, s);
-    case 8: return launch_kind_w<T, OP, 8>(kind, a, grid, s);
-    default: return launch_kind_w<T, OP, 0>(kind, a, grid, s);
-  }
+  return with_world_t(a.c.world, [&](auto wt) { return launch_kind_w<T, OP, decltype(wt)::value>(kind, a, grid, s); });
 }
 
 template <typename T>

@@ -271,7 +271,8 @@ def test_block_cyclic_granules(W):
     large-message layout), with ragged tails, for every kernel that uses it."""
     from ant_ray_b200.loopback import LoopbackWorld
 
-    w = LoopbackWorld(W, device=0, key=f"lb-gran{W}", staging_bytes=4 << 20, max_blocks=3, granule_bytes=16384, timeout_ms=20000)
+    w = LoopbackWorld(W, device=0, key=f"lb-gran{W}", staging_bytes=4 << 20, max_blocks=3, granule_bytes=16384,
+                      bcast_rounds_min_bytes=4 << 20, timeout_ms=20000)
     try:
         n = 300_007
         for dtype, algo in ((torch.float32, N.ALGO_TWOSHOT), (torch.int32, N.ALGO_ONESHOT), (torch.bfloat16, N.ALGO_TWOSHOT)):
@@ -298,12 +299,17 @@ def test_block_cyclic_granules(W):
             assert_equal_bits(outs[r], want[r], "granules: reducescatter")
             for j in range(W):
                 assert_equal_bits(gouts[r][j], lists[j][0], "granules: allgather")
+        # past one staging half: the first 4 MiB piece takes the pipelined unicast push (bcast_rounds_min_bytes),
+        # the ragged rest the plain kernel
+        big = [make_input(torch.float32, 1_300_007, r) for r in range(W)]
         for root in (0, W - 1):
-            dev = [t.cuda() for t in ins]
-            w.run(lambda r, c: c.broadcast(dev[r].data_ptr(), n, N.FLOAT32, root))
-            torch.cuda.synchronize()
-            for r in range(W):
-                assert_equal_bits(dev[r], ins[root], "granules: broadcast")
+            for src, what in ((ins, "granules: broadcast"), (big, "granules: pipelined broadcast")):
+                dev = [t.cuda() for t in src]
+                w.run(lambda r, c: c.broadcast(dev[r].data_ptr(), dev[r].numel(), N.FLOAT32, root))
+                torch.cuda.synchronize()
+                w.check()
+                for r in range(W):
+                    assert_equal_bits(dev[r], src[root], what)
             dev = [t.cuda() for t in ins]
             w.run(lambda r, c: c.reduce(dev[r].data_ptr(), dev[r].data_ptr(), n, N.FLOAT32, N.SUM, root))
             torch.cuda.synchronize()

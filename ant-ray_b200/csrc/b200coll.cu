@@ -569,13 +569,14 @@ extern "C" int b200c_comm_check(b200c_comm_t* c) {
   if (!c->status_host) return B200C_OK;
   int e = c->status_host->error;
   if (e == 0) return B200C_OK;
-  static const char* phases[] = {"arrive", "flagA", "flagB", "p2p-ready", "p2p-ack"};
+  static const char* const phases[] = {"arrive", "flagA", "flagB", "p2p-ready", "p2p-ack", "ll-slot"};  // by WaitPhase
+  static_assert(sizeof(phases) / sizeof(phases[0]) == kNumWaitPhases, "one name per WaitPhase");
   int ph = c->status_host->err_phase;
   if (e == B200C_EMISMATCH)
     return fail(e, "%s: rank %d, op seq %u, peer %d announced signature %08x, this rank expected %08x", b200c_status_string(e), c->rank,
                 c->status_host->err_seq, c->status_host->err_peer, c->status_host->err_a, c->status_host->err_b);
   return fail(e, "%s: rank %d, op seq %u, waiting on peer %d (%s)", b200c_status_string(e), c->rank, c->status_host->err_seq,
-              c->status_host->err_peer, ph >= 0 && ph < 5 ? phases[ph] : "?");
+              c->status_host->err_peer, ph >= 0 && ph < kNumWaitPhases ? phases[ph] : "?");
 }
 
 extern "C" int b200c_comm_destroy(b200c_comm_t* c) {

@@ -18,26 +18,21 @@ __global__ void __launch_bounds__(kThreads) k_allgather(const __grid_constant__ 
   const uint8_t* in = static_cast<const uint8_t*>(a.in);
   uint8_t* own_out = static_cast<uint8_t*>(a.out_ptrs[r]);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
-    for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
-      copy_tile<uint8_t, false>(staging_ptr<uint8_t>(c, j, a.seq, (size_t)r * slot_bytes) + t0, in + t0, t1 - t0);
-    }
+    for (int k = 1; k < W; k++)
+      copy_tile<uint8_t, false>(staging_ptr<uint8_t>(c, peer_at(r, k, W), a.seq, (size_t)r * slot_bytes) + t0, in + t0, t1 - t0);
     if (own_out != in) copy_tile<uint8_t, false>(own_out + t0, in + t0, t1 - t0);
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
+      const int j = peer_at(r, k, W);
       copy_tile<uint8_t, true>(static_cast<uint8_t*>(a.out_ptrs[j]) + t0, staging_ptr<uint8_t>(c, r, a.seq, (size_t)j * slot_bytes) + t0, t1 - t0);
     }
   }
 }
 
-__device__ __forceinline__ void multimem_st16_bytes(void* p, uint4 v) {
-  asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 // nv 16-byte vectors: src (plain or staging) -> multicast address
 template <bool SRC_BYPASS>
 __device__ __forceinline__ void multicast_tile(char* mc, const uint4* s, size_t nv) {
@@ -47,9 +42,9 @@ __device__ __forceinline__ void multicast_tile(char* mc, const uint4* s, size_t 
 #pragma unroll
     for (int u = 0; u < kUnroll; u++) v[u] = SRC_BYPASS ? ld_bypass16(s + i + (size_t)u * kThreads) : s[i + (size_t)u * kThreads];
 #pragma unroll
-    for (int u = 0; u < kUnroll; u++) multimem_st16_bytes(mc + (i + (size_t)u * kThreads) * 16, v[u]);
+    for (int u = 0; u < kUnroll; u++) multimem_st16(mc + (i + (size_t)u * kThreads) * 16, v[u]);
   }
-  for (; i < nv; i += kThreads) multimem_st16_bytes(mc + i * 16, SRC_BYPASS ? ld_bypass16(s + i) : s[i]);
+  for (; i < nv; i += kThreads) multimem_st16(mc + i * 16, SRC_BYPASS ? ld_bypass16(s + i) : s[i]);
 }
 
 // a.symmetric selects the variant:
@@ -72,15 +67,13 @@ __global__ void __launch_bounds__(kThreads) k_broadcast(const __grid_constant__ 
         done = nv * 16;
       }
       if (done < cnt) {
-        for (int k = 1; k < W; k++) {
-          int j = r + k; if (j >= W) j -= W;
-          copy_tile<uint8_t, false>(staging_ptr<uint8_t>(c, j, a.seq, 0) + t0 + done, src + done, cnt - done);
-        }
+        for (int k = 1; k < W; k++)
+          copy_tile<uint8_t, false>(staging_ptr<uint8_t>(c, peer_at(r, k, W), a.seq, 0) + t0 + done, src + done, cnt - done);
       }
     }
     block_signal_all(kOffFlagA, a.seq, c);
   } else {
-    if (!block_wait_one(my_flags(kOffFlagA, c) + root, a.seq, c, root, 1)) return;
+    if (!block_wait_one(flag_at(c, r, kOffFlagA, blockIdx.x, root), a.seq, c, root, kWaitFlagA)) return;
     check_signature(a);
     B200C_FOR_GRANULES(t0, t1, a, a.n) {
       copy_tile<uint8_t, true>(static_cast<uint8_t*>(a.out) + t0, staging_ptr<uint8_t>(c, r, a.seq, 0) + t0, t1 - t0);
@@ -106,12 +99,10 @@ __global__ void __launch_bounds__(kThreads, 2) k_broadcast_rounds(const __grid_c
   check_signature(a);
   const size_t half_off = c.off_staging + (size_t)(a.seq & 1) * c.staging_bytes;
   uint8_t* mine = reinterpret_cast<uint8_t*>(c.arena[r] + half_off);
-  const size_t first = (size_t)blockIdx.x * a.tile, step = (size_t)gridDim.x * a.tile;
-  if (first >= a.chunk) return;
-  const int R = (int)((a.chunk - first + step - 1) / step);
+  const BlockRounds rd(a);
+  if (rd.empty()) return;
+  const int R = rd.count();
   const int t = threadIdx.x;
-  auto lo_of = [&](int q) { return first + (size_t)q * step; };
-  auto hi_of = [&](int q) { size_t h = first + (size_t)q * step + a.tile; return h < a.chunk ? h : a.chunk; };
   if (a.symmetric == 3) {
     // Unicast rounds (world of two, or no multicast object): chunk == the whole message.  The root pushes
     // granule q to every peer and raises pipeA; a peer copies granule q out as soon as it has landed, so
@@ -119,31 +110,30 @@ __global__ void __launch_bounds__(kThreads, 2) k_broadcast_rounds(const __grid_c
     if (r == root) {
       const uint8_t* src = static_cast<const uint8_t*>(a.in);
       for (int q = 0; q < R; q++) {
-        const size_t g0 = lo_of(q), cnt = clip_count(g0, hi_of(q), a.n);
-        for (int k = 1; k < W && cnt; k++) {
-          int j = r + k; if (j >= W) j -= W;
-          copy_tile<uint8_t, false>(reinterpret_cast<uint8_t*>(c.arena[j] + half_off) + g0, src + g0, cnt);
-        }
-        round_signal(kOffPipeA, a.pipe_base + q + 1, c);
+        const auto [g0, cnt] = chunk_span(a, 0, rd.lo(q), rd.hi(q));
+        for (int k = 1; k < W && cnt; k++)
+          copy_tile<uint8_t, false>(reinterpret_cast<uint8_t*>(c.arena[peer_at(r, k, W)] + half_off) + g0, src + g0, cnt);
+        block_signal_all(kOffPipeA, a.pipe_base + q + 1, c);
       }
       return;
     }
     uint8_t* out = static_cast<uint8_t*>(a.out);
-    const uint32_t* fA = reinterpret_cast<const uint32_t*>(c.arena[r] + kOffPipeA) + (size_t)blockIdx.x * 8 + root;
+    const uint32_t* fA = flag_at(c, r, kOffPipeA, blockIdx.x, root);
     for (int q = 0; q < R; q++) {
-      if (!block_wait_one(fA, a.pipe_base + q + 1, c, root, 1)) return;
-      const size_t g0 = lo_of(q), cnt = clip_count(g0, hi_of(q), a.n);
+      if (!block_wait_one(fA, a.pipe_base + q + 1, c, root, kWaitFlagA)) return;
+      const auto [g0, cnt] = chunk_span(a, 0, rd.lo(q), rd.hi(q));
       if (cnt) copy_tile<uint8_t, true>(out + g0, mine + g0, cnt);
     }
     return;
   }
+  // the multicast rounds clip by hand: chunk_span() here changes this kernel's register allocation
   char* mc = c.mc_arena + half_off;
   if (r == root) {
     const uint8_t* src = static_cast<const uint8_t*>(a.in);
     for (int q = 0; q < R; q++) {
-      const size_t g0 = lo_of(q), g1 = hi_of(q);
+      const size_t g0 = rd.lo(q), g1 = rd.hi(q);
       for (int k = 1; k < W; k++) {
-        int j = r + k; if (j >= W) j -= W;
+        const int j = peer_at(r, k, W);
         size_t lo = (size_t)j * a.chunk + g0;
         size_t cnt = clip_count(lo, (size_t)j * a.chunk + g1, a.n);
         if (cnt) copy_tile<uint8_t, false>(reinterpret_cast<uint8_t*>(c.arena[j] + half_off) + lo, src + lo, cnt);
@@ -157,28 +147,27 @@ __global__ void __launch_bounds__(kThreads, 2) k_broadcast_rounds(const __grid_c
       if (t < W && t != r) {
         // one fence covers both flags of this peer
         asm volatile("fence.acq_rel.sys;" ::: "memory");
-        st_relaxed_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffPipeA) + (size_t)blockIdx.x * 8 + r, a.pipe_base + q + 1);
-        st_relaxed_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffPipeB) + (size_t)blockIdx.x * 8 + r, a.pipe_base + q + 1);
+        st_relaxed_sys(flag_at(c, t, kOffPipeA, blockIdx.x, r), a.pipe_base + q + 1);
+        st_relaxed_sys(flag_at(c, t, kOffPipeB, blockIdx.x, r), a.pipe_base + q + 1);
       }
     }
     return;
   }
   uint8_t* out = static_cast<uint8_t*>(a.out);
-  const uint32_t* fA = reinterpret_cast<const uint32_t*>(c.arena[r] + kOffPipeA) + (size_t)blockIdx.x * 8 + root;
+  const uint32_t* fA = flag_at(c, r, kOffPipeA, blockIdx.x, root);
   for (int q = 0; q <= R; q++) {
     if (q < R) {
-      if (!block_wait_one(fA, a.pipe_base + q + 1, c, root, 1)) return;
-      size_t lo = (size_t)r * a.chunk + lo_of(q);
-      size_t cnt = clip_count(lo, (size_t)r * a.chunk + hi_of(q), a.n);
+      if (!block_wait_one(fA, a.pipe_base + q + 1, c, root, kWaitFlagA)) return;
+      size_t lo = (size_t)r * a.chunk + rd.lo(q);
+      size_t cnt = clip_count(lo, (size_t)r * a.chunk + rd.hi(q), a.n);
       if (cnt) multicast_tile<true>(mc + lo, reinterpret_cast<const uint4*>(mine + lo), cnt / 16);
-      round_signal(kOffPipeB, a.pipe_base + q + 1, c);
+      block_signal_all(kOffPipeB, a.pipe_base + q + 1, c);
     }
     if (q >= 1) {
-      if (!round_wait(kOffPipeB, a.pipe_base + q, c, 2)) return;
-      const size_t g0 = lo_of(q - 1), g1 = hi_of(q - 1);
+      if (!block_wait_all(kOffPipeB, a.pipe_base + q, c, kWaitFlagB)) return;
       for (int j = 0; j < W; j++) {
-        size_t lo = (size_t)j * a.chunk + g0;
-        size_t cnt = clip_count(lo, (size_t)j * a.chunk + g1, a.n);
+        size_t lo = (size_t)j * a.chunk + rd.lo(q - 1);
+        size_t cnt = clip_count(lo, (size_t)j * a.chunk + rd.hi(q - 1), a.n);
         if (cnt) copy_tile<uint8_t, true>(out + lo, mine + lo, cnt);
       }
     }
@@ -190,8 +179,8 @@ __global__ void __launch_bounds__(32) k_barrier(const __grid_constant__ CollArgs
   const DevComm& c = a.c;
   int t = threadIdx.x;
   if (t < c.world && t != c.rank) {
-    st_release_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffArrive) + c.rank, a.seq);
-    wait_flag(reinterpret_cast<const uint32_t*>(c.arena[c.rank] + kOffArrive) + t, a.seq, c, t, 0);
+    st_release_sys(flag_at(c, t, kOffArrive, 0, c.rank), a.seq);
+    wait_flag(flag_at(c, c.rank, kOffArrive, 0, t), a.seq, c, t, kWaitArrive);
   }
 }
 
@@ -234,7 +223,7 @@ __global__ void __launch_bounds__(kThreads) k_send(const __grid_constant__ P2PAr
       uint32_t i = i0 + (uint32_t)t * gridDim.x, k = a.first_cell + i;
       if (i < a.ncells && k >= (uint32_t)a.cells) {
         uint32_t pos = k % (uint32_t)a.cells;
-        ok = wait_flag(reinterpret_cast<const uint32_t*>(c.arena[r] + a.off_ack) + (size_t)d * kMaxCells + pos, k + 1 - (uint32_t)a.cells, c, d, 4);
+        ok = wait_flag(reinterpret_cast<const uint32_t*>(c.arena[r] + a.off_ack) + (size_t)d * kMaxCells + pos, k + 1 - (uint32_t)a.cells, c, d, kWaitP2PAck);
       }
     }
     if (!__syncthreads_and(ok)) return;
@@ -277,7 +266,7 @@ __global__ void __launch_bounds__(kThreads) k_send_multi(const __grid_constant__
     uint32_t pos = k % (uint32_t)a.cells;
     if (k >= (uint32_t)a.cells) {
       int ok = 1;
-      if (reader) ok = wait_flag(reinterpret_cast<const uint32_t*>(c.arena[r] + a.off_ack) + (size_t)t * kMaxCells + pos, k + 1 - (uint32_t)a.cells, c, t, 4);
+      if (reader) ok = wait_flag(reinterpret_cast<const uint32_t*>(c.arena[r] + a.off_ack) + (size_t)t * kMaxCells + pos, k + 1 - (uint32_t)a.cells, c, t, kWaitP2PAck);
       if (!__syncthreads_and(ok)) return;
     }
     size_t off = (size_t)i * cb;
@@ -306,7 +295,7 @@ __global__ void __launch_bounds__(kThreads) k_recv(const __grid_constant__ P2PAr
     uint32_t k = a.first_cell + i;
     uint32_t pos = k % (uint32_t)a.cells;
     const uint32_t* ready = reinterpret_cast<const uint32_t*>(c.arena[r] + a.off_ready) + (size_t)s * kMaxCells + pos;
-    if (!block_wait_one(ready, k + 1, c, s, 3)) return;
+    if (!block_wait_one(ready, k + 1, c, s, kWaitP2PReady)) return;
     size_t off = (size_t)i * cb;
     size_t cnt = a.bytes - off < cb ? a.bytes - off : cb;
     const uint8_t* src = reinterpret_cast<const uint8_t*>(c.arena[r] + a.off_ring + ((size_t)s * a.cells + pos) * cb);

@@ -21,11 +21,6 @@ template <typename T>
 __device__ __forceinline__ T* staging_ptr(const DevComm& c, int rank, uint32_t seq, size_t byte_off) {
   return reinterpret_cast<T*>(c.arena[rank] + c.off_staging + (size_t)(seq & 1) * c.staging_bytes + byte_off);
 }
-// clip [lo, hi) against n, return count
-__device__ __forceinline__ size_t clip_count(size_t lo, size_t hi, size_t n) {
-  if (lo >= n) return 0;
-  return (hi < n ? hi : n) - lo;
-}
 // granules of a chunk of `extent` elements owned by this block: [g0, g1) for g0 = first, first + step, ...
 #define B200C_FOR_GRANULES(g0, g1, a, extent)                                                                 \
   for (size_t g0 = (size_t)blockIdx.x * (a).tile, g1 = g0 + (a).tile < (extent) ? g0 + (a).tile : (extent); \
@@ -48,13 +43,11 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_oneshot(const __grid_
   TI* out = static_cast<TI*>(a.out);
   const size_t slot_bytes = a.chunk * sizeof(TW);  // chunk == padded n for one-shot
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
-    for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
-      move_tile<TI, TW, false>(staging_ptr<TW>(c, j, a.seq, (size_t)r * slot_bytes) + t0, in + t0, t1 - t0);
-    }
+    for (int k = 1; k < W; k++)
+      move_tile<TI, TW, false>(staging_ptr<TW>(c, peer_at(r, k, W), a.seq, (size_t)r * slot_bytes) + t0, in + t0, t1 - t0);
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     reduce_tile<TI, TW, OP, WT>(a, staging_ptr<TW>(c, r, a.seq, 0) + t0, a.chunk, r, in + t0, nullptr, out + t0, t1 - t0);
@@ -107,6 +100,8 @@ __device__ __forceinline__ void ll_allreduce_body(const CollArgs& a) {
       for (int e = 0; e < V; e++)
         if (e0 + e < a.n) mine.e[e] = in[e0 + e];
     }
+    // the peer order and the signature compare below are spelled out here rather than through peer_at() /
+    // compare_signature(): through the helpers sm_90a allocates the LL bodies differently (local memory at W = 4)
     for (int k = 1; k < W; k++) {
       int j = r + k; if (j >= W) j -= W;
       char* dst = ll_slot(c, j, flag, r) + i * 32;
@@ -134,12 +129,12 @@ __device__ __forceinline__ void ll_allreduce_body(const CollArgs& a) {
           asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(sv) : "l"(sl) : "memory");
           if ((uint32_t)(sv >> 32) == a.seq && (uint32_t)sv != a.sig) {
             if (c.status->error == 0) { c.status->err_a = (uint32_t)sv; c.status->err_b = a.sig; }
-            record_error(c.status, B200C_EMISMATCH, a.seq, s, 5);
+            record_error(c.status, B200C_EMISMATCH, a.seq, s, kWaitLL);
             c.status->abort_flag = 1;
             ok = false; break;
           }
-          if (c.status->abort_flag) { record_error(c.status, B200C_EABORTED, a.seq, s, 5); ok = false; break; }
-          if (globaltimer_ns() - t_start > c.timeout_ns) { record_error(c.status, B200C_ETIMEOUT, a.seq, s, 5); ok = false; break; }
+          if (c.status->abort_flag) { record_error(c.status, B200C_EABORTED, a.seq, s, kWaitLL); ok = false; break; }
+          if (globaltimer_ns() - t_start > c.timeout_ns) { record_error(c.status, B200C_ETIMEOUT, a.seq, s, kWaitLL); ok = false; break; }
         }
       }
       raw[s] = make_uint4((uint32_t)q0, (uint32_t)q1, (uint32_t)q2, (uint32_t)q3);
@@ -183,27 +178,16 @@ __global__ void __launch_bounds__(kLLThreads) k_allreduce_ll(const __grid_consta
   const int t = threadIdx.x;
   // announce (seq, signature) first — a plain store, no fence — so a peer that entered this op with
   // different arguments is diagnosed instead of both sides timing out
-  if (blockIdx.x == 0 && t < c.world && t != c.rank) {
-    unsigned long long* sig = reinterpret_cast<unsigned long long*>(c.arena[t] + kOffOpSig) + (a.seq & 1) * 8 + c.rank;
-    unsigned long long tagged = ((unsigned long long)a.seq << 32) | a.sig;
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sig), "l"(tagged) : "memory");
-  }
+  if (blockIdx.x == 0 && t < c.world && t != c.rank) announce_signature(a, t);
   ll_allreduce_body<T, OP, WT>(a);
   // arrival (the op after this one may start: arrive rule) goes last so that the fence of the release
   // does not sit in front of the data stores
   if (blockIdx.x == 0 && t < c.world && t != c.rank) {
-    st_release_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffArrive) + c.rank, a.seq);
+    st_release_sys(flag_at(c, t, kOffArrive, 0, c.rank), a.seq);
     // a rank whose message is the SHORTER one receives everything it waits for and would not notice a
     // peer that passed other arguments: compare the announcement that peer made at the start of its kernel
     // (no waiting: if it has not landed yet the check is skipped, the longer side reports the mismatch)
-    const unsigned long long* sl = reinterpret_cast<const unsigned long long*>(c.arena[c.rank] + kOffOpSig) + (a.seq & 1) * 8 + t;
-    unsigned long long sv;
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(sv) : "l"(sl) : "memory");
-    if ((uint32_t)(sv >> 32) == a.seq && (uint32_t)sv != a.sig) {
-      if (c.status->error == 0) { c.status->err_a = (uint32_t)sv; c.status->err_b = a.sig; }
-      record_error(c.status, B200C_EMISMATCH, a.seq, t, 5);
-      c.status->abort_flag = 1;
-    }
+    compare_signature(a, t, kWaitLL);
   }
 }
 
@@ -224,30 +208,27 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_twoshot(const __grid_
   // ---- A
   B200C_FOR_GRANULES(t0, t1, a, a.chunk) {
     for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
-      size_t lo = (size_t)j * a.chunk + t0;
-      size_t cnt = clip_count(lo, (size_t)j * a.chunk + t1, a.n);
+      const int j = peer_at(r, k, W);
+      const auto [lo, cnt] = chunk_span(a, j, t0, t1);
       if (cnt) move_tile<TI, TW, false>(staging_ptr<TW>(c, j, a.seq, (size_t)r * slot_bytes) + t0, in + lo, cnt);
     }
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   // ---- B
   B200C_FOR_GRANULES(t0, t1, a, a.chunk) {
-    size_t lo = (size_t)r * a.chunk + t0;
-    size_t cnt = clip_count(lo, (size_t)r * a.chunk + t1, a.n);
+    const auto [lo, cnt] = chunk_span(a, r, t0, t1);
     if (cnt)
       reduce_tile<TI, TW, OP, WT>(a, staging_ptr<TW>(c, r, a.seq, 0) + t0, a.chunk, r, in + lo, staging_ptr<TW>(c, r, a.seq, (size_t)r * slot_bytes) + t0, out + lo, cnt);
   }
   block_signal_all(kOffFlagB, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagB, c), a.seq, c, 2)) return;
+  if (!block_wait_all(kOffFlagB, a.seq, c, kWaitFlagB)) return;
   // ---- C
   B200C_FOR_GRANULES(t0, t1, a, a.chunk) {
     for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
-      size_t lo = (size_t)j * a.chunk + t0;
-      size_t cnt = clip_count(lo, (size_t)j * a.chunk + t1, a.n);
+      const int j = peer_at(r, k, W);
+      const auto [lo, cnt] = chunk_span(a, j, t0, t1);
       if (cnt) move_tile<TW, TI, true>(out + lo, staging_ptr<TW>(c, j, a.seq, (size_t)j * slot_bytes) + t0, cnt);
     }
   }
@@ -266,12 +247,12 @@ __global__ void __launch_bounds__(kThreads, 2) k_reducescatter(const __grid_cons
   const size_t slot_bytes = a.chunk * sizeof(T);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
+      const int j = peer_at(r, k, W);
       copy_tile<T, false>(staging_ptr<T>(c, j, a.seq, (size_t)r * slot_bytes) + t0, static_cast<const T*>(a.in_ptrs[j]) + t0, t1 - t0);
     }
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     reduce_tile<T, T, OP, WT>(a, staging_ptr<T>(c, r, a.seq, 0) + t0, a.chunk, r, static_cast<const T*>(a.in_ptrs[r]) + t0, nullptr, static_cast<T*>(a.out) + t0, t1 - t0);
@@ -292,12 +273,12 @@ __global__ void __launch_bounds__(kThreads, 2) k_reducescatter_scaled(const __gr
   const size_t slot_bytes = a.chunk * sizeof(TW);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     for (int k = 1; k < W; k++) {
-      int j = r + k; if (j >= W) j -= W;
+      const int j = peer_at(r, k, W);
       move_tile<TI, TW, false>(staging_ptr<TW>(c, j, a.seq, (size_t)r * slot_bytes) + t0, static_cast<const TI*>(a.in_ptrs[j]) + t0, t1 - t0);
     }
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   B200C_FOR_GRANULES(t0, t1, a, a.n) {
     TW* own_slot = WT == 8 && sizeof(TI) > sizeof(TW) ? staging_ptr<TW>(c, r, a.seq, (size_t)r * slot_bytes) + t0 : nullptr;
@@ -318,9 +299,9 @@ __global__ void __launch_bounds__(kThreads, 2) k_reduce(const __grid_constant__ 
     }
     block_signal_one(kOffFlagA, a.seq, c, root);
     // wait for root's release: completion of any rank then implies every rank has arrived
-    block_wait_one(my_flags(kOffFlagB, c) + root, a.seq, c, root, 2);
+    block_wait_one(flag_at(c, r, kOffFlagB, blockIdx.x, root), a.seq, c, root, kWaitFlagB);
   } else {
-    if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+    if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
     check_signature(a);
     B200C_FOR_GRANULES(t0, t1, a, a.n) {
       reduce_tile<T, T, OP, WT>(a, staging_ptr<T>(c, r, a.seq, 0) + t0, a.chunk, r, static_cast<const T*>(a.in) + t0, nullptr, static_cast<T*>(a.out) + t0, t1 - t0);
@@ -368,32 +349,14 @@ __device__ __forceinline__ void multimem_st16(void* p, uint4 v) {
 // U = 4 vectors are in flight per thread.
 template <typename TW, int U>
 __device__ __forceinline__ void nvls_reduce_bcast_u(char* mc, size_t nv, const CollArgs& a, size_t i) {
-  constexpr int V = 16 / sizeof(TW);
   for (; i + (U - 1) * kThreads < nv; i += U * kThreads) {
     uint4 v[U];
 #pragma unroll
     for (int u = 0; u < U; u++) v[u] = Multimem<TW>::ld_reduce(mc + (i + u * kThreads) * 16);
 #pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (a.has_scale) {
-        Pack16<TW> p; p.u = v[u];
-#pragma unroll
-        for (int e = 0; e < V; e++) p.e[e] = Traits<TW>::from_acc(Traits<TW>::to_acc(p.e[e]) * a.scale);
-        v[u] = p.u;
-      }
-      multimem_st16(mc + (i + u * kThreads) * 16, v[u]);
-    }
+    for (int u = 0; u < U; u++) multimem_st16(mc + (i + u * kThreads) * 16, scale_vector<TW>(v[u], a));
   }
-  for (; i < nv; i += kThreads) {
-    uint4 v = Multimem<TW>::ld_reduce(mc + i * 16);
-    if (a.has_scale) {
-      Pack16<TW> p; p.u = v;
-#pragma unroll
-      for (int e = 0; e < V; e++) p.e[e] = Traits<TW>::from_acc(Traits<TW>::to_acc(p.e[e]) * a.scale);
-      v = p.u;
-    }
-    multimem_st16(mc + i * 16, v);
-  }
+  for (; i < nv; i += kThreads) multimem_st16(mc + i * 16, scale_vector<TW>(Multimem<TW>::ld_reduce(mc + i * 16), a));
 }
 template <typename TW>
 __device__ __forceinline__ void nvls_reduce_bcast(char* mc, size_t nv, const CollArgs& a) {
@@ -403,25 +366,18 @@ __device__ __forceinline__ void nvls_reduce_bcast(char* mc, size_t nv, const Col
 // switch reduces defined values)
 template <typename TI, typename TW>
 __device__ __forceinline__ void nvls_stage_in(const CollArgs& a, TW* mine, const TI* in, size_t g0, size_t g1) {
-  constexpr int V = 16 / sizeof(TW);
   const int W = a.c.world;
   for (int j = 0; j < W; j++) {
-    size_t lo = (size_t)j * a.chunk + g0, hi = (size_t)j * a.chunk + g1;
-    size_t cnt = clip_count(lo, hi, a.n);
+    const auto [lo, cnt] = chunk_span(a, j, g0, g1);
     if (cnt) move_tile<TI, TW, false>(mine + lo, in + lo, cnt);
-    size_t end = lo + cnt, padded = (end + V - 1) / V * V;
-    if (cnt && padded > end && padded <= hi) {
-      TW z = Traits<TW>::from_acc((typename Traits<TW>::A)0);
-      for (size_t k = end + threadIdx.x; k < padded; k += kThreads) mine[k] = z;
-    }
+    zero_pad_vector(mine, lo, cnt, lo + (g1 - g0));
   }
 }
 template <typename TI, typename TW>
 __device__ __forceinline__ void nvls_stage_out(const CollArgs& a, const TW* mine, TI* out, size_t g0, size_t g1) {
   const int W = a.c.world;
   for (int j = 0; j < W; j++) {
-    size_t lo = (size_t)j * a.chunk + g0;
-    size_t cnt = clip_count(lo, (size_t)j * a.chunk + g1, a.n);
+    const auto [lo, cnt] = chunk_span(a, j, g0, g1);
     if (cnt) move_tile<TW, TI, true>(out + lo, mine + lo, cnt);
   }
 }
@@ -442,16 +398,15 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls(const __grid_con
     B200C_FOR_GRANULES(g0, g1, a, a.chunk) nvls_stage_in<TI, TW>(a, mine, in, g0, g1);
   }
   block_signal_all(kOffFlagA, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagA, c), a.seq, c, 1)) return;
+  if (!block_wait_all(kOffFlagA, a.seq, c, kWaitFlagA)) return;
   check_signature(a);
   // ---- B: in-switch reduce of the own chunk's granules, broadcast back in place
   B200C_FOR_GRANULES(g0, g1, a, a.chunk) {
-    size_t lo = (size_t)r * a.chunk + g0;
-    size_t cnt = clip_count(lo, (size_t)r * a.chunk + g1, a.n);
+    const auto [lo, cnt] = chunk_span(a, r, g0, g1);
     if (cnt) nvls_reduce_bcast<TW>(c.mc_arena + base_off + lo * sizeof(TW), (cnt + V - 1) / V, a);
   }
   block_signal_all(kOffFlagB, a.seq, c);
-  if (!block_wait_all(my_flags(kOffFlagB, c), a.seq, c, 2)) return;
+  if (!block_wait_all(kOffFlagB, a.seq, c, kWaitFlagB)) return;
   // ---- C: stage out
   if (!a.symmetric) {
     B200C_FOR_GRANULES(g0, g1, a, a.chunk) nvls_stage_out<TI, TW>(a, mine, out, g0, g1);
@@ -473,22 +428,6 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls(const __grid_con
 // Round flags live in pipeA / pipeB [block][src]; the value of round q is pipe_base + q + 1, and the
 // host advances pipe_base by the number of rounds of every such op.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void round_signal(size_t flag_off, uint32_t v, const DevComm& c) {
-  __syncthreads();
-  int t = threadIdx.x;
-  if (t < c.world && t != c.rank) {
-    uint32_t* f = reinterpret_cast<uint32_t*>(c.arena[t] + flag_off) + (size_t)blockIdx.x * 8 + c.rank;
-    st_release_sys(f, v);
-  }
-}
-__device__ __forceinline__ bool round_wait(size_t flag_off, uint32_t v, const DevComm& c, int phase) {
-  const uint32_t* f = reinterpret_cast<const uint32_t*>(c.arena[c.rank] + flag_off) + (size_t)blockIdx.x * 8;
-  int ok = 1;
-  int t = threadIdx.x;
-  if (t < c.world && t != c.rank) ok = wait_flag(f + t, v, c, t, phase);
-  return __syncthreads_and(ok) != 0;
-}
-
 template <typename TI, typename TW>
 __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_rounds(const __grid_constant__ CollArgs a) {
   const DevComm& c = a.c;
@@ -500,32 +439,30 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_rounds(const __g
   TI* out = static_cast<TI*>(a.out);
   const size_t base_off = c.off_staging + (size_t)(a.seq & 1) * c.staging_bytes;
   TW* mine = reinterpret_cast<TW*>(c.arena[r] + base_off);
-  const size_t first = (size_t)blockIdx.x * a.tile, step = (size_t)gridDim.x * a.tile;
-  if (first >= a.chunk) return;
-  const int R = (int)((a.chunk - first + step - 1) / step);
-  auto lo_of = [&](int q) { return first + (size_t)q * step; };
-  auto hi_of = [&](int q) { size_t h = first + (size_t)q * step + a.tile; return h < a.chunk ? h : a.chunk; };
-  nvls_stage_in<TI, TW>(a, mine, in, lo_of(0), hi_of(0));
-  round_signal(kOffPipeA, a.pipe_base + 1, c);
+  const BlockRounds rd(a);
+  if (rd.empty()) return;
+  const int R = rd.count();
+  nvls_stage_in<TI, TW>(a, mine, in, rd.lo(0), rd.hi(0));
+  block_signal_all(kOffPipeA, a.pipe_base + 1, c);
   for (int q = 0; q < R; q++) {
     if (q + 1 < R) {
-      nvls_stage_in<TI, TW>(a, mine, in, lo_of(q + 1), hi_of(q + 1));
-      round_signal(kOffPipeA, a.pipe_base + q + 2, c);
+      nvls_stage_in<TI, TW>(a, mine, in, rd.lo(q + 1), rd.hi(q + 1));
+      block_signal_all(kOffPipeA, a.pipe_base + q + 2, c);
     }
-    if (!round_wait(kOffPipeA, a.pipe_base + q + 1, c, 1)) return;
-    {
-      size_t lo = (size_t)r * a.chunk + lo_of(q);
-      size_t cnt = clip_count(lo, (size_t)r * a.chunk + hi_of(q), a.n);
+    if (!block_wait_all(kOffPipeA, a.pipe_base + q + 1, c, kWaitFlagA)) return;
+    {  // clipped by hand: chunk_span() here changes this kernel's register allocation
+      size_t lo = (size_t)r * a.chunk + rd.lo(q);
+      size_t cnt = clip_count(lo, (size_t)r * a.chunk + rd.hi(q), a.n);
       if (cnt) nvls_reduce_bcast<TW>(c.mc_arena + base_off + lo * sizeof(TW), (cnt + V - 1) / V, a);
     }
-    round_signal(kOffPipeB, a.pipe_base + q + 1, c);
+    block_signal_all(kOffPipeB, a.pipe_base + q + 1, c);
     if (q >= 1) {
-      if (!round_wait(kOffPipeB, a.pipe_base + q, c, 2)) return;
-      nvls_stage_out<TI, TW>(a, mine, out, lo_of(q - 1), hi_of(q - 1));
+      if (!block_wait_all(kOffPipeB, a.pipe_base + q, c, kWaitFlagB)) return;
+      nvls_stage_out<TI, TW>(a, mine, out, rd.lo(q - 1), rd.hi(q - 1));
     }
   }
-  if (!round_wait(kOffPipeB, a.pipe_base + R, c, 2)) return;
-  nvls_stage_out<TI, TW>(a, mine, out, lo_of(R - 1), hi_of(R - 1));
+  if (!block_wait_all(kOffPipeB, a.pipe_base + R, c, kWaitFlagB)) return;
+  nvls_stage_out<TI, TW>(a, mine, out, rd.lo(R - 1), rd.hi(R - 1));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -564,26 +501,26 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_lanes(const __gr
   const int R = (size_t)lane < ngran ? (int)((ngran - lane + L - 1) / L) : 0;
   const size_t half_off = c.off_staging + (size_t)(a.seq & 1) * c.staging_bytes;
   auto ring_elem = [&](int slot, int j) { return (((size_t)lane * kLaneSlots + slot) * W + j) * T; };
-  uint32_t* laneIn = reinterpret_cast<uint32_t*>(c.arena[r] + kOffLaneIn) + (size_t)lane * 8;
+  uint32_t* laneIn = flag_at(c, r, kOffLaneIn, lane, 0);
   if (role == 0) {
     // ------------------------------------------------------------------ switch CTA
-    const uint32_t* fA = reinterpret_cast<const uint32_t*>(c.arena[r] + kOffPipeA) + (size_t)lane * 8;
+    const uint32_t* fA = flag_at(c, r, kOffPipeA, lane, 0);
     for (int q = 0; q < R; q++) {
       const uint32_t v = a.pipe_base + q + 1;
       int ok = 1;
-      if (t < Kc) ok = wait_flag(laneIn + t, v, c, r, 1);
+      if (t < Kc) ok = wait_flag(laneIn + t, v, c, r, kWaitFlagA);
       if (!__syncthreads_and(ok)) return;
-      if (t < W && t != r) st_release_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffPipeA) + (size_t)lane * 8 + r, v);
+      if (t < W && t != r) st_release_sys(flag_at(c, t, kOffPipeA, lane, r), v);
       ok = 1;
-      if (t < W && t != r) ok = wait_flag(fA + t, v, c, t, 1);
+      if (t < W && t != r) ok = wait_flag(fA + t, v, c, t, kWaitFlagA);
       if (!__syncthreads_and(ok)) return;
-      const size_t g0 = ((size_t)q * L + lane) * T;
+      const size_t g0 = ((size_t)q * L + lane) * T;   // clipped by hand, as in k_allreduce_nvls_rounds
       const size_t lo = (size_t)r * a.chunk + g0;
       const size_t hi = (size_t)r * a.chunk + (g0 + T < a.chunk ? g0 + T : a.chunk);
       const size_t cnt = clip_count(lo, hi, a.n);
       if (cnt) nvls_reduce_bcast<TW>(c.mc_arena + half_off + ring_elem(q % kLaneSlots, r) * sizeof(TW), (cnt + V - 1) / V, a);
       __syncthreads();
-      if (t < W) st_release_sys(reinterpret_cast<uint32_t*>(c.arena[t] + kOffPipeB) + (size_t)lane * 8 + r, v);
+      if (t < W) st_release_sys(flag_at(c, t, kOffPipeB, lane, r), v);
     }
     return;
   }
@@ -593,7 +530,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_lanes(const __gr
   TI* out = static_cast<TI*>(a.out);
   TW* ring = reinterpret_cast<TW*>(c.arena[r] + half_off);
   const size_t Tk = ((T + Kc - 1) / Kc + V - 1) / V * V;   // this CTA's share of a granule (whole vectors)
-  const uint32_t* fB = reinterpret_cast<const uint32_t*>(c.arena[r] + kOffPipeB) + (size_t)lane * 8;
+  const uint32_t* fB = flag_at(c, r, kOffPipeB, lane, 0);
   for (int q = 0; q < R + 2; q++) {
     if (q < R) {
       const size_t g0 = ((size_t)q * L + lane) * T;
@@ -618,7 +555,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_allreduce_nvls_lanes(const __gr
     if (q >= 2) {
       const int qq = q - 2;
       int ok = 1;
-      if (t < W) ok = wait_flag(fB + t, a.pipe_base + qq + 1, c, t, 2);
+      if (t < W) ok = wait_flag(fB + t, a.pipe_base + qq + 1, c, t, kWaitFlagB);
       if (!__syncthreads_and(ok)) return;
       const size_t g0 = ((size_t)qq * L + lane) * T;
       const size_t s0 = (size_t)k * Tk, s1 = s0 + Tk < T ? s0 + Tk : T;

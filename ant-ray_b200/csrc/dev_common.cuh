@@ -41,13 +41,17 @@ constexpr size_t kOffLaneIn = kOffMAck + 8 * kMaxCells * 4;     // u32 [kMaxBloc
 constexpr size_t kPadUsed = kOffLaneIn + kMaxBlocks * 8 * 4;
 static_assert(kPadUsed <= kPadBytes, "signal pad overflow");
 
+// What a failed wait was waiting for (Status::err_phase; b200c_comm_check names them in this order).
+// kWaitFlagA / kWaitFlagB also cover the round flags pipeA / pipeB and the lane kernel's laneIn.
+enum WaitPhase : int { kWaitArrive, kWaitFlagA, kWaitFlagB, kWaitP2PReady, kWaitP2PAck, kWaitLL, kNumWaitPhases };
+
 // host-pinned, device-mapped status block
 struct Status {
   volatile int abort_flag;   // host sets to 1: every spinning kernel gives up
   volatile int error;        // first error recorded by a kernel (b200c_status_t), 0 = none
   volatile unsigned err_seq; // sequence number of the op that failed
   volatile int err_peer;     // peer the kernel was waiting for
-  volatile int err_phase;    // 0 = arrive, 1 = flagA, 2 = flagB, 3 = p2p ready, 4 = p2p ack
+  volatile int err_phase;    // WaitPhase
   volatile unsigned err_a, err_b;  // mismatch: signature seen / expected
 };
 
@@ -106,11 +110,6 @@ __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
 __device__ __forceinline__ void st_relaxed_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
-__device__ __forceinline__ uint32_t ld_relaxed_sys(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 // 16-byte L1-bypassing load (staging written by peers, or peer memory over NVLink)
 __device__ __forceinline__ uint4 ld_bypass16(const void* p) {
   uint4 v;
@@ -153,11 +152,11 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 // ---------------------------------------------------------------------------------------------
 // bounded wait.  One thread per awaited flag.  Returns false on abort / timeout (and records it).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void record_error(Status* st, int code, uint32_t seq, int peer, int phase) {
+__device__ __forceinline__ void record_error(Status* st, int code, uint32_t seq, int peer, WaitPhase phase) {
   if (st->error == 0) { st->error = code; st->err_seq = seq; st->err_peer = peer; st->err_phase = phase; }
 }
 static __device__ __noinline__ bool wait_slow(const uint32_t* flag, uint32_t seq, Status* st, unsigned long long timeout_ns,
-                                       int peer, int phase) {
+                                       int peer, WaitPhase phase) {
   unsigned long long t0 = globaltimer_ns();
   unsigned spins = 0;
   for (;;) {
@@ -174,29 +173,31 @@ static __device__ __noinline__ bool wait_slow(const uint32_t* flag, uint32_t seq
   }
 }
 __device__ __forceinline__ bool wait_flag(const uint32_t* flag, uint32_t seq, const DevComm& c, int peer,
-                                          int phase) {
+                                          WaitPhase phase) {
 #pragma unroll 1
   for (int i = 0; i < 64; i++)
     if ((int32_t)(ld_acquire_sys(flag) - seq) >= 0) return true;
   return wait_slow(flag, seq, c.status, c.timeout_ns, peer, phase);
 }
 
-// named barrier among `nthreads` (multiple of 32) threads of one warp-specialised role
-__device__ __forceinline__ void role_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+// Flag [slot][src] of the u32 [kMaxBlocks][8] flag array at pad offset `off` in rank x's arena.  The slot is
+// the block index (the lane in the lane kernel); arrive[8] is an array of one slot.
+__device__ __forceinline__ uint32_t* flag_at(const DevComm& c, int x, size_t off, size_t slot, int src) {
+  return reinterpret_cast<uint32_t*>(c.arena[x] + off) + slot * 8 + src;
 }
 
-// All threads call.  Thread t < world, t != rank waits for flags[t] >= seq.  Returns block-uniform ok.
-__device__ __forceinline__ bool block_wait_all(const uint32_t* flags, uint32_t seq, const DevComm& c,
-                                               int phase) {
+// All threads call.  Thread t < world, t != rank waits for own flag [block][t] >= seq of the array at
+// `flag_off`.  Returns block-uniform ok.
+__device__ __forceinline__ bool block_wait_all(size_t flag_off, uint32_t seq, const DevComm& c, WaitPhase phase) {
+  const uint32_t* f = flag_at(c, c.rank, flag_off, blockIdx.x, 0);
   int ok = 1;
   int t = threadIdx.x;
-  if (t < c.world && t != c.rank) ok = wait_flag(flags + t, seq, c, t, phase);
+  if (t < c.world && t != c.rank) ok = wait_flag(f + t, seq, c, t, phase);
   return __syncthreads_and(ok) != 0;
 }
 // wait for a single peer's flag
 __device__ __forceinline__ bool block_wait_one(const uint32_t* flag, uint32_t seq, const DevComm& c, int peer,
-                                               int phase) {
+                                               WaitPhase phase) {
   int ok = 1;
   if (threadIdx.x == 0) ok = wait_flag(flag, seq, c, peer, phase);
   return __syncthreads_and(ok) != 0;
@@ -206,20 +207,37 @@ __device__ __forceinline__ bool block_wait_one(const uint32_t* flag, uint32_t se
 __device__ __forceinline__ void block_signal_all(size_t flag_off, uint32_t seq, const DevComm& c) {
   __syncthreads();
   int t = threadIdx.x;
-  if (t < c.world && t != c.rank) {
-    uint32_t* f = reinterpret_cast<uint32_t*>(c.arena[t] + flag_off) + (size_t)blockIdx.x * 8 + c.rank;
-    st_release_sys(f, seq);
-  }
+  if (t < c.world && t != c.rank) st_release_sys(flag_at(c, t, flag_off, blockIdx.x, c.rank), seq);
 }
 __device__ __forceinline__ void block_signal_one(size_t flag_off, uint32_t seq, const DevComm& c, int peer) {
   __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t* f = reinterpret_cast<uint32_t*>(c.arena[peer] + flag_off) + (size_t)blockIdx.x * 8 + c.rank;
-    st_release_sys(f, seq);
-  }
+  if (threadIdx.x == 0) st_release_sys(flag_at(c, peer, flag_off, blockIdx.x, c.rank), seq);
 }
-__device__ __forceinline__ const uint32_t* my_flags(size_t flag_off, const DevComm& c) {
-  return reinterpret_cast<const uint32_t*>(c.arena[c.rank] + flag_off) + (size_t)blockIdx.x * 8;
+
+// Mismatch detection (diagnostic).  Each rank announces (seq, signature) to every peer in one atomic
+// 8-byte store.  A peer's announcement is compared only if it carries exactly this op's sequence
+// number; anything else (the peer is still behind, or — a producer-only rank such as a broadcast
+// root — already ahead) is not evidence of a mismatch and is ignored, so the check can never raise a
+// false alarm.  On mismatch the communicator is poisoned: the error is recorded and the abort flag
+// raised so this rank's other blocks stop waiting.
+__device__ __forceinline__ void announce_signature(const CollArgs& a, int peer) {
+  const DevComm& c = a.c;
+  unsigned long long* sig = reinterpret_cast<unsigned long long*>(c.arena[peer] + kOffOpSig) + (a.seq & 1) * 8 + c.rank;
+  unsigned long long tagged = ((unsigned long long)a.seq << 32) | a.sig;  // one atomic 8-byte store
+  asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sig), "l"(tagged) : "memory");
+}
+// Compares what `peer` announced with this op; a mismatch is recorded and raises the abort flag.
+__device__ __forceinline__ void compare_signature(const CollArgs& a, int peer, WaitPhase phase) {
+  const DevComm& c = a.c;
+  const unsigned long long* slot = reinterpret_cast<const unsigned long long*>(c.arena[c.rank] + kOffOpSig) + (a.seq & 1) * 8 + peer;
+  unsigned long long v;
+  asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(slot) : "memory");
+  uint32_t s = (uint32_t)v;
+  if ((uint32_t)(v >> 32) == a.seq && s != a.sig) {
+    if (c.status->error == 0) { c.status->err_a = s; c.status->err_b = a.sig; }
+    record_error(c.status, B200C_EMISMATCH, a.seq, peer, phase);
+    c.status->abort_flag = 1;
+  }
 }
 
 // Kernel prologue shared by every collective:
@@ -231,41 +249,54 @@ __device__ __forceinline__ bool coll_prologue(const CollArgs& a) {
   const DevComm& c = a.c;
   int t = threadIdx.x;
   if (blockIdx.x == 0 && t < c.world && t != c.rank) {
-    unsigned long long* sig = reinterpret_cast<unsigned long long*>(c.arena[t] + kOffOpSig) + (a.seq & 1) * 8 + c.rank;
-    unsigned long long tagged = ((unsigned long long)a.seq << 32) | a.sig;  // one atomic 8-byte store
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sig), "l"(tagged) : "memory");
-    uint32_t* arr = reinterpret_cast<uint32_t*>(c.arena[t] + kOffArrive) + c.rank;
-    st_release_sys(arr, a.seq);
+    announce_signature(a, t);
+    st_release_sys(flag_at(c, t, kOffArrive, 0, c.rank), a.seq);
   }
-  const uint32_t* arrive = reinterpret_cast<const uint32_t*>(c.arena[c.rank] + kOffArrive);
+  const uint32_t* arrive = flag_at(c, c.rank, kOffArrive, 0, 0);
   int ok = 1;
-  if (t < c.world && t != c.rank) ok = wait_flag(arrive + t, a.seq - 1, c, t, 0);
+  if (t < c.world && t != c.rank) ok = wait_flag(arrive + t, a.seq - 1, c, t, kWaitArrive);
   return __syncthreads_and(ok) != 0;
 }
-// Mismatch detection (block 0 only, diagnostic).  Each rank announces (seq, signature) to every peer
-// in one atomic 8-byte store.  A peer's announcement is compared only if it carries exactly this
-// op's sequence number; anything else (the peer is still behind, or — a producer-only rank such as
-// a broadcast root — already ahead) is not evidence of a mismatch and is ignored, so the check can
-// never raise a false alarm.  On mismatch the communicator is poisoned: the error is recorded and
-// the abort flag raised so this rank's other blocks stop waiting.
+// Block 0 compares each peer's announcement once that peer has arrived at this op.
 __device__ __forceinline__ void check_signature(const CollArgs& a) {
   const DevComm& c = a.c;
   int t = threadIdx.x;
   if (blockIdx.x == 0 && t < c.world && t != c.rank) {
-    const uint32_t* arrive = reinterpret_cast<const uint32_t*>(c.arena[c.rank] + kOffArrive);
-    if (wait_flag(arrive + t, a.seq, c, t, 0)) {
-      const unsigned long long* slot = reinterpret_cast<const unsigned long long*>(c.arena[c.rank] + kOffOpSig) + (a.seq & 1) * 8 + t;
-      unsigned long long v;
-      asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(slot) : "memory");
-      uint32_t s = (uint32_t)v;
-      if ((uint32_t)(v >> 32) == a.seq && s != a.sig) {
-        if (c.status->error == 0) { c.status->err_a = s; c.status->err_b = a.sig; }
-        record_error(c.status, B200C_EMISMATCH, a.seq, t, 0);
-        c.status->abort_flag = 1;
-      }
-    }
+    if (wait_flag(flag_at(c, c.rank, kOffArrive, 0, t), a.seq, c, t, kWaitArrive)) compare_signature(a, t, kWaitArrive);
   }
 }
+
+// k-th rank after r in ring order (0 <= k < W): the order in which a rank visits its peers
+__device__ __forceinline__ int peer_at(int r, int k, int W) {
+  int j = r + k;
+  if (j >= W) j -= W;
+  return j;
+}
+// clip [lo, hi) against n, return count
+__device__ __forceinline__ size_t clip_count(size_t lo, size_t hi, size_t n) {
+  if (lo >= n) return 0;
+  return (hi < n ? hi : n) - lo;
+}
+struct Span {
+  size_t lo, cnt;
+};
+// granule [g0, g1) of rank chunk j: first element and element count inside the piece (0 past its end)
+__device__ __forceinline__ Span chunk_span(const CollArgs& a, int j, size_t g0, size_t g1) {
+  const size_t lo = (size_t)j * a.chunk + g0;
+  return {lo, clip_count(lo, (size_t)j * a.chunk + g1, a.n)};
+}
+// The granules a block owns in the round-pipelined kernels: round q < count() is the granule [lo(q), hi(q))
+// of every rank chunk, the same granules B200C_FOR_GRANULES walks.  An empty() block owns none.
+struct BlockRounds {
+  const CollArgs& a;
+  size_t first, step;
+  __device__ __forceinline__ explicit BlockRounds(const CollArgs& args)
+      : a(args), first((size_t)blockIdx.x * args.tile), step((size_t)gridDim.x * args.tile) {}
+  __device__ __forceinline__ bool empty() const { return first >= a.chunk; }
+  __device__ __forceinline__ int count() const { return (int)((a.chunk - first + step - 1) / step); }
+  __device__ __forceinline__ size_t lo(int q) const { return first + (size_t)q * step; }
+  __device__ __forceinline__ size_t hi(int q) const { size_t h = first + (size_t)q * step + a.tile; return h < a.chunk ? h : a.chunk; }
+};
 
 // ---------------------------------------------------------------------------------------------
 // dtype traits: R = storage type, A = accumulator type
@@ -314,56 +345,64 @@ template <typename T> union Pack16 {
   __device__ Pack16() {}
 };
 
+// a 16-byte vector of TW, multiplied element-wise by a.scale when the op has one (the NVLS kernels' AVG / mean)
+template <typename TW>
+__device__ __forceinline__ uint4 scale_vector(uint4 v, const CollArgs& a) {
+  if (a.has_scale) {
+    Pack16<TW> p; p.u = v;
+#pragma unroll
+    for (int e = 0; e < 16 / (int)sizeof(TW); e++) p.e[e] = Traits<TW>::from_acc(Traits<TW>::to_acc(p.e[e]) * a.scale);
+    v = p.u;
+  }
+  return v;
+}
+
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // ---------------------------------------------------------------------------------------------
 // tile primitives: the whole block cooperates on `n` contiguous elements.
 // ---------------------------------------------------------------------------------------------
 constexpr int kUnroll = 4;
-#ifndef B200C_CONVERT_UNROLL
-#define B200C_CONVERT_UNROLL 1   // converting copies (float bucket <-> 16-bit wire): vector steps in flight per thread
-#endif
 
 // Plain byte copy of n elements of T.  SRC_BYPASS: source is staging / peer memory.
-// `t` / `nt`: index of the calling thread within, and size of, the group of threads that cooperates
-// on the tile (the whole CTA by default; one warp-specialised role in the pipelined kernels).
 template <typename T, bool SRC_BYPASS>
-__device__ __forceinline__ void copy_tile(T* __restrict__ dst, const T* __restrict__ src, size_t n,
-                                          int t = threadIdx.x, int nt = kThreads) {
+__device__ __forceinline__ void copy_tile(T* __restrict__ dst, const T* __restrict__ src, size_t n) {
   constexpr int V = 16 / sizeof(T);
+  const int t = threadIdx.x;
   if (aligned16(dst) && aligned16(src)) {
     size_t nv = n / V;
     uint4* d = reinterpret_cast<uint4*>(dst);
     const uint4* s = reinterpret_cast<const uint4*>(src);
     size_t i = t;
-    for (; i + (size_t)(kUnroll - 1) * nt < nv; i += (size_t)kUnroll * nt) {
+    for (; i + (size_t)(kUnroll - 1) * kThreads < nv; i += (size_t)kUnroll * kThreads) {
       uint4 v[kUnroll];
 #pragma unroll
-      for (int u = 0; u < kUnroll; u++) v[u] = SRC_BYPASS ? ld_bypass16(s + i + (size_t)u * nt) : s[i + (size_t)u * nt];
+      for (int u = 0; u < kUnroll; u++) v[u] = SRC_BYPASS ? ld_bypass16(s + i + (size_t)u * kThreads) : s[i + (size_t)u * kThreads];
 #pragma unroll
-      for (int u = 0; u < kUnroll; u++) d[i + (size_t)u * nt] = v[u];
+      for (int u = 0; u < kUnroll; u++) d[i + (size_t)u * kThreads] = v[u];
     }
-    for (; i < nv; i += nt) d[i] = SRC_BYPASS ? ld_bypass16(s + i) : s[i];
-    for (size_t k = nv * V + t; k < n; k += nt) dst[k] = SRC_BYPASS ? ld_bypass(src + k) : src[k];
+    for (; i < nv; i += kThreads) d[i] = SRC_BYPASS ? ld_bypass16(s + i) : s[i];
+    for (size_t k = nv * V + t; k < n; k += kThreads) dst[k] = SRC_BYPASS ? ld_bypass(src + k) : src[k];
   } else {
-    for (size_t k = t; k < n; k += nt) dst[k] = SRC_BYPASS ? ld_bypass(src + k) : src[k];
+    for (size_t k = t; k < n; k += kThreads) dst[k] = SRC_BYPASS ? ld_bypass(src + k) : src[k];
   }
 }
 
 // Converting copy TS -> TD through the accumulator domain (fp32 for half types).
 template <typename TS, typename TD, bool SRC_BYPASS>
-__device__ __forceinline__ void convert_tile(TD* __restrict__ dst, const TS* __restrict__ src, size_t n,
-                                             int t = threadIdx.x, int nt = kThreads) {
+__device__ __forceinline__ void convert_tile(TD* __restrict__ dst, const TS* __restrict__ src, size_t n) {
   // vector step = number of elements in 16 bytes of the narrower type
   constexpr int VS = 16 / sizeof(TS), VD = 16 / sizeof(TD);
   constexpr int V = VS > VD ? VS : VD;
+  const int t = threadIdx.x;
   if (aligned16(dst) && aligned16(src)) {
     size_t nv = n / V;
     constexpr int NS = V / VS, ND = V / VD;   // 16-byte loads / stores per vector step
-#if B200C_CONVERT_UNROLL > 1
-    constexpr int U = B200C_CONVERT_UNROLL;   // vector steps in flight per thread
-#endif
-    auto convert_store = [&](const uint4* raw, size_t i) {
+    for (size_t i = t; i < nv; i += kThreads) {
+      uint4 raw[NS];
+      const uint4* s = reinterpret_cast<const uint4*>(src + i * V);
+#pragma unroll
+      for (int q = 0; q < NS; q++) raw[q] = SRC_BYPASS ? ld_bypass16(s + q) : s[q];
       TD dv[V];
 #pragma unroll
       for (int q = 0; q < NS; q++) {
@@ -380,45 +419,36 @@ __device__ __forceinline__ void convert_tile(TD* __restrict__ dst, const TS* __r
         for (int e = 0; e < VD; e++) p.e[e] = dv[q * VD + e];
         d[q] = p.u;
       }
-    };
-    size_t i = t;
-#if B200C_CONVERT_UNROLL > 1
-    for (; i + (size_t)(U - 1) * nt < nv; i += (size_t)U * nt) {
-      uint4 raw[U][NS];
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const uint4* s = reinterpret_cast<const uint4*>(src + (i + (size_t)u * nt) * V);
-#pragma unroll
-        for (int q = 0; q < NS; q++) raw[u][q] = SRC_BYPASS ? ld_bypass16(s + q) : s[q];
-      }
-#pragma unroll
-      for (int u = 0; u < U; u++) convert_store(raw[u], i + (size_t)u * nt);
     }
-#endif
-    for (; i < nv; i += nt) {
-      uint4 raw[NS];
-      const uint4* s = reinterpret_cast<const uint4*>(src + i * V);
-#pragma unroll
-      for (int q = 0; q < NS; q++) raw[q] = SRC_BYPASS ? ld_bypass16(s + q) : s[q];
-      convert_store(raw, i);
-    }
-    for (size_t k = nv * V + t; k < n; k += nt)
+    for (size_t k = nv * V + t; k < n; k += kThreads)
       dst[k] = Traits<TD>::from_acc((typename Traits<TD>::A)Traits<TS>::to_acc(SRC_BYPASS ? ld_bypass(src + k) : src[k]));
   } else {
-    for (size_t k = t; k < n; k += nt)
+    for (size_t k = t; k < n; k += kThreads)
       dst[k] = Traits<TD>::from_acc((typename Traits<TD>::A)Traits<TS>::to_acc(SRC_BYPASS ? ld_bypass(src + k) : src[k]));
   }
 }
 
 template <typename TS, typename TD, bool SRC_BYPASS> struct Mover {
-  static __device__ __forceinline__ void run(TD* dst, const TS* src, size_t n, int t, int nt) { convert_tile<TS, TD, SRC_BYPASS>(dst, src, n, t, nt); }
+  static __device__ __forceinline__ void run(TD* dst, const TS* src, size_t n) { convert_tile<TS, TD, SRC_BYPASS>(dst, src, n); }
 };
 template <typename T, bool SRC_BYPASS> struct Mover<T, T, SRC_BYPASS> {
-  static __device__ __forceinline__ void run(T* dst, const T* src, size_t n, int t, int nt) { copy_tile<T, SRC_BYPASS>(dst, src, n, t, nt); }
+  static __device__ __forceinline__ void run(T* dst, const T* src, size_t n) { copy_tile<T, SRC_BYPASS>(dst, src, n); }
 };
 template <typename TS, typename TD, bool SRC_BYPASS>
-__device__ __forceinline__ void move_tile(TD* dst, const TS* src, size_t n, int t = threadIdx.x, int nt = kThreads) {
-  Mover<TS, TD, SRC_BYPASS>::run(dst, src, n, t, nt);
+__device__ __forceinline__ void move_tile(TD* dst, const TS* src, size_t n) {
+  Mover<TS, TD, SRC_BYPASS>::run(dst, src, n);
+}
+
+// Zero-fills elements [end, end rounded up to the 16-byte vector) of dst when that stays below `limit`, so
+// that the switch reduces defined values in the message's last vector.
+template <typename TW>
+__device__ __forceinline__ void zero_pad_vector(TW* dst, size_t lo, size_t cnt, size_t limit) {
+  constexpr int V = 16 / sizeof(TW);
+  size_t end = lo + cnt, padded = (end + V - 1) / V * V;
+  if (cnt && padded > end && padded <= limit) {
+    TW z = Traits<TW>::from_acc((typename Traits<TW>::A)0);
+    for (size_t k = end + threadIdx.x; k < padded; k += kThreads) dst[k] = z;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -165,6 +165,7 @@ struct b200c_comm {
 };
 
 static size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+static int load_kernels(int device);
 
 // symmetric pool state (see b200c_pool_bind)
 struct PoolBlock { size_t off, len; };
@@ -363,6 +364,8 @@ extern "C" int b200c_comm_create(int rank, int world, int device, const b200c_co
   if (device < 0 || device >= ndev) return fail(B200C_EINVAL, "device %d not visible (count %d)", device, ndev);
   DeviceGuard g(device);
   RT(cudaFree(0));
+  rc = load_kernels(device);
+  if (rc) return rc;
   b200c_comm* c = new b200c_comm();
   c->rank = rank; c->world = world; c->device = device; c->cfg = cfg;
   c->vmm = cfg.share_mode == B200C_SHARE_VMM_FD;
@@ -921,6 +924,56 @@ static int pipeline_setup(b200c_comm* c) {
     RT(cudaEventCreateWithFlags(&c->pe_nv[i], cudaEventDisableTiming));
     RT(cudaEventCreateWithFlags(&c->pe_out[i], cudaEventDisableTiming));
   }
+  return B200C_OK;
+}
+// Lazy module loading (CUDA_MODULE_LOADING=LAZY, torch's default) loads a kernel at its first launch, and the load
+// can wait for the kernels already running in the context.  A kernel that waits for a peer's kernel in the same
+// context -- a receive posted before the matching send on another stream, the ranks of a loopback world -- then
+// waits for a launch that waits for it, until timeout_ms.  So the first communicator of a device loads every kernel
+// that waits for a peer before any of them runs.  (tests/test_gpu_zz_schedules.py posts receives first.)
+static int load_kernels(int device) {
+  static std::mutex mu;
+  static uint32_t loaded = 0;   // bit d: device d is done
+  std::lock_guard<std::mutex> lk(mu);
+  if (device < 32 && ((loaded >> device) & 1)) return B200C_OK;
+  int rc = B200C_OK;
+  auto load = [&](auto kernel) { if (!rc) rc = load_kernel(kernel); };
+  CollArgs a;
+  memset(&a, 0, sizeof a);
+  for (int world : {2, 3, 4, 8}) {   // 3 stands for every world size taken at run time (WT = 0)
+    a.c.world = world;
+    for (int dt = 0; dt < B200C_NUM_DTYPES; dt++)
+      for (int op : {B200C_SUM, B200C_PROD, B200C_MAX, B200C_MIN})
+        if (!rc) rc = launch_same_type(dt, KIND_LOAD, op, a, 0, nullptr);
+    with_world_t(world, [&](auto wt) {
+      constexpr int WT = decltype(wt)::value;
+      load(k_allreduce_oneshot<float, bf16_t, B200C_SUM, WT>);
+      load(k_allreduce_twoshot<float, bf16_t, B200C_SUM, WT>);
+      load(k_allreduce_oneshot<float, f16_t, B200C_SUM, WT>);
+      load(k_allreduce_twoshot<float, f16_t, B200C_SUM, WT>);
+      for (const auto& p : kScaledPairs)
+        with_scaled_types(p[0], p[1], [&](auto ti, auto tw) {
+          load(k_reducescatter_scaled<typename decltype(ti)::type, typename decltype(tw)::type, WT>);
+        });
+    });
+  }
+  for (const auto& p : kScaledPairs)
+    with_scaled_types(p[0], p[1], [&](auto ti, auto tw) {
+      using TI = typename decltype(ti)::type;
+      using TW = typename decltype(tw)::type;
+      load(k_allreduce_nvls<TI, TW>);
+      load(k_allreduce_nvls_rounds<TI, TW>);
+      load(k_allreduce_nvls_lanes<TI, TW>);
+    });
+  load(k_allgather);
+  load(k_broadcast);
+  load(k_broadcast_rounds);
+  load(k_barrier);
+  load(k_send);
+  load(k_send_multi);
+  load(k_recv);
+  if (rc) return fail(rc, "loading the collective kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (device < 32) loaded |= 1u << device;
   return B200C_OK;
 }
 static int barrier_op(b200c_comm* c, cudaStream_t s) {

@@ -19,11 +19,27 @@ static auto with_world_t(int world, F&& f) {
   }
 }
 
-enum Kind { KIND_ONESHOT = 0, KIND_TWOSHOT = 1, KIND_REDUCESCATTER = 2, KIND_REDUCE = 3, KIND_LL = 4 };
+// KIND_LOAD launches nothing: it loads the kernels of every kind for (T, OP, WT) into the context (load_kernels)
+enum Kind { KIND_ONESHOT = 0, KIND_TWOSHOT = 1, KIND_REDUCESCATTER = 2, KIND_REDUCE = 3, KIND_LL = 4, KIND_LOAD = 5 };
+
+// cudaFuncGetAttributes loads a kernel that lazy module loading has not loaded yet
+template <typename K>
+static int load_kernel(K* kernel) {
+  cudaFuncAttributes attr;
+  return cudaFuncGetAttributes(&attr, kernel) == cudaSuccess ? B200C_OK : B200C_ECUDA;
+}
 
 template <typename T, int OP, int WT>
 static int launch_kind_w(int kind, const CollArgs& a, int grid, cudaStream_t s) {
   switch (kind) {
+    case KIND_LOAD: {
+      int rc = load_kernel(k_allreduce_oneshot<T, T, OP, WT>);
+      if (!rc) rc = load_kernel(k_allreduce_twoshot<T, T, OP, WT>);
+      if (!rc) rc = load_kernel(k_reducescatter<T, OP, WT>);
+      if (!rc) rc = load_kernel(k_reduce<T, OP, WT>);
+      if (!rc) rc = load_kernel(k_allreduce_ll<T, OP, WT>);
+      return rc;
+    }
     case KIND_ONESHOT: k_allreduce_oneshot<T, T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;
     case KIND_TWOSHOT: k_allreduce_twoshot<T, T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;
     case KIND_REDUCESCATTER: k_reducescatter<T, OP, WT><<<grid, kThreads, 0, s>>>(a); break;

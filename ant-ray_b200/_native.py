@@ -105,7 +105,9 @@ SYMBOLS = {
     "b200c_debug_fill_flags": (c_int, [c_void_p, c_uint32]),
     "b200c_bn_scratch_bytes": (c_size_t, [c_int]),
     "b200c_bn_forward": (c_int, [c_void_p] * 10 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "b200c_bn_forward_mask": (c_int, [c_void_p] * 11 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_backward": (c_int, [c_void_p] * 10 + [c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_backward_mask": (c_int, [c_void_p] * 11 + [c_int, c_int, c_void_p, c_void_p]),
     "b200c_launch_count": (c_uint64, []),
 }
 

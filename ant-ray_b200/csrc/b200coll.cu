@@ -217,32 +217,73 @@ extern "C" size_t b200c_bn_scratch_bytes(int channels) {
   return channels < 1 || channels > bn::kMaxChannels ? 0 : bn::scratch_bytes(channels);
 }
 
-extern "C" int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
-                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
-                                float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
-                                b200c_stream_t stream) {
+static int bn_forward(const void* x, const void* identity, void* y, void* mask, const float* weight, const float* bias,
+                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                      float* save_invstd, int m, int channels, float momentum, float eps, void* scratch, b200c_stream_t stream) {
   int rc = check_bn_shape(m, channels, scratch);
   if (rc) return rc;
   if (!x || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
     return fail(B200C_EINVAL, "batch norm forward: null buffer");
-  bn::FwdArgs a{x, identity, y, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
+  bn::FwdArgs a{x, identity, y, mask, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
                 save_mean, save_invstd, m, channels, momentum, eps, scratch};
   RT(bn::forward(a, (cudaStream_t)stream));
   g_launches.fetch_add(2);
   return B200C_OK;
 }
 
-extern "C" int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
-                                 const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
-                                 int channels, void* scratch, b200c_stream_t stream) {
+static int bn_backward(const void* dy, const void* dy2, const void* y, const void* mask, const void* x, void* dy_masked,
+                       void* dx, const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
+                       float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream) {
   int rc = check_bn_shape(m, channels, scratch);
   if (rc) return rc;
-  if (!dy || !y || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias)
+  if (!dy || !(y || mask) || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias)
     return fail(B200C_EINVAL, "batch norm backward: null buffer");
-  bn::BwdArgs a{dy, y, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
+  bn::BwdArgs a{dy, dy2, y, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
   RT(bn::backward(a, (cudaStream_t)stream));
   g_launches.fetch_add(2);
   return B200C_OK;
+}
+
+// The mask holds 8 channels per byte of a row, so its calls take C % 8 == 0 only.
+static int check_bn_mask(const void* mask, int channels) {
+  if (!mask) return fail(B200C_EINVAL, "batch norm mask: null mask");
+  if (channels % 8) return fail(B200C_EINVAL, "batch norm mask: channels=%d is not a multiple of 8", channels);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
+                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
+                                b200c_stream_t stream) {
+  return bn_forward(x, identity, y, nullptr, weight, bias, running_mean, running_var, num_batches_tracked, save_mean, save_invstd,
+                    m, channels, momentum, eps, scratch, stream);
+}
+
+extern "C" int b200c_bn_forward_mask(const void* x, const void* identity, void* y, uint8_t* mask, const float* weight,
+                                     const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                                     float* save_mean, float* save_invstd, int m, int channels, float momentum, float eps,
+                                     void* scratch, b200c_stream_t stream) {
+  int rc = check_bn_mask(mask, channels);
+  if (rc) return rc;
+  return bn_forward(x, identity, y, mask, weight, bias, running_mean, running_var, num_batches_tracked, save_mean, save_invstd,
+                    m, channels, momentum, eps, scratch, stream);
+}
+
+extern "C" int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
+                                 const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
+                                 int channels, void* scratch, b200c_stream_t stream) {
+  return bn_backward(dy, nullptr, y, nullptr, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m,
+                     channels, scratch, stream);
+}
+
+extern "C" int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask, const void* x, void* dy_masked,
+                                      void* dx, const float* weight, const float* save_mean, const float* save_invstd,
+                                      float* grad_weight, float* grad_bias, int m, int channels, void* scratch,
+                                      b200c_stream_t stream) {
+  int rc = check_bn_mask(mask, channels);
+  if (rc) return rc;
+  return bn_backward(dy, dy2, nullptr, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m,
+                     channels, scratch, stream);
 }
 
 extern "C" void b200c_default_config(b200c_config_t* cfg) {

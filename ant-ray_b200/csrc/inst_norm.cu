@@ -95,7 +95,9 @@ cudaError_t forward(const FwdArgs& a, cudaStream_t st) {
   ew_config(a.m, a.c, vec, &block, &grid);
   const bf16* id = static_cast<const bf16*>(a.identity);
   bf16* y = static_cast<bf16*>(a.y);
-#define B200C_BN_TRANSFORM(V, R) k_bn_transform<V, R><<<grid, block, 0, st>>>(x, id, y, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c)
+  uint8_t* mask = static_cast<uint8_t*>(a.mask);
+#define B200C_BN_TRANSFORM(V, R) \
+  k_bn_transform<V, R><<<grid, block, 0, st>>>(x, id, y, mask, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c)
   if (vec == kEwVec) {
     if (id) B200C_BN_TRANSFORM(kEwVec, true); else B200C_BN_TRANSFORM(kEwVec, false);
   } else {
@@ -113,23 +115,36 @@ cudaError_t backward(const BwdArgs& a, cudaStream_t st) {
   reduce_config(a.m, a.c, &block, &grid);
   const bf16* x = static_cast<const bf16*>(a.x);
   const bf16* dy = static_cast<const bf16*>(a.dy);
+  const bf16* dy2 = static_cast<const bf16*>(a.dy2);
   const bf16* y = static_cast<const bf16*>(a.y);
+  const uint8_t* mask = static_cast<const uint8_t*>(a.mask);
   bf16* masked = static_cast<bf16*>(a.dy_masked);
-  k_bn_bwd_reduce<<<grid, block, 0, st>>>(x, dy, y, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu, a.grad_weight,
-                                          a.grad_bias, s.staging, s.semaphores, a.m, a.c);
-  const void* ptrs[4] = {a.x, a.dy, a.y, a.dx};
-  const void* mptrs[3] = {a.x, a.dy_masked, a.dx};
-  const int vec = (masked ? vec_ok(a.c, mptrs, 3) : vec_ok(a.c, ptrs, 4)) ? kEwVec : 1;
+  if (mask)
+    k_bn_bwd_reduce<true><<<grid, block, 0, st>>>(x, dy, dy2, y, mask, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu,
+                                                  a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m, a.c);
+  else
+    k_bn_bwd_reduce<false><<<grid, block, 0, st>>>(x, dy, dy2, y, mask, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu,
+                                                   a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m, a.c);
+  // g comes from the tensor the reduce kernel wrote (tail), else from dy and the mask or y
+  const GradSrc src = masked ? kGradMasked : mask ? kGradBits : kGradY;
+  const void* ptrs[5] = {a.x, a.dx, masked ? a.dy_masked : a.dy, dy2 && !masked ? a.dy2 : a.dy, a.y};
+  const int vec = vec_ok(a.c, ptrs, src == kGradY ? 5 : 4) ? kEwVec : 1;
   ew_config(a.m, a.c, vec, &block, &grid);
   const float norm_fct = (float)(1.0 / a.m);
   bf16* dx = static_cast<bf16*>(a.dx);
-#define B200C_BN_ELEMT(V, M, G) \
-  k_bn_bwd_elemt<V, M><<<grid, block, 0, st>>>(G, y, x, dx, a.save_mean, a.save_invstd, a.weight, sum_dy, sum_dy_xmu, norm_fct, a.m, a.c)
+#define B200C_BN_ELEMT(V, S, G) \
+  k_bn_bwd_elemt<V, S><<<grid, block, 0, st>>>(G, dy2, y, mask, x, dx, a.save_mean, a.save_invstd, a.weight, sum_dy, sum_dy_xmu, \
+                                               norm_fct, a.m, a.c)
+#define B200C_BN_ELEMT_SRC(V)                                  \
+  if (src == kGradMasked) B200C_BN_ELEMT(V, kGradMasked, masked); \
+  else if (src == kGradBits) B200C_BN_ELEMT(V, kGradBits, dy);    \
+  else B200C_BN_ELEMT(V, kGradY, dy);
   if (vec == kEwVec) {
-    if (masked) B200C_BN_ELEMT(kEwVec, true, masked); else B200C_BN_ELEMT(kEwVec, false, dy);
+    B200C_BN_ELEMT_SRC(kEwVec)
   } else {
-    if (masked) B200C_BN_ELEMT(1, true, masked); else B200C_BN_ELEMT(1, false, dy);
+    B200C_BN_ELEMT_SRC(1)
   }
+#undef B200C_BN_ELEMT_SRC
 #undef B200C_BN_ELEMT
   return cudaGetLastError();
 }

@@ -269,12 +269,19 @@ __global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restri
 // y = relu(bn(x)) (RESID false) or y = relu(bf16(bn(x)) + identity) (RESID true), rounded where eager torch
 // rounds: the batch-norm output to bf16, the bf16 sum of the residual add to bf16.  `t <= 0 ? 0 : bf16(t)` is
 // relu(bf16(t)) because rounding keeps the sign; NaN passes through as in torch's relu.
+//
+// With `mask` set (C % 8 == 0) the kernel also writes the ReLU's backward predicate !(y <= 0), computed from the
+// stored bf16 y, as one bit per element: element a = m * C + c is bit a % 8 of byte a / 8.  V = 8 threads write
+// one byte each per row.  V = 1 threads pack a byte with a ballot over the 8 lanes of one 8-channel group: block.x
+// = min(C, 256) is then a multiple of 8, so those lanes share a row and are all in or all out of range, and they
+// reach the ballot together or return together.
 template <int V, bool RESID>
 __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restrict__ input, const bf16* __restrict__ identity,
-                                                             bf16* __restrict__ out, const float* __restrict__ mean,
-                                                             const float* __restrict__ inv_std, const float* __restrict__ weight,
-                                                             const float* __restrict__ shift, const int reduction_size,
-                                                             const int stride) {
+                                                             bf16* __restrict__ out, uint8_t* __restrict__ mask,
+                                                             const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                             const float* __restrict__ weight, const float* __restrict__ shift,
+                                                             const int reduction_size, const int stride) {
+  static_assert(V == 1 || V == 8, "a thread writes a whole mask byte (V = 8) or one bit of a ballot (V = 1)");
   const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   if (c0 >= stride) return;
   float m_c[V], inv_std_c[V], w_c[V], s_c[V];
@@ -285,6 +292,8 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
     w_c[j] = weight[c0 + j];
     s_c[j] = shift[c0 + j];
   }
+  const unsigned lane = (threadIdx.x + threadIdx.y * blockDim.x) % 32;
+  const unsigned group = 0xffu << (lane & ~7u);
   const int row_step = blockDim.y * gridDim.y;
   for (int m = blockIdx.y * blockDim.y + threadIdx.y; m < reduction_size; m += row_step) {
     const int a = m * stride + c0;
@@ -292,6 +301,7 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
     BVec<V> zv;
     if (RESID) zv = *reinterpret_cast<const BVec<V>*>(identity + a);
     BVec<V> yv;
+    unsigned bits = 0;
 #pragma unroll
     for (int j = 0; j < V; j++) {
       auto tmp = w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j];
@@ -301,23 +311,36 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
       } else {
         yv.v[j] = tmp <= 0.f ? __float2bfloat16(0.f) : __float2bfloat16(tmp);
       }
+      bits |= (unsigned)!(__bfloat162float(yv.v[j]) <= 0.f) << j;
     }
     *reinterpret_cast<BVec<V>*>(out + a) = yv;
+    if (mask) {
+      if (V == 1) bits = (__ballot_sync(group, bits) >> (lane & ~7u)) & 0xffu;
+      if (V == 8 || lane % 8 == 0) mask[a >> 3] = (uint8_t)bits;
+    }
   }
 }
 
-// The ReLU's backward (threshold_backward: y <= 0 ? 0 : dy), read from dy and the saved output y.
+// The ReLU's backward (threshold_backward: y <= 0 ? 0 : dy), read from dy and the saved output y, or from dy and
+// the predicate !(y <= 0) that k_bn_transform wrote as a bit.
 __device__ __forceinline__ bf16 relu_grad(bf16 dy, bf16 y) { return __bfloat162float(y) <= 0.f ? __float2bfloat16(0.f) : dy; }
+__device__ __forceinline__ bf16 relu_grad_bit(bf16 dy, unsigned bit) { return bit ? dy : __float2bfloat16(0.f); }
+// autograd's sum of two gradients of one bf16 tensor
+__device__ __forceinline__ bf16 add_grads(bf16 a, bf16 b) { return __float2bfloat16(__bfloat162float(a) + __bfloat162float(b)); }
 
 // Per-channel sums of g and g * (x - mean) with g = relu_grad(dy, y) (torch:
-// batch_norm_backward_reduce_channels_last_kernel<4>), and dweight / dbias.  With `masked` set (the block tail,
-// where g is also the identity branch's gradient) g is written there as well.  As in k_bn_stats, all rows of an
-// iteration are loaded before the first sum uses one.
-__global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output, const bf16* __restrict__ output,
-                                bf16* __restrict__ masked, const float* __restrict__ mean, const float* __restrict__ inv_std,
-                                float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o, float* __restrict__ grad_weight,
-                                float* __restrict__ grad_bias, volatile float* staging_data, int* semaphores,
-                                const int reduction_size, const int stride) {
+// batch_norm_backward_reduce_channels_last_kernel<4>), and dweight / dbias.  BITS reads the ReLU's predicate from
+// `mask` (k_bn_transform's bits) instead of y from `output`.  With `grad_output2` set, dy is the bf16 sum of the
+// two gradients, as autograd rounds it when a tensor has two consumers; without it dy is taken as it is, so a
+// -0.0 gradient stays -0.0.  With `masked` set (the block tail, where g is also the identity branch's gradient) g
+// is written there as well.  As in k_bn_stats, all rows of an iteration are loaded before the first sum uses one.
+template <bool BITS>
+__global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
+                                const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
+                                const uint8_t* __restrict__ mask, bf16* __restrict__ masked, const float* __restrict__ mean,
+                                const float* __restrict__ inv_std, float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
+                                float* __restrict__ grad_weight, float* __restrict__ grad_bias, volatile float* staging_data,
+                                int* semaphores, const int reduction_size, const int stride) {
   constexpr int PARALLEL_LOADS = kParallelLoads;
   float sum_dy[PARALLEL_LOADS];
   float sum_dy_xmu[PARALLEL_LOADS];
@@ -338,13 +361,16 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
   auto factor = inv_std[c_offset];
 
   for (int i = 0; i < loop_count; i++) {
-    bf16 dy_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS];
+    bf16 dy_v[PARALLEL_LOADS], dy2_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS];
+    uint8_t mask_v[PARALLEL_LOADS];
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (m_offset + j * inner_loop_stride < reduction_size) {
         const int a = address_base + j * address_increment;
         dy_v[j] = grad_output[a];
-        y_v[j] = output[a];
+        if (grad_output2) dy2_v[j] = grad_output2[a];
+        if (BITS) mask_v[j] = mask[a >> 3];
+        else y_v[j] = output[a];
         x_v[j] = input[a];
       }
     }
@@ -353,7 +379,8 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (c_offset < stride && m_offset < reduction_size) {
-        const bf16 g = relu_grad(dy_v[j], y_v[j]);
+        const bf16 dy = grad_output2 ? add_grads(dy_v[j], dy2_v[j]) : dy_v[j];
+        const bf16 g = BITS ? relu_grad_bit(dy, (mask_v[j] >> (address_base & 7)) & 1u) : relu_grad(dy, y_v[j]);
         if (masked) masked[address_base] = g;
         x_input[j] = __bfloat162float(x_v[j]);
         x_grad_output[j] = __bfloat162float(g);
@@ -425,10 +452,16 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
   }
 }
 
-// dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g = relu_grad(dy, y) (MASKED false) or g
-// read from the tensor the reduce kernel wrote (MASKED true).
-template <int V, bool MASKED>
-__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restrict__ grad_output, const bf16* __restrict__ output,
+// Where the backward elementwise kernel takes g from: the tensor the reduce kernel wrote (kGradMasked), or
+// relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits).
+enum GradSrc { kGradMasked, kGradY, kGradBits };
+
+// dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g from G; dy is summed with `grad_output2`
+// when that is set, as in k_bn_bwd_reduce.
+template <int V, GradSrc G>
+__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restrict__ grad_output,
+                                                             const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
+                                                             const uint8_t* __restrict__ mask,
                                                              const bf16* __restrict__ input, bf16* __restrict__ grad_input,
                                                              const float* __restrict__ mean, const float* __restrict__ inv_std,
                                                              const float* __restrict__ weight, const float* __restrict__ sum_dy,
@@ -449,13 +482,17 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restr
   for (int m = blockIdx.y * blockDim.y + threadIdx.y; m < reduction_size; m += row_step) {
     const int a = m * stride + c0;
     const BVec<V> gv = *reinterpret_cast<const BVec<V>*>(grad_output + a);
-    BVec<V> yv;
-    if (!MASKED) yv = *reinterpret_cast<const BVec<V>*>(output + a);
+    BVec<V> gv2, yv;
+    if (G != kGradMasked && grad_output2) gv2 = *reinterpret_cast<const BVec<V>*>(grad_output2 + a);
+    unsigned bits = 0;
+    if (G == kGradY) yv = *reinterpret_cast<const BVec<V>*>(output + a);
+    if (G == kGradBits) bits = mask[a >> 3] >> (a & 7);
     const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
     BVec<V> dxv;
 #pragma unroll
     for (int j = 0; j < V; j++) {
-      const float g = __bfloat162float(MASKED ? gv.v[j] : relu_grad(gv.v[j], yv.v[j]));
+      const bf16 dy = G != kGradMasked && grad_output2 ? add_grads(gv.v[j], gv2.v[j]) : gv.v[j];
+      const float g = __bfloat162float(G == kGradMasked ? dy : G == kGradY ? relu_grad(dy, yv.v[j]) : relu_grad_bit(dy, (bits >> j) & 1u));
       dxv.v[j] = __float2bfloat16((g - m_dy_c[j] - (__bfloat162float(xv.v[j]) - m_c[j]) * factor_1_c[j]) * factor_2_c[j]);
     }
     *reinterpret_cast<BVec<V>*>(grad_input + a) = dxv;

@@ -10,6 +10,7 @@ struct FwdArgs {
   const void* x;         // bf16 [m][c]
   const void* identity;  // bf16 [m][c], or null: no residual add
   void* y;               // bf16 [m][c]
+  void* mask;            // uint8 [m * c / 8], or null: receives the ReLU's predicate, one bit per element (c % 8 == 0)
   const float* weight;
   const float* bias;
   float* running_mean;
@@ -24,7 +25,9 @@ struct FwdArgs {
 
 struct BwdArgs {
   const void* dy;        // bf16 [m][c], gradient of the ReLU's output
-  const void* y;         // bf16 [m][c], the ReLU's output
+  const void* dy2;       // bf16 [m][c], or null: a second gradient of the ReLU's output, added to dy
+  const void* y;         // bf16 [m][c], the ReLU's output (read when mask is null)
+  const void* mask;      // uint8 [m * c / 8], or null: the forward's mask, read instead of y (c % 8 == 0)
   const void* x;         // bf16 [m][c], the batch norm's input
   void* dy_masked;       // bf16 [m][c], or null: receives the ReLU's input gradient (residual site)
   void* dx;              // bf16 [m][c]

@@ -29,6 +29,8 @@ _lib = None
 _scratch = {}
 _scratch_need = {}   # channels -> b200c_bn_scratch_bytes(channels); 0: more channels than the kernels take
 _NATIVE = torch._C._BatchNormBackend.Native
+# the current stream's handle without building a torch.cuda.Stream object: each step makes 98 fused calls
+_raw_stream = torch._C._cuda_getCurrentRawStream
 
 
 def _native_lib():
@@ -56,43 +58,64 @@ def _scratch_ptr(device, stream, channels):
 
 
 class _FusedBatchNorm(torch.autograd.Function):
-    """relu(bn(x)) or, with `identity`, relu(bn(x) + identity) in training mode."""
+    """relu(bn(x)) or, with `identity`, relu(bn(x) + identity) in training mode.
+
+    With `pair` the output is returned twice, as y and a view of it, for a block tail whose output feeds both
+    branches of the next block: autograd then hands the backward the two branches' gradients apart (None for an
+    unused one), and the kernel sums them as autograd would.  Where C % 8 == 0 the forward writes the ReLU's mask
+    as bits and the backward reads those instead of y."""
 
     @staticmethod
-    def forward(ctx, x, identity, weight, bias, bn):
+    def forward(ctx, x, identity, weight, bias, bn, pair):
         lib = _native_lib()
         c = x.shape[1]
         m = x.numel() // c
         y = torch.empty_like(x)
         stats = torch.empty(2, c, dtype=torch.float32, device=x.device)
-        stream = torch.cuda.current_stream(x.device).cuda_stream
+        stream = _raw_stream(x.device.index)
         nbt = bn.num_batches_tracked
-        N.check(lib.b200c_bn_forward(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
-                                     weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                                     nbt.data_ptr() if nbt is not None else None, stats[0].data_ptr(), stats[1].data_ptr(),
-                                     m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, c), stream))
-        ctx.save_for_backward(x, y, weight, stats)
+        mean = stats.data_ptr()   # stats = [save_mean; save_invstd]
+        args = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c,
+                m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, c), stream)
+        id_ptr = identity.data_ptr() if identity is not None else None
+        if c % 8 == 0:
+            relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device)
+            N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), relu_src.data_ptr(), *args))
+        else:
+            relu_src = y
+            N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *args))
+        ctx.save_for_backward(x, relu_src, weight, stats)
         ctx.residual = identity is not None
-        return y
+        ctx.set_materialize_grads(False)
+        return (y, y.view_as(y)) if pair else y
 
     @staticmethod
     @once_differentiable
-    def backward(ctx, dy):
+    def backward(ctx, *grads):
+        grads = [g.contiguous(memory_format=torch.channels_last) for g in grads if g is not None]
+        if not grads:
+            return None, None, None, None, None, None
         lib = _native_lib()
-        x, y, weight, stats = ctx.saved_tensors
-        dy = dy.contiguous(memory_format=torch.channels_last)
+        x, relu_src, weight, stats = ctx.saved_tensors
         c = x.shape[1]
         m = x.numel() // c
         dx = torch.empty_like(x)
         d_identity = torch.empty_like(x) if ctx.residual else None
         grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
         grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-        N.check(lib.b200c_bn_backward(dy.data_ptr(), y.data_ptr(), x.data_ptr(),
-                                      d_identity.data_ptr() if d_identity is not None else None, dx.data_ptr(),
-                                      weight.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), grad_weight.data_ptr(),
-                                      grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, c), stream))
-        return dx, d_identity, grad_weight, grad_bias, None
+        stream = _raw_stream(x.device.index)
+        mean = stats.data_ptr()
+        args = (x.data_ptr(), d_identity.data_ptr() if d_identity is not None else None, dx.data_ptr(), weight.data_ptr(),
+                mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, c),
+                stream)
+        if relu_src.dtype == torch.uint8:
+            dy2 = grads[1].data_ptr() if len(grads) == 2 else None
+            N.check(lib.b200c_bn_backward_mask(grads[0].data_ptr(), dy2, relu_src.data_ptr(), *args))
+        else:
+            dy = grads[0] + grads[1] if len(grads) == 2 else grads[0]
+            N.check(lib.b200c_bn_backward(dy.data_ptr(), relu_src.data_ptr(), *args))
+        return dx, d_identity, grad_weight, grad_bias, None, None
 
 
 def _activation(t):
@@ -122,17 +145,30 @@ def _fusable(bn, relu, x):
 def bn_relu(bn, relu, x):
     """relu(bn(x)), fused when the site allows it."""
     if _fusable(bn, relu, x):
-        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn)
+        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False)
     return relu(bn(x))
 
 
-def bn_add_relu(bn, relu, x, identity):
-    """`out = bn(x); out += identity; relu(out)`, fused when the site allows it."""
+def bn_add_relu(bn, relu, x, identity, pair=False):
+    """`out = bn(x); out += identity; relu(out)`, fused when the site allows it.  With `pair`, returns `(out,
+    out_id)`: the same values, whose gradients a fused site receives apart and sums in its backward kernel."""
     if _fusable(bn, relu, x) and _activation(identity) and identity.shape == x.shape:
-        return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn)
+        return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair)
     out = bn(x)
     out += identity
-    return relu(out)
+    out = relu(out)
+    return (out, out) if pair else out
+
+
+def _hooked(mod):
+    return bool(mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks)
+
+
+def _global_hooks():
+    from torch.nn.modules import module
+
+    return bool(module._global_forward_hooks or module._global_forward_pre_hooks or module._global_backward_hooks
+                or module._global_backward_pre_hooks)
 
 
 try:
@@ -141,32 +177,54 @@ except ImportError:  # without torchvision there is nothing to rewrite
     _SWAP = {}
 else:
 
+    # A block's input x feeds conv1 and the identity branch.  forward_pair(x, x_id) -> (out, out_id) takes the two
+    # as separate tensors and returns its output twice, so that chained blocks hand each tail's backward the two
+    # gradients of its output apart, to be summed inside the kernel instead of by a separate add.
+
     class FusedBasicBlock(BasicBlock):
         def forward(self, x):
             if not self.training:
                 return super().forward(x)
+            return self.forward_pair(x, x)[0]
+
+        def forward_pair(self, x, x_id):
             out = bn_relu(self.bn1, self.relu, self.conv1(x))
             out = self.conv2(out)
-            identity = self.downsample(x) if self.downsample is not None else x
-            return bn_add_relu(self.bn2, self.relu, out, identity)
+            identity = self.downsample(x_id) if self.downsample is not None else x_id
+            return bn_add_relu(self.bn2, self.relu, out, identity, pair=True)
 
     class FusedBottleneck(Bottleneck):
         def forward(self, x):
             if not self.training:
                 return super().forward(x)
+            return self.forward_pair(x, x)[0]
+
+        def forward_pair(self, x, x_id):
             out = bn_relu(self.bn1, self.relu, self.conv1(x))
             out = bn_relu(self.bn2, self.relu, self.conv2(out))
             out = self.conv3(out)
-            identity = self.downsample(x) if self.downsample is not None else x
-            return bn_add_relu(self.bn3, self.relu, out, identity)
+            identity = self.downsample(x_id) if self.downsample is not None else x_id
+            return bn_add_relu(self.bn3, self.relu, out, identity, pair=True)
+
+    def _pairwise(layer):
+        """Whether `layer`'s blocks can be chained through forward_pair: a plain Sequential of fused blocks, where
+        calling forward_pair directly skips no module hook."""
+        return (type(layer) is nn.Sequential and not _hooked(layer)
+                and all(type(b) in (FusedBasicBlock, FusedBottleneck) and not _hooked(b) for b in layer))
 
     class FusedResNet(ResNet):
         def forward(self, x):
             if not self.training:
                 return super().forward(x)
             x = bn_relu(self.bn1, self.relu, self.conv1(x))
-            x = self.maxpool(x)
-            x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+            x = x_id = self.maxpool(x)   # the maxpool output's two gradients are summed by autograd
+            hooks = _global_hooks()
+            for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
+                if not hooks and _pairwise(layer):
+                    for block in layer:
+                        x, x_id = block.forward_pair(x, x_id)
+                else:
+                    x = x_id = layer(x)
             x = torch.flatten(self.avgpool(x), 1)
             return self.fc(x)
 

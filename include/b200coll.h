@@ -296,15 +296,30 @@ int b200c_debug_fill_flags(b200c_comm_t* comm, uint32_t value);
  * Forward: writes y, save_mean, save_invstd (1 / sqrt(biased var + eps)), updates running_mean / running_var
  * with `momentum` (unbiased variance) and adds 1 to *num_batches_tracked (may be NULL).  2 kernels.
  * Backward: from dy (the gradient of y), y and x writes dx, grad_weight and grad_bias; `dy_masked` (may be NULL)
- * receives the gradient of the ReLU's input, the identity branch's gradient.  2 kernels. */
+ * receives the gradient of the ReLU's input, the identity branch's gradient.  2 kernels.
+ *
+ * The _mask variants (channels % 8 == 0 only; EINVAL otherwise, and for a NULL mask) replace the backward's
+ * 2-byte read of y by a 1-bit read.  Forward: as b200c_bn_forward, and also writes `mask`, m * channels / 8 bytes:
+ * element e = row * channels + channel is bit e % 8 of byte e / 8, set where y > 0 or y is NaN (the ReLU passes
+ * the gradient).  Backward: as b200c_bn_backward with that mask in place of y.  `dy2` (may be NULL) is a second
+ * gradient of y, for a y with two consumers: the kernels use bf16(float(dy) + float(dy2)), autograd's sum of the
+ * two; with dy2 NULL, dy is used as it is.  2 kernels each.  b200c_bn_forward and b200c_bn_backward run the same
+ * kernels without a mask and without dy2. */
 size_t b200c_bn_scratch_bytes(int channels);
 int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
                      float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
                      b200c_stream_t stream);
+int b200c_bn_forward_mask(const void* x, const void* identity, void* y, uint8_t* mask, const float* weight,
+                          const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                          float* save_mean, float* save_invstd, int m, int channels, float momentum, float eps,
+                          void* scratch, b200c_stream_t stream);
 int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
                       const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
                       int channels, void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask, const void* x, void* dy_masked, void* dx,
+                           const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
+                           float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream);
 
 /* Launch statistics (bench.py's gpu_launches claim). */
 uint64_t b200c_launch_count(void);

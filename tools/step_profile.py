@@ -44,23 +44,25 @@ FAMILIES = [
 ]
 
 # bytes each family's kernels move per element of a batch-norm site, by site kind (relu: BN -> ReLU; tail:
-# BN -> += identity -> ReLU; plain: downsample BN, always torch's kernels)
+# BN -> += identity -> ReLU whose output feeds another block; last_tail: the tail that feeds the pooling; plain:
+# downsample BN, always torch's kernels)
 TORCH_BYTES = {  # family -> {kind: bytes per element}
-    "bn_stats_torch": {"relu": 2, "tail": 2, "plain": 2},
-    "bn_transform": {"relu": 4, "tail": 4, "plain": 4},
-    "relu": {"relu": 4, "tail": 4},
-    "add": {"tail": 6},
-    "threshold_backward": {"relu": 6, "tail": 6},
-    "bn_bwd_reduce_torch": {"relu": 4, "tail": 4, "plain": 4},
-    "bn_bwd_elemt": {"relu": 6, "tail": 6, "plain": 6},
+    "bn_stats_torch": {"relu": 2, "tail": 2, "last_tail": 2, "plain": 2},
+    "bn_transform": {"relu": 4, "tail": 4, "last_tail": 4, "plain": 4},
+    "relu": {"relu": 4, "tail": 4, "last_tail": 4},
+    "add": {"tail": 6, "last_tail": 6},
+    "threshold_backward": {"relu": 6, "tail": 6, "last_tail": 6},
+    "bn_bwd_reduce_torch": {"relu": 4, "tail": 4, "last_tail": 4, "plain": 4},
+    "bn_bwd_elemt": {"relu": 6, "tail": 6, "last_tail": 6, "plain": 6},
 }
+# the fused sites' ReLU mask is 1 bit (1/8 byte) per element
 FUSED_BYTES = {
-    "bn_stats": {"relu": 2, "tail": 2},
+    "bn_stats": {"relu": 2, "tail": 2, "last_tail": 2},
     "bn_stats_torch": {"plain": 2},
-    "bn_transform": {"relu": 4, "tail": 6, "plain": 4},              # tail: x, identity -> y
-    "bn_bwd_reduce": {"relu": 6, "tail": 8},                         # dy, y, x (tail: -> dy')
+    "bn_transform": {"relu": 4.125, "tail": 6.125, "last_tail": 6.125, "plain": 4},   # x (, identity) -> y, mask
+    "bn_bwd_reduce": {"relu": 4.125, "tail": 8.125, "last_tail": 6.125},            # dy (, dy2), mask, x (tail: -> dy')
     "bn_bwd_reduce_torch": {"plain": 4},
-    "bn_bwd_elemt": {"relu": 8, "tail": 6, "plain": 6},              # dy, y, x -> dx (tail: dy', x -> dx)
+    "bn_bwd_elemt": {"relu": 6.125, "tail": 6, "last_tail": 6, "plain": 6},         # dy, mask, x -> dx (tail: dy', x -> dx)
 }
 
 
@@ -76,6 +78,7 @@ def bn_sites(batch):
             kinds.update({id(mod.bn1): "relu", id(mod.bn2): "relu", id(mod.bn3): "tail"})
             if mod.downsample is not None:
                 kinds[id(mod.downsample[1])] = "plain"
+    kinds[id(model.layer4[-1].bn3)] = "last_tail"
     sites = []
     hooks = [m.register_forward_pre_hook(lambda m, a: sites.append((kinds[id(m)], a[0].numel() * batch)))
              for m in model.modules() if isinstance(m, torch.nn.BatchNorm2d)]
@@ -181,7 +184,7 @@ def main():
     out = {"mode": "unfused" if args.unfused else "fused", "batch": args.batch, "steps": args.steps,
            "ms_per_step": round(ms / args.steps, 3), "kernel_ms_per_step": round(total, 3),
            "images_per_sec": round(args.batch * args.steps / (ms / 1e3), 1), **gpu_identity(), "families": fams,
-           "bn_site_elements": {k: sum(e for kind, e in sites if kind == k) for k in ("relu", "tail", "plain")}}
+           "bn_site_elements": {k: sum(e for kind, e in sites if kind == k) for k in ("relu", "tail", "last_tail", "plain")}}
     os.makedirs(args.out, exist_ok=True)
     path = os.path.join(args.out, f"step_profile_{out['mode']}.json")
     with open(path, "w") as f:

@@ -971,7 +971,8 @@ static int pipeline_setup(b200c_comm* c) {
 // can wait for the kernels already running in the context.  A kernel that waits for a peer's kernel in the same
 // context -- a receive posted before the matching send on another stream, the ranks of a loopback world -- then
 // waits for a launch that waits for it, until timeout_ms.  So the first communicator of a device loads every kernel
-// that waits for a peer before any of them runs.  (tests/test_gpu_zz_schedules.py posts receives first.)
+// that waits for a peer before any of them runs, and the batch-norm kernels that a sync batch norm launches between
+// its collectives.  (tests/test_gpu_zz_schedules.py posts receives first.)
 static int load_kernels(int device) {
   static std::mutex mu;
   static uint32_t loaded = 0;   // bit d: device d is done
@@ -1013,6 +1014,8 @@ static int load_kernels(int device) {
   load(k_send);
   load(k_send_multi);
   load(k_recv);
+  // the sync batch norm's kernels run between collectives on the ranks' streams
+  if (!rc && bn::load_kernels() != cudaSuccess) rc = B200C_ECUDA;
   if (rc) return fail(rc, "loading the collective kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
   if (device < 32) loaded |= 1u << device;
   return B200C_OK;
@@ -1433,6 +1436,74 @@ extern "C" int b200c_allgather(b200c_comm_t* c, const void* send, void* const* r
     k_allgather<<<grid, kThreads, 0, s>>>(a);
     return B200C_OK;
   });
+}
+
+// ------------------------------------------------------------------------------------------------
+// sync batch norm: the local batch-norm phases (inst_norm.cu) around b200c_allgather and b200c_allreduce
+// ------------------------------------------------------------------------------------------------
+extern "C" size_t b200c_bn_sync_scratch_bytes(int channels, int world) {
+  return channels < 1 || channels > bn::kMaxChannels || world < 1 || world > kMaxRanks ? 0 : bn::sync_scratch_bytes(channels, world);
+}
+
+// Checks shared by both directions; m = 0 is a rank without rows.  A plain site (relu == 0) has no identity, no
+// mask and no second gradient.
+static int check_bn_sync(int m, int c, const void* scratch, int relu, const void* mask, const void* identity, const void* dy2) {
+  if (m < 0 || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX)
+    return fail(B200C_EINVAL, "sync batch norm: bad shape m=%d c=%d", m, c);
+  if (!scratch) return fail(B200C_EINVAL, "sync batch norm: null scratch");
+  if (!relu && (mask || identity || dy2)) return fail(B200C_EINVAL, "sync batch norm: a site without ReLU takes no mask, identity or dy2");
+  if (mask && c % 8) return fail(B200C_EINVAL, "sync batch norm mask: channels=%d is not a multiple of 8", c);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_sync_forward(b200c_comm_t* comm, const void* x, const void* identity, void* y, uint8_t* mask, int relu,
+                                     const float* weight, const float* bias, float* running_mean, float* running_var,
+                                     int64_t* num_batches_tracked, float* save_mean, float* save_invstd, float* norm_fct, int m,
+                                     int channels, float momentum, float eps, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn_sync(m, channels, scratch, relu, mask, identity, nullptr);
+  if (rc) return rc;
+  if ((m && (!x || !y)) || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !norm_fct)
+    return fail(B200C_EINVAL, "sync batch norm forward: null buffer");
+  rc = check_ready(comm);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard g(comm->device);
+  bn::FwdArgs a{x, identity, y, mask, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
+                save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  g_launches.fetch_add(bn::sync_stats(a, s));
+  RT(cudaGetLastError());
+  const bn::SyncRows r = bn::sync_rows(scratch, channels);
+  void* gathered[kMaxRanks];
+  for (int j = 0; j < comm->world; j++) gathered[j] = r.gathered + j * r.row_floats;
+  rc = b200c_allgather(comm, r.local, gathered, (size_t)2 * channels + 1, B200C_FLOAT32, stream);
+  if (rc) return rc;
+  g_launches.fetch_add(bn::sync_apply(a, relu != 0, comm->world, norm_fct, s));
+  RT(cudaGetLastError());
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_sync_backward(b200c_comm_t* comm, const void* dy, const void* dy2, const void* y, const uint8_t* mask, int relu,
+                                      const void* x, void* dy_masked, void* dx, const float* weight, const float* save_mean,
+                                      const float* save_invstd, const float* norm_fct, float* grad_weight, float* grad_bias, int m,
+                                      int channels, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn_sync(m, channels, scratch, relu, mask, dy_masked, dy2);
+  if (rc) return rc;
+  if ((m && (!dy || !x || !dx || (relu && !y && !mask))) || !weight || !save_mean || !save_invstd || !norm_fct || !grad_weight ||
+      !grad_bias)
+    return fail(B200C_EINVAL, "sync batch norm backward: null buffer");
+  rc = check_ready(comm);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard g(comm->device);
+  bn::BwdArgs a{dy, dy2, y, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
+  g_launches.fetch_add(bn::sync_bwd_reduce(a, relu != 0, s));
+  RT(cudaGetLastError());
+  float* sums = bn::sync_rows(scratch, channels).sums;
+  rc = b200c_allreduce(comm, sums, sums, (size_t)2 * channels, B200C_FLOAT32, B200C_SUM, B200C_ALGO_AUTO, stream);
+  if (rc) return rc;
+  g_launches.fetch_add(bn::sync_bwd_elemt(a, relu != 0, norm_fct, s));
+  RT(cudaGetLastError());
+  return B200C_OK;
 }
 
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {

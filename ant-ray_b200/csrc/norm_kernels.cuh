@@ -131,17 +131,17 @@ __device__ __forceinline__ void finish_stats(const StatsOut& o, int c, float mea
   o.save_invstd[c] = rsqrtf(var + o.eps);
 }
 
-// Welford statistics per channel (torch: batch_norm_collect_statistics_channels_last_kernel<Var, ..., 4>), then
-// the running-statistics update and inversion by the thread that owns the channel's final value.  The last block
-// of each column leaves its semaphore at zero for the next call.
+// Welford statistics per channel (torch: batch_norm_collect_statistics_channels_last_kernel<..., 4>), ending in
+// finish(c, mean, m2n, count) by the thread that owns channel c's final value.  The last block of each column
+// leaves its semaphore at zero for the next call.
 //
 // Each of torch's threads walks rows m_offset + r * inner_loop_stride into PARALLEL_LOADS accumulators, one
 // iteration of PARALLEL_LOADS rows at a time.  Here all rows of an iteration are loaded (V channels in one load)
 // before the first update, so that they are in flight together; torch's kernel waits for each row's value before it
 // loads the next.  The V channels of a thread share each row's validity, hence count[j] and its reciprocal.
-template <int V>
-__global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile float* staging_data,
-                                                            int* semaphores, const int reduction_size, const int stride) {
+template <int V, typename Finish>
+__device__ __forceinline__ void bn_stats_body(const bf16* __restrict__ input, volatile float* staging_data, int* semaphores,
+                                              const int reduction_size, const int stride, Finish finish) {
   constexpr int PARALLEL_LOADS = kParallelLoads;
   float x_mean[PARALLEL_LOADS][V];
   float m_2_n[PARALLEL_LOADS][V];
@@ -155,8 +155,6 @@ __global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restri
     }
     count[i] = 0;
   }
-  if (o.num_batches_tracked && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0)
-    *o.num_batches_tracked += 1;
 
   int inner_loop_stride = blockDim.y * gridDim.y;
   int m_offset = blockIdx.y * blockDim.y + threadIdx.y;
@@ -257,12 +255,115 @@ __global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restri
       welford_merge_block_vertical<V>(count_th, mean_th, m2_th, shmem_count, shmem_mean, shmem_m2n);
       if (threadIdx.y == 0 && c_valid)
 #pragma unroll
-        for (int k = 0; k < V; k++) finish_stats(o, c_offset + k, mean_th[k], m2_th[k], count_th[k]);
+        for (int k = 0; k < V; k++) finish(c_offset + k, mean_th[k], m2_th[k], count_th[k]);
     }
   } else {
     if (blockIdx.y == 0 && threadIdx.y == 0 && c_valid)
 #pragma unroll
-      for (int k = 0; k < V; k++) finish_stats(o, c_offset + k, mean_th[k], m2_th[k], count_th[k]);
+      for (int k = 0; k < V; k++) finish(c_offset + k, mean_th[k], m2_th[k], count_th[k]);
+  }
+}
+
+// Local batch norm: the statistics, then the running-statistics update and inversion (finish_stats).
+template <int V>
+__global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restrict__ input, StatsOut o, volatile float* staging_data,
+                                                            int* semaphores, const int reduction_size, const int stride) {
+  if (o.num_batches_tracked && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0)
+    *o.num_batches_tracked += 1;
+  bn_stats_body<V>(input, staging_data, semaphores, reduction_size, stride,
+                   [&](int c, float mean, float m2n, int count) { finish_stats(o, c, mean, m2n, count); });
+}
+
+// ---- sync batch norm (torch.nn.SyncBatchNorm's autograd function) ----
+// A rank's statistics travel as one row [mean (C) | invstd (C) | count] of fp32, as in torch's all_gather.
+
+// torch.batch_norm_stats: the same statistics, ending in torch's InvStd transform instead of Var.  InvStd computes
+// in double: invstd = (var != 0 || eps != 0) ? 1 / sqrt(var + (double)eps) : 0, where eps is the kernel's fp32
+// copy.  Writes this rank's row `local`, with count = (float)m; no running statistics.
+template <int V>
+__global__ void __launch_bounds__(kMaxBlock / V) k_bn_sync_stats(const bf16* __restrict__ input, float* __restrict__ local,
+                                                                 const float eps, volatile float* staging_data, int* semaphores,
+                                                                 const int reduction_size, const int stride) {
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0) local[2 * stride] = (float)reduction_size;
+  bn_stats_body<V>(input, staging_data, semaphores, reduction_size, stride, [&](int c, float mean, float m2n, int count) {
+    const float var = m2n / count;
+    local[c] = mean;
+    local[stride + c] = (var != 0.f || eps != 0.f) ? (float)(1.0 / sqrt((double)var + (double)eps)) : 0.f;
+  });
+}
+
+// torch.batch_norm_gather_stats_with_counts (batch_norm_reduce_statistics_kernel<float, float, int>) over the W
+// gathered rows, ranks folded 0..W-1; ranks with count < 1 are skipped, as torch's SyncBatchNorm drops them before
+// the call.  The expressions are torch's with the contractions nvcc made in its sm_90 build (read from the SASS of
+// libtorch_cuda.so): v * v - eps and (v * v - eps) * count + t are FMAs, as is the mean's n * factor * avg term;
+// factor = 1.0 / (n + count) is a correctly rounded fp32 reciprocal, and n stays an int, n = int(float(n) + count).
+// Also writes norm_fct = 1 / float(sum of int(count)), torch.batch_norm_backward_elemt's factor for the backward,
+// and adds 1 to num_batches_tracked (the module's increment).
+__global__ void __launch_bounds__(kEwThreads) k_bn_sync_merge(const float* __restrict__ rows, const int row_stride, const int world,
+                                                              float* __restrict__ save_mean, float* __restrict__ save_invstd,
+                                                              float* __restrict__ norm_fct, float* __restrict__ running_mean,
+                                                              float* __restrict__ running_var, long long* num_batches_tracked,
+                                                              const float momentum, const float eps, const int stride) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    long long total = 0;
+    for (int j = 0; j < world; j++) {
+      const float count = rows[(size_t)j * row_stride + 2 * stride];
+      if (count >= 1.f) total += (int)count;
+    }
+    *norm_fct = 1.f / (float)total;
+    if (num_batches_tracked) *num_batches_tracked += 1;
+  }
+  if (i >= stride) return;
+  float avg = 0.f, var_n = 0.f;
+  int n = 0;
+  for (int j = 0; j < world; j++) {
+    const float* row = rows + (size_t)j * row_stride;
+    const float count = row[2 * stride];
+    if (!(count >= 1.f)) continue;
+    const float m = row[i];
+    float v = __fdiv_rn(1.f, row[stride + i]);
+    v = __fmaf_rn(v, v, -eps);
+    const float nf = (float)n;
+    const float factor = __fdiv_rn(1.f, __fadd_rn(nf, count));
+    const float d = __fsub_rn(avg, m);
+    const float t = __fmul_rn(__fmul_rn(__fmul_rn(__fmul_rn(d, d), nf), count), factor);   // (avg - m)^2 * n * count * factor
+    var_n = __fadd_rn(var_n, __fmaf_rn(v, count, t));
+    avg = __fmaf_rn(__fmul_rn(nf, factor), avg, __fmul_rn(__fmul_rn(count, factor), m));  // n * factor * avg + count * factor * m
+    n = (int)__fadd_rn(nf, count);
+  }
+  save_mean[i] = avg;
+  save_invstd[i] = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(__fdiv_rn(var_n, (float)n), eps)));
+  running_mean[i] = __fmaf_rn(avg, momentum, __fmul_rn(1 - momentum, running_mean[i]));
+  const float unbiased_var = __fdiv_rn(var_n, (float)(n - 1));
+  running_var[i] = __fmaf_rn(unbiased_var, momentum, __fmul_rn(1 - momentum, running_var[i]));
+}
+
+// y = bf16(bn(x)) (torch.batch_norm_elemt): k_bn_transform's expression without the ReLU, for a batch norm that
+// nothing is fused after.
+template <int V>
+__global__ void __launch_bounds__(kEwThreads) k_bn_sync_transform(const bf16* __restrict__ input, bf16* __restrict__ out,
+                                                                  const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                                  const float* __restrict__ weight, const float* __restrict__ shift,
+                                                                  const int reduction_size, const int stride) {
+  const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
+  if (c0 >= stride) return;
+  float m_c[V], inv_std_c[V], w_c[V], s_c[V];
+#pragma unroll
+  for (int j = 0; j < V; j++) {
+    m_c[j] = mean[c0 + j];
+    inv_std_c[j] = inv_std[c0 + j];
+    w_c[j] = weight[c0 + j];
+    s_c[j] = shift[c0 + j];
+  }
+  const int row_step = blockDim.y * gridDim.y;
+  for (int m = blockIdx.y * blockDim.y + threadIdx.y; m < reduction_size; m += row_step) {
+    const int a = m * stride + c0;
+    const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
+    BVec<V> yv;
+#pragma unroll
+    for (int j = 0; j < V; j++) yv.v[j] = __float2bfloat16(w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j]);
+    *reinterpret_cast<BVec<V>*>(out + a) = yv;
   }
 }
 
@@ -328,19 +429,28 @@ __device__ __forceinline__ bf16 relu_grad_bit(bf16 dy, unsigned bit) { return bi
 // autograd's sum of two gradients of one bf16 tensor
 __device__ __forceinline__ bf16 add_grads(bf16 a, bf16 b) { return __float2bfloat16(__bfloat162float(a) + __bfloat162float(b)); }
 
-// Per-channel sums of g and g * (x - mean) with g = relu_grad(dy, y) (torch:
-// batch_norm_backward_reduce_channels_last_kernel<4>), and dweight / dbias.  BITS reads the ReLU's predicate from
-// `mask` (k_bn_transform's bits) instead of y from `output`.  With `grad_output2` set, dy is the bf16 sum of the
-// two gradients, as autograd rounds it when a tensor has two consumers; without it dy is taken as it is, so a
-// -0.0 gradient stays -0.0.  With `masked` set (the block tail, where g is also the identity branch's gradient) g
-// is written there as well.  As in k_bn_stats, all rows of an iteration are loaded before the first sum uses one.
-template <bool BITS>
-__global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
-                                const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
-                                const uint8_t* __restrict__ mask, bf16* __restrict__ masked, const float* __restrict__ mean,
-                                const float* __restrict__ inv_std, float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
-                                float* __restrict__ grad_weight, float* __restrict__ grad_bias, volatile float* staging_data,
-                                int* semaphores, const int reduction_size, const int stride) {
+// Where the backward kernels take g, the batch norm's output gradient, from: the tensor the reduce kernel wrote
+// (kGradMasked), relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits), or dy itself, for
+// a batch norm without a ReLU after it (kGradDy).
+enum GradSrc { kGradMasked, kGradY, kGradBits, kGradDy };
+
+// Per-channel sums of g and g * (x - mean) with g from G (torch: batch_norm_backward_reduce_channels_last_kernel<4>),
+// and dweight / dbias.  kGradBits reads the ReLU's predicate from `mask` (k_bn_transform's bits) instead of y from
+// `output`.  With `grad_output2` set, dy is the bf16 sum of the two gradients, as autograd rounds it when a tensor
+// has two consumers; without it dy is taken as it is, so a -0.0 gradient stays -0.0.  With `masked` set (the block
+// tail, where g is also the identity branch's gradient) g is written there as well.  As in k_bn_stats, all rows of
+// an iteration are loaded before the first sum uses one.
+template <GradSrc G>
+__device__ __forceinline__ void bn_bwd_reduce_body(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
+                                                   const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
+                                                   const uint8_t* __restrict__ mask, bf16* __restrict__ masked,
+                                                   const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                   float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
+                                                   float* __restrict__ grad_weight, float* __restrict__ grad_bias,
+                                                   volatile float* staging_data, int* semaphores, const int reduction_size,
+                                                   const int stride) {
+  static_assert(G != kGradMasked, "the reduce kernel computes g");
+  constexpr bool BITS = G == kGradBits;
   constexpr int PARALLEL_LOADS = kParallelLoads;
   float sum_dy[PARALLEL_LOADS];
   float sum_dy_xmu[PARALLEL_LOADS];
@@ -370,7 +480,7 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
         dy_v[j] = grad_output[a];
         if (grad_output2) dy2_v[j] = grad_output2[a];
         if (BITS) mask_v[j] = mask[a >> 3];
-        else y_v[j] = output[a];
+        else if (G == kGradY) y_v[j] = output[a];
         x_v[j] = input[a];
       }
     }
@@ -380,7 +490,7 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (c_offset < stride && m_offset < reduction_size) {
         const bf16 dy = grad_output2 ? add_grads(dy_v[j], dy2_v[j]) : dy_v[j];
-        const bf16 g = BITS ? relu_grad_bit(dy, (mask_v[j] >> (address_base & 7)) & 1u) : relu_grad(dy, y_v[j]);
+        const bf16 g = BITS ? relu_grad_bit(dy, (mask_v[j] >> (address_base & 7)) & 1u) : G == kGradY ? relu_grad(dy, y_v[j]) : dy;
         if (masked) masked[address_base] = g;
         x_input[j] = __bfloat162float(x_v[j]);
         x_grad_output[j] = __bfloat162float(g);
@@ -452,21 +562,38 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
   }
 }
 
-// Where the backward elementwise kernel takes g from: the tensor the reduce kernel wrote (kGradMasked), or
-// relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits).
-enum GradSrc { kGradMasked, kGradY, kGradBits };
+#define B200C_BN_BWD_REDUCE_PARAMS                                                                                        \
+  const bf16 *__restrict__ input, const bf16 *__restrict__ grad_output, const bf16 *__restrict__ grad_output2,           \
+      const bf16 *__restrict__ output, const uint8_t *__restrict__ mask, bf16 *__restrict__ masked,                      \
+      const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy_o,                   \
+      float *__restrict__ sum_dy_xmu_o, float *__restrict__ grad_weight, float *__restrict__ grad_bias,                  \
+      volatile float *staging_data, int *semaphores, const int reduction_size, const int stride
+#define B200C_BN_BWD_REDUCE_ARGS                                                                                          \
+  input, grad_output, grad_output2, output, mask, masked, mean, inv_std, sum_dy_o, sum_dy_xmu_o, grad_weight, grad_bias, \
+      staging_data, semaphores, reduction_size, stride
+
+// g = relu_grad(dy, y), or with BITS relu_grad_bit(dy, mask)
+template <bool BITS>
+__global__ void k_bn_bwd_reduce(B200C_BN_BWD_REDUCE_PARAMS) {
+  bn_bwd_reduce_body<BITS ? kGradBits : kGradY>(B200C_BN_BWD_REDUCE_ARGS);
+}
+
+// g = dy: a batch norm without a ReLU after it
+__global__ void k_bn_sync_bwd_reduce(B200C_BN_BWD_REDUCE_PARAMS) { bn_bwd_reduce_body<kGradDy>(B200C_BN_BWD_REDUCE_ARGS); }
+
+#undef B200C_BN_BWD_REDUCE_ARGS
+#undef B200C_BN_BWD_REDUCE_PARAMS
 
 // dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g from G; dy is summed with `grad_output2`
 // when that is set, as in k_bn_bwd_reduce.
 template <int V, GradSrc G>
-__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restrict__ grad_output,
-                                                             const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
-                                                             const uint8_t* __restrict__ mask,
-                                                             const bf16* __restrict__ input, bf16* __restrict__ grad_input,
-                                                             const float* __restrict__ mean, const float* __restrict__ inv_std,
-                                                             const float* __restrict__ weight, const float* __restrict__ sum_dy,
-                                                             const float* __restrict__ sum_dy_xmu, const float norm_fct,
-                                                             const int reduction_size, const int stride) {
+__device__ __forceinline__ void bn_bwd_elemt_body(const bf16* __restrict__ grad_output, const bf16* __restrict__ grad_output2,
+                                                  const bf16* __restrict__ output, const uint8_t* __restrict__ mask,
+                                                  const bf16* __restrict__ input, bf16* __restrict__ grad_input,
+                                                  const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                  const float* __restrict__ weight, const float* __restrict__ sum_dy,
+                                                  const float* __restrict__ sum_dy_xmu, const float norm_fct,
+                                                  const int reduction_size, const int stride) {
   const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   if (c0 >= stride) return;
   float m_c[V], m_dy_c[V], factor_1_c[V], factor_2_c[V];
@@ -492,12 +619,37 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restr
 #pragma unroll
     for (int j = 0; j < V; j++) {
       const bf16 dy = G != kGradMasked && grad_output2 ? add_grads(gv.v[j], gv2.v[j]) : gv.v[j];
-      const float g = __bfloat162float(G == kGradMasked ? dy : G == kGradY ? relu_grad(dy, yv.v[j]) : relu_grad_bit(dy, (bits >> j) & 1u));
+      const float g = __bfloat162float(G == kGradMasked || G == kGradDy ? dy
+                                       : G == kGradY ? relu_grad(dy, yv.v[j]) : relu_grad_bit(dy, (bits >> j) & 1u));
       dxv.v[j] = __float2bfloat16((g - m_dy_c[j] - (__bfloat162float(xv.v[j]) - m_c[j]) * factor_1_c[j]) * factor_2_c[j]);
     }
     *reinterpret_cast<BVec<V>*>(grad_input + a) = dxv;
   }
 }
+
+#define B200C_BN_BWD_ELEMT_PARAMS                                                                                          \
+  const bf16 *__restrict__ grad_output, const bf16 *__restrict__ grad_output2, const bf16 *__restrict__ output,           \
+      const uint8_t *__restrict__ mask, const bf16 *__restrict__ input, bf16 *__restrict__ grad_input,                    \
+      const float *__restrict__ mean, const float *__restrict__ inv_std, const float *__restrict__ weight,                 \
+      const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xmu
+#define B200C_BN_BWD_ELEMT_ARGS grad_output, grad_output2, output, mask, input, grad_input, mean, inv_std, weight, sum_dy, sum_dy_xmu
+
+// norm_fct = (float)(1.0 / m), computed by the launcher from this call's rows
+template <int V, GradSrc G>
+__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(B200C_BN_BWD_ELEMT_PARAMS, const float norm_fct, const int reduction_size,
+                                                             const int stride) {
+  bn_bwd_elemt_body<V, G>(B200C_BN_BWD_ELEMT_ARGS, norm_fct, reduction_size, stride);
+}
+
+// norm_fct read from k_bn_sync_merge's output: 1 / float(rows of all ranks)
+template <int V, GradSrc G>
+__global__ void __launch_bounds__(kEwThreads) k_bn_sync_bwd_elemt(B200C_BN_BWD_ELEMT_PARAMS, const float* __restrict__ norm_fct,
+                                                                  const int reduction_size, const int stride) {
+  bn_bwd_elemt_body<V, G>(B200C_BN_BWD_ELEMT_ARGS, *norm_fct, reduction_size, stride);
+}
+
+#undef B200C_BN_BWD_ELEMT_ARGS
+#undef B200C_BN_BWD_ELEMT_PARAMS
 
 }  // namespace bn
 }  // namespace b200c

@@ -47,5 +47,24 @@ size_t scratch_bytes(int c);
 cudaError_t forward(const FwdArgs& a, cudaStream_t s);   // 2 kernels
 cudaError_t backward(const BwdArgs& a, cudaStream_t s);  // 2 kernels
 
+// Sync batch norm: the local phases around the two collectives, which b200coll.cu runs between them.
+//   forward:  sync_stats -> allgather of `local` (2c + 1 floats) into the W `gathered` rows -> sync_apply
+//   backward: sync_bwd_reduce -> allreduce SUM of `sums` (2c floats, in place) -> sync_bwd_elemt
+// FwdArgs.save_mean / save_invstd receive the global statistics, which the backward reads.  m may be 0: the rank
+// then sends zeros and launches only the merge.  Each phase returns the number of kernels it launched.
+struct SyncRows {
+  float* local;       // [mean (c) | invstd (c) | count], 16-byte aligned
+  float* gathered;    // W rows like `local`, row_floats apart (16-byte aligned)
+  size_t row_floats;
+  float* sums;        // [sum_dy (c) | sum_dy_xmu (c)], 16-byte aligned
+};
+size_t sync_scratch_bytes(int c, int world);
+SyncRows sync_rows(void* scratch, int c);
+int sync_stats(const FwdArgs& a, cudaStream_t s);
+int sync_apply(const FwdArgs& a, bool relu, int world, float* norm_fct, cudaStream_t s);
+int sync_bwd_reduce(const BwdArgs& a, bool relu, cudaStream_t s);
+int sync_bwd_elemt(const BwdArgs& a, bool relu, const float* norm_fct, cudaStream_t s);
+cudaError_t load_kernels();   // every kernel above, into the current context
+
 }  // namespace bn
 }  // namespace b200c

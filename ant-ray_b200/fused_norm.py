@@ -13,10 +13,21 @@ value per channel, a channel stride of 1 and at most 131072 channels, its batch 
 a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum, and
 torch would run it on its native kernels (`torch._C._select_batch_norm_backend`).  Otherwise the block runs the
 parent class's ops, so the choice never changes a result.
+
+Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
+`FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
+more than one rank (a "sync site"), its statistics are gathered and its gradient sums reduced over that
+communicator instead of torch's NCCL process group, with one native call per direction that also fuses the ReLU and
+the residual add at ResNet positions; the results have the bits of torch's SyncBatchNorm function (ranks folded in
+rank order).  Whether a site syncs depends only on the module and the input's layout, never on the rank's batch
+size, so every rank joins the same collectives: a rank with an empty batch still contributes its zero row.  A
+SyncBatchNorm that torch would not synchronise (no process group, or one rank) runs the local fused site above,
+which is what torch's F.batch_norm computes.
 """
 import numbers
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
@@ -47,10 +58,17 @@ def _scratch_bytes(channels):
     return need
 
 
-def _scratch_ptr(device, stream, channels):
+def _sync_scratch_bytes(channels, world):
+    key = (channels, world)
+    need = _scratch_need.get(key)
+    if need is None:
+        need = _scratch_need[key] = int(_native_lib().b200c_bn_sync_scratch_bytes(channels, world))
+    return need
+
+
+def _scratch_ptr(device, stream, need):
     key = (device.index, stream)
     entry = _scratch.get(key)
-    need = _scratch_need[channels]   # filled by _fusable
     if entry is None or entry[0] < need:
         buf = torch.zeros(need, dtype=torch.uint8, device=device)
         entry = _scratch[key] = (need, buf.data_ptr(), buf)
@@ -63,22 +81,47 @@ class _FusedBatchNorm(torch.autograd.Function):
     With `pair` the output is returned twice, as y and a view of it, for a block tail whose output feeds both
     branches of the next block: autograd then hands the backward the two branches' gradients apart (None for an
     unused one), and the kernel sums them as autograd would.  Where C % 8 == 0 the forward writes the ReLU's mask
-    as bits and the backward reads those instead of y."""
+    as bits and the backward reads those instead of y.
+
+    With `comm` (a PeerMemoryComm) the site is a sync site over its ranks; `relu` False then runs bn(x) alone, the
+    forward of a SyncBatchNorm with nothing fused after it."""
 
     @staticmethod
-    def forward(ctx, x, identity, weight, bias, bn, pair):
+    def forward(ctx, x, identity, weight, bias, bn, pair, comm=None, relu=True):
         lib = _native_lib()
         c = x.shape[1]
         m = x.numel() // c
         y = torch.empty_like(x)
+        nbt = bn.num_batches_tracked
+        nbt_ptr = nbt.data_ptr() if nbt is not None else None
+        id_ptr = identity.data_ptr() if identity is not None else None
+        ctx.residual = identity is not None
+        ctx.comm, ctx.relu = comm, relu
+        ctx.set_materialize_grads(False)
+        if comm is not None:
+            stream = comm.stream().cuda_stream
+            # stats = [save_mean (c) | save_invstd (c) | norm_fct]: the global statistics and the backward's 1 / rows
+            stats = torch.empty(2 * c + 1, dtype=torch.float32, device=x.device)
+            mean = stats.data_ptr()
+            # what the backward reads of the ReLU: its mask, else y; nothing at a site without ReLU, whose output may
+            # then be modified in place (an inplace ReLU or `+= identity` after a SyncBatchNorm)
+            relu_src = None
+            if relu:
+                relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if c % 8 == 0 else y
+            mask_ptr = relu_src.data_ptr() if relu_src is not None and relu_src.dtype == torch.uint8 else None
+            scratch = _scratch_ptr(x.device, stream, _sync_scratch_bytes(c, comm.world_size))
+            N.check(lib.b200c_bn_sync_forward(comm._h(), x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, int(relu),
+                                              weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(),
+                                              bn.running_var.data_ptr(), nbt_ptr, mean, mean + 4 * c, mean + 8 * c, m, c,
+                                              bn.momentum, bn.eps, scratch, stream))
+            ctx.save_for_backward(x, relu_src, weight, stats)
+            return (y, y.view_as(y)) if pair else y
         stats = torch.empty(2, c, dtype=torch.float32, device=x.device)
         stream = _raw_stream(x.device.index)
-        nbt = bn.num_batches_tracked
         mean = stats.data_ptr()   # stats = [save_mean; save_invstd]
         args = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c,
-                m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, c), stream)
-        id_ptr = identity.data_ptr() if identity is not None else None
+                nbt_ptr, mean, mean + 4 * c,
+                m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_need[c]), stream)
         if c % 8 == 0:
             relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device)
             N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), relu_src.data_ptr(), *args))
@@ -86,36 +129,52 @@ class _FusedBatchNorm(torch.autograd.Function):
             relu_src = y
             N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *args))
         ctx.save_for_backward(x, relu_src, weight, stats)
-        ctx.residual = identity is not None
-        ctx.set_materialize_grads(False)
         return (y, y.view_as(y)) if pair else y
 
     @staticmethod
     @once_differentiable
     def backward(ctx, *grads):
         grads = [g.contiguous(memory_format=torch.channels_last) for g in grads if g is not None]
-        if not grads:
-            return None, None, None, None, None, None
-        lib = _native_lib()
         x, relu_src, weight, stats = ctx.saved_tensors
+        if not grads:
+            if ctx.comm is None:
+                return None, None, None, None, None, None, None, None
+            # the other ranks wait in this site's all-reduce: join it with a zero gradient
+            grads = [torch.zeros_like(x, memory_format=torch.channels_last)]
+        lib = _native_lib()
         c = x.shape[1]
         m = x.numel() // c
         dx = torch.empty_like(x)
         d_identity = torch.empty_like(x) if ctx.residual else None
         grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
         grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
-        stream = _raw_stream(x.device.index)
         mean = stats.data_ptr()
-        args = (x.data_ptr(), d_identity.data_ptr() if d_identity is not None else None, dx.data_ptr(), weight.data_ptr(),
-                mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, c),
-                stream)
+        did_ptr = d_identity.data_ptr() if d_identity is not None else None
+        if ctx.comm is not None:
+            comm = ctx.comm
+            stream = comm.stream().cuda_stream
+            scratch = _scratch_ptr(x.device, stream, _sync_scratch_bytes(c, comm.world_size))
+            mask = relu_src.data_ptr() if ctx.relu and relu_src.dtype == torch.uint8 else None
+            y = relu_src.data_ptr() if ctx.relu and mask is None else None
+            dy2 = grads[1].data_ptr() if len(grads) == 2 else None
+            N.check(lib.b200c_bn_sync_backward(comm._h(), grads[0].data_ptr(), dy2, y, mask, int(ctx.relu), x.data_ptr(),
+                                               did_ptr, dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, mean + 8 * c,
+                                               grad_weight.data_ptr(), grad_bias.data_ptr(), m, c, scratch, stream))
+            if m == 0:
+                # as torch's SyncBatchNorm: no gradient for an empty input, nor for weight and bias from this rank
+                return None, d_identity, None, None, None, None, None, None
+            return dx, d_identity, grad_weight, grad_bias, None, None, None, None
+        stream = _raw_stream(x.device.index)
+        args = (x.data_ptr(), did_ptr, dx.data_ptr(), weight.data_ptr(),
+                mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c,
+                _scratch_ptr(x.device, stream, _scratch_need[c]), stream)
         if relu_src.dtype == torch.uint8:
             dy2 = grads[1].data_ptr() if len(grads) == 2 else None
             N.check(lib.b200c_bn_backward_mask(grads[0].data_ptr(), dy2, relu_src.data_ptr(), *args))
         else:
             dy = grads[0] + grads[1] if len(grads) == 2 else grads[0]
             N.check(lib.b200c_bn_backward(dy.data_ptr(), relu_src.data_ptr(), *args))
-        return dx, d_identity, grad_weight, grad_bias, None, None
+        return dx, d_identity, grad_weight, grad_bias, None, None, None, None
 
 
 def _activation(t):
@@ -125,9 +184,17 @@ def _activation(t):
             and t.stride(1) == 1)
 
 
+def _torch_syncs(bn):
+    """Whether torch's SyncBatchNorm.forward would synchronise `bn` (its need_sync, in training mode)."""
+    if not (dist.is_available() and dist.is_initialized()):
+        return False
+    return dist.get_world_size(bn.process_group or dist.group.WORLD) > 1
+
+
 def _fusable(bn, relu, x):
     """Whether this site can run fused: the conditions of the module docstring."""
-    if type(bn) is not nn.BatchNorm2d or type(relu) is not nn.ReLU or not bn.training or not bn.track_running_stats:
+    local = type(bn) is nn.BatchNorm2d or (isinstance(bn, nn.SyncBatchNorm) and not _torch_syncs(bn))
+    if not local or type(relu) is not nn.ReLU or not bn.training or not bn.track_running_stats:
         return False
     w, b, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
     if w is None or b is None or rm is None or bn._forward_hooks or bn._forward_pre_hooks:
@@ -142,9 +209,41 @@ def _fusable(bn, relu, x):
     return torch._C._select_batch_norm_backend(x, w, b, rm, rv, True, bn.eps) == _NATIVE
 
 
+def _rows(t):
+    """_activation, where a tensor without elements (a rank with an empty batch) passes on its device, dtype and rank
+    alone: its strides say nothing (a convolution over an empty batch returns default strides whatever its input's
+    layout), the kernels read none of its elements, and the sync decision must not depend on a rank's batch size."""
+    return _activation(t) or (t.numel() == 0 and t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 4)
+
+
+def _sync_comm(bn, x):
+    """The communicator of a sync site (the conditions of the module docstring), else None.  Only conditions that
+    every rank meets alike decide; an input the kernels cannot take raises instead of falling back, since the other
+    ranks would wait in this site's collectives."""
+    comm = getattr(bn, "b200_comm", None)
+    if comm is None or comm.world_size <= 1 or not bn.training or not bn.track_running_stats:
+        return None
+    w, b, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
+    if w is None or b is None or rm is None or not isinstance(bn.momentum, numbers.Real) or not _rows(x):
+        return None
+    if any(t.dtype != torch.float32 or not t.is_contiguous() for t in (w, b, rm, rv)):
+        return None
+    if x.numel() >= 2 ** 31 or not _sync_scratch_bytes(x.shape[1], comm.world_size):
+        raise RuntimeError(f"sync batch norm: input of shape {tuple(x.shape)} exceeds the kernels' limits "
+                           "(< 2^31 elements, at most 131072 channels)")
+    return comm
+
+
+def _relu_fusable(bn, relu):
+    return type(relu) is nn.ReLU and not bn._forward_hooks and not bn._forward_pre_hooks
+
+
 def bn_relu(bn, relu, x):
     """relu(bn(x)), fused when the site allows it."""
-    if _fusable(bn, relu, x):
+    comm = _sync_comm(bn, x)
+    if comm is not None and _relu_fusable(bn, relu):
+        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, comm, True)
+    if comm is None and _fusable(bn, relu, x):
         return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False)
     return relu(bn(x))
 
@@ -152,7 +251,11 @@ def bn_relu(bn, relu, x):
 def bn_add_relu(bn, relu, x, identity, pair=False):
     """`out = bn(x); out += identity; relu(out)`, fused when the site allows it.  With `pair`, returns `(out,
     out_id)`: the same values, whose gradients a fused site receives apart and sums in its backward kernel."""
-    if _fusable(bn, relu, x) and _activation(identity) and identity.shape == x.shape:
+    comm = _sync_comm(bn, x)
+    if comm is not None:
+        if _relu_fusable(bn, relu) and _rows(identity) and identity.shape == x.shape:
+            return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair, comm, True)
+    elif _fusable(bn, relu, x) and _activation(identity) and identity.shape == x.shape:
         return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair)
     out = bn(x)
     out += identity
@@ -229,6 +332,41 @@ else:
             return self.fc(x)
 
     _SWAP = {ResNet: FusedResNet, Bottleneck: FusedBottleneck, BasicBlock: FusedBasicBlock}
+
+
+class FusedSyncBatchNorm(nn.SyncBatchNorm):
+    """nn.SyncBatchNorm whose sync sites run on the peer-memory communicator `b200_comm` (see `sync_batch_norm`).
+    Its own forward is a site with nothing fused after it; anything that is not a sync site runs nn.SyncBatchNorm's
+    forward unchanged."""
+
+    b200_comm = None
+
+    def forward(self, x):
+        comm = _sync_comm(self, x)
+        if comm is None:
+            return super().forward(x)
+        return _FusedBatchNorm.apply(x, None, self.weight, self.bias, self, False, comm, False)
+
+
+def _world_group(pg):
+    return pg is None or (dist.is_available() and dist.is_initialized() and pg == dist.group.WORLD)
+
+
+def has_world_sync_batch_norm(model):
+    """Whether `model` has an nn.SyncBatchNorm over the world group (process_group None or WORLD)."""
+    return any(isinstance(m, nn.SyncBatchNorm) and _world_group(m.process_group) for m in model.modules())
+
+
+def sync_batch_norm(model, comm):
+    """Rewrite `model` in place: every nn.SyncBatchNorm (exactly that class, or FusedSyncBatchNorm) over the world
+    group becomes a FusedSyncBatchNorm that runs its sync sites over `comm`, a PeerMemoryComm of the same ranks.
+    Parameters, buffers, state_dict keys, hooks and the object itself are unchanged.  SyncBatchNorm over a process
+    subgroup is left to torch."""
+    for mod in model.modules():
+        if type(mod) in (nn.SyncBatchNorm, FusedSyncBatchNorm) and _world_group(mod.process_group):
+            mod.__class__ = FusedSyncBatchNorm
+            mod.b200_comm = comm
+    return model
 
 
 def fuse_resnet(model):

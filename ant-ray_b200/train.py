@@ -125,7 +125,9 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     Same arguments as the reference (v2/torch/train_loop_utils.py:166-248); `grad_wire` overrides
     the backend config's wire type, `wrap_single` wraps in DDP / FSDP even at world size 1 (the
     reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
-    torchvision ResNet is first rewritten in place by `fused_norm.fuse_resnet`.
+    torchvision ResNet is first rewritten in place by `fused_norm.fuse_resnet`, and with more than one rank the
+    model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
+    communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.
     """
     parallel_strategy_kwargs = dict(parallel_strategy_kwargs or {})
     device = move_to_device if isinstance(move_to_device, torch.device) else get_device()
@@ -139,6 +141,7 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
 
         fused_norm.fuse_resnet(model)
     world_size = dist.get_world_size() if dist.is_initialized() else 1
+    norm_comm = _attach_sync_norm(model, device, world_size)
     if parallel_strategy and (world_size > 1 or wrap_single):
         if parallel_strategy not in ("ddp", "fsdp"):
             raise RuntimeError(f"Unknown parallel_strategy {parallel_strategy!r}: the B200 backend supports 'ddp' and 'fsdp'.")
@@ -160,4 +163,32 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
 
             model = FullyShardedDataParallel(model, **parallel_strategy_kwargs)
             model.b200_grad_state = fsdp.register_fsdp1(model, wire=wire)
+    if norm_comm is not None:
+        model.b200_norm_comm = norm_comm
     return model
+
+
+def _attach_sync_norm(model, device, world_size):
+    """Run the model's world-group SyncBatchNorm layers on peer memory instead of NCCL (fused_norm.sync_batch_norm);
+    returns the communicator, or None where there is nothing to synchronise.  It is a communicator of its own: these
+    collectives run on the compute stream, the gradient hook's on its own stream.  The returned module owns it
+    (`.b200_norm_comm`), like the hook's communicator it lives until the process ends; a caller that keeps the
+    process after training calls `model.b200_norm_comm.destroy()`, after which the model's sync sites raise."""
+    if device.type != "cuda" or world_size <= 1:
+        return None
+    from . import fused_norm
+
+    if not fused_norm.has_world_sync_batch_norm(model):
+        return None
+    comm = _sync_norm_comm(device)
+    fused_norm.sync_batch_norm(model, comm)
+    return comm
+
+
+def _sync_norm_comm(device):
+    """The sync batch norm's communicator over the default store.  Its messages are at most W * (2C + 1) floats
+    (C <= 2048 for a ResNet: 16 KiB a rank), so a small staging area and a few CTAs per collective suffice."""
+    from .b200_group import PeerMemoryComm, make_config, next_comm_key
+
+    config = make_config(staging_bytes=1 << 20, max_blocks=8)
+    return PeerMemoryComm(dist.get_world_size(), dist.get_rank(), next_comm_key("train/syncbn"), device.index, None, config)

@@ -321,6 +321,39 @@ int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask,
                            const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
                            float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream);
 
+/* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
+ * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
+ * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)
+ * whose all_gather stacks the ranks in order and whose all_reduce folds them in rank order.  Every rank calls both
+ * functions for every site, in the same order, with its own rows: `m` may differ between ranks and may be 0 (the
+ * rank then contributes count 0 and zero sums, and its dweight / dbias are written as zeros; torch's SyncBatchNorm
+ * has no gradient there, which is what fused_norm returns for such a rank).
+ *
+ * `relu` != 0: y = relu(bn(x)) or, with `identity`, relu(bn(x) + identity), as b200c_bn_forward; `mask` (may be
+ * NULL; channels % 8 == 0) as in b200c_bn_forward_mask.  relu == 0: y = bn(x); identity, mask, dy2 and dy_masked
+ * must then be NULL.
+ *
+ * Forward: local statistics -> b200c_allgather of [mean, invstd, count] (2 * channels + 1 floats) -> merge of the
+ * ranks with count >= 1 -> transform, in stream order.  Writes save_mean / save_invstd (the global statistics),
+ * norm_fct (one float: 1 / the global row count, which the backward reads), y and mask, updates running_mean /
+ * running_var with the unbiased global variance and adds 1 to num_batches_tracked (may be NULL).
+ * Backward: local sums of g and g * (x - mean) and dweight / dbias (kept local, as torch keeps them) ->
+ * b200c_allreduce SUM of the 2 * channels sums -> dx (and dy_masked as in b200c_bn_backward).
+ *
+ * `scratch` holds at least b200c_bn_sync_scratch_bytes(channels, world) bytes, zero-filled before its first use,
+ * with the same contract as b200c_bn_scratch_bytes: it serves sites of any channel count on one stream, and its
+ * semaphores are left at zero.  b200c_bn_sync_scratch_bytes returns 0 for channels outside 1..131072 or world
+ * outside 1..8.  Every argument is checked before the first launch. */
+size_t b200c_bn_sync_scratch_bytes(int channels, int world);
+int b200c_bn_sync_forward(b200c_comm_t* comm, const void* x, const void* identity, void* y, uint8_t* mask, int relu,
+                          const float* weight, const float* bias, float* running_mean, float* running_var,
+                          int64_t* num_batches_tracked, float* save_mean, float* save_invstd, float* norm_fct, int m,
+                          int channels, float momentum, float eps, void* scratch, b200c_stream_t stream);
+int b200c_bn_sync_backward(b200c_comm_t* comm, const void* dy, const void* dy2, const void* y, const uint8_t* mask, int relu,
+                           const void* x, void* dy_masked, void* dx, const float* weight, const float* save_mean,
+                           const float* save_invstd, const float* norm_fct, float* grad_weight, float* grad_bias, int m,
+                           int channels, void* scratch, b200c_stream_t stream);
+
 /* Launch statistics (bench.py's gpu_launches claim). */
 uint64_t b200c_launch_count(void);
 

@@ -203,89 +203,6 @@ extern "C" size_t b200c_dtype_size(int dtype) {
 }
 extern "C" uint64_t b200c_launch_count(void) { return g_launches.load(); }
 
-// ------------------------------------------------------------------------------------------------
-// fused batch norm (norm_kernels.cuh)
-// ------------------------------------------------------------------------------------------------
-static int check_bn_shape(int m, int c, const void* scratch) {
-  if (m < 1 || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX)
-    return fail(B200C_EINVAL, "batch norm: bad shape m=%d c=%d", m, c);
-  if (!scratch) return fail(B200C_EINVAL, "batch norm: null scratch");
-  return B200C_OK;
-}
-
-extern "C" size_t b200c_bn_scratch_bytes(int channels) {
-  return channels < 1 || channels > bn::kMaxChannels ? 0 : bn::scratch_bytes(channels);
-}
-
-static int bn_forward(const void* x, const void* identity, void* y, void* mask, const float* weight, const float* bias,
-                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
-                      float* save_invstd, int m, int channels, float momentum, float eps, void* scratch, b200c_stream_t stream) {
-  int rc = check_bn_shape(m, channels, scratch);
-  if (rc) return rc;
-  if (!x || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
-    return fail(B200C_EINVAL, "batch norm forward: null buffer");
-  bn::FwdArgs a{x, identity, y, mask, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
-                save_mean, save_invstd, m, channels, momentum, eps, scratch};
-  RT(bn::forward(a, (cudaStream_t)stream));
-  g_launches.fetch_add(2);
-  return B200C_OK;
-}
-
-static int bn_backward(const void* dy, const void* dy2, const void* y, const void* mask, const void* x, void* dy_masked,
-                       void* dx, const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
-                       float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream) {
-  int rc = check_bn_shape(m, channels, scratch);
-  if (rc) return rc;
-  if (!dy || !(y || mask) || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias)
-    return fail(B200C_EINVAL, "batch norm backward: null buffer");
-  bn::BwdArgs a{dy, dy2, y, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
-  RT(bn::backward(a, (cudaStream_t)stream));
-  g_launches.fetch_add(2);
-  return B200C_OK;
-}
-
-// The mask holds 8 channels per byte of a row, so its calls take C % 8 == 0 only.
-static int check_bn_mask(const void* mask, int channels) {
-  if (!mask) return fail(B200C_EINVAL, "batch norm mask: null mask");
-  if (channels % 8) return fail(B200C_EINVAL, "batch norm mask: channels=%d is not a multiple of 8", channels);
-  return B200C_OK;
-}
-
-extern "C" int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
-                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
-                                float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
-                                b200c_stream_t stream) {
-  return bn_forward(x, identity, y, nullptr, weight, bias, running_mean, running_var, num_batches_tracked, save_mean, save_invstd,
-                    m, channels, momentum, eps, scratch, stream);
-}
-
-extern "C" int b200c_bn_forward_mask(const void* x, const void* identity, void* y, uint8_t* mask, const float* weight,
-                                     const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked,
-                                     float* save_mean, float* save_invstd, int m, int channels, float momentum, float eps,
-                                     void* scratch, b200c_stream_t stream) {
-  int rc = check_bn_mask(mask, channels);
-  if (rc) return rc;
-  return bn_forward(x, identity, y, mask, weight, bias, running_mean, running_var, num_batches_tracked, save_mean, save_invstd,
-                    m, channels, momentum, eps, scratch, stream);
-}
-
-extern "C" int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
-                                 const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
-                                 int channels, void* scratch, b200c_stream_t stream) {
-  return bn_backward(dy, nullptr, y, nullptr, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m,
-                     channels, scratch, stream);
-}
-
-extern "C" int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask, const void* x, void* dy_masked,
-                                      void* dx, const float* weight, const float* save_mean, const float* save_invstd,
-                                      float* grad_weight, float* grad_bias, int m, int channels, void* scratch,
-                                      b200c_stream_t stream) {
-  int rc = check_bn_mask(mask, channels);
-  if (rc) return rc;
-  return bn_backward(dy, dy2, nullptr, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m,
-                     channels, scratch, stream);
-}
-
 extern "C" void b200c_default_config(b200c_config_t* cfg) {
   memset(cfg, 0, sizeof *cfg);
   cfg->struct_size = sizeof *cfg;
@@ -1439,71 +1356,144 @@ extern "C" int b200c_allgather(b200c_comm_t* c, const void* send, void* const* r
 }
 
 // ------------------------------------------------------------------------------------------------
-// sync batch norm: the local batch-norm phases (inst_norm.cu) around b200c_allgather and b200c_allreduce
+// fused batch norm (norm_kernels.cuh, launched by inst_norm.cu): a local site runs two kernels per direction; a sync
+// site runs the local phases around b200c_allgather and b200c_allreduce
 // ------------------------------------------------------------------------------------------------
+extern "C" size_t b200c_bn_scratch_bytes(int channels) {
+  return channels < 1 || channels > bn::kMaxChannels ? 0 : bn::scratch_bytes(channels);
+}
+
 extern "C" size_t b200c_bn_sync_scratch_bytes(int channels, int world) {
   return channels < 1 || channels > bn::kMaxChannels || world < 1 || world > kMaxRanks ? 0 : bn::sync_scratch_bytes(channels, world);
 }
 
-// Checks shared by both directions; m = 0 is a rank without rows.  A plain site (relu == 0) has no identity, no
-// mask and no second gradient.
-static int check_bn_sync(int m, int c, const void* scratch, int relu, const void* mask, const void* identity, const void* dy2) {
-  if (m < 0 || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX)
-    return fail(B200C_EINVAL, "sync batch norm: bad shape m=%d c=%d", m, c);
-  if (!scratch) return fail(B200C_EINVAL, "sync batch norm: null scratch");
-  if (!relu && (mask || identity || dy2)) return fail(B200C_EINVAL, "sync batch norm: a site without ReLU takes no mask, identity or dy2");
-  if (mask && c % 8) return fail(B200C_EINVAL, "sync batch norm mask: channels=%d is not a multiple of 8", c);
+static const char* bn_site(bool sync) { return sync ? "sync batch norm" : "batch norm"; }
+
+// Checks shared by every call.  min_m is 1 for a local site and 0 for a sync site, where a rank may have no rows.  A
+// site without ReLU has no identity (forward) or gradient for it (backward), no mask and no second gradient.  The
+// mask holds 8 channels per byte of a row, so it takes C % 8 == 0 only.
+static int check_bn(const char* site, int min_m, int m, int c, const void* scratch, int relu, const void* mask, const void* residual,
+                    const void* dy2) {
+  if (m < min_m || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX)
+    return fail(B200C_EINVAL, "%s: bad shape m=%d c=%d", site, m, c);
+  if (!scratch) return fail(B200C_EINVAL, "%s: null scratch", site);
+  if (!relu && (mask || residual || dy2)) return fail(B200C_EINVAL, "%s: a site without ReLU takes no mask, identity or dy2", site);
+  if (mask && c % 8) return fail(B200C_EINVAL, "%s mask: channels=%d is not a multiple of 8", site, c);
   return B200C_OK;
+}
+
+// All arguments are checked before the communicator and before any launch.  A sync rank without rows launches only
+// the merge.
+static int bn_forward(b200c_comm_t* comm, bool sync, const void* x, const void* identity, void* y, void* mask, int relu,
+                      const float* weight, const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                      float* save_mean, float* save_invstd, float* norm_fct, int m, int channels, float momentum, float eps,
+                      void* scratch, b200c_stream_t stream) {
+  int rc = check_bn(bn_site(sync), sync ? 0 : 1, m, channels, scratch, relu, mask, identity, nullptr);
+  if (rc) return rc;
+  if ((m && (!x || !y)) || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || (sync && !norm_fct))
+    return fail(B200C_EINVAL, "%s forward: null buffer", bn_site(sync));
+  const bn::FwdArgs a{x, identity, y, mask, relu != 0, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!sync) {
+    RT(bn::forward(a, s));
+    g_launches.fetch_add(2);
+    return B200C_OK;
+  }
+  rc = check_ready(comm);
+  if (rc) return rc;
+  DeviceGuard g(comm->device);
+  const int rows = m != 0;
+  RT(bn::sync_stats(a, s));
+  g_launches.fetch_add(rows);
+  const bn::SyncRows r = bn::sync_rows(scratch, channels);
+  void* gathered[kMaxRanks];
+  for (int j = 0; j < comm->world; j++) gathered[j] = r.gathered + j * r.row_floats;
+  rc = b200c_allgather(comm, r.local, gathered, (size_t)2 * channels + 1, B200C_FLOAT32, stream);
+  if (rc) return rc;
+  RT(bn::sync_apply(a, comm->world, norm_fct, s));
+  g_launches.fetch_add(1 + rows);
+  return B200C_OK;
+}
+
+static int bn_backward(b200c_comm_t* comm, bool sync, const void* dy, const void* dy2, const void* y, const void* mask, int relu,
+                       const void* x, void* dy_masked, void* dx, const float* weight, const float* save_mean, const float* save_invstd,
+                       const float* norm_fct, float* grad_weight, float* grad_bias, int m, int channels, void* scratch,
+                       b200c_stream_t stream) {
+  int rc = check_bn(bn_site(sync), sync ? 0 : 1, m, channels, scratch, relu, mask, dy_masked, dy2);
+  if (rc) return rc;
+  if ((m && (!dy || !x || !dx || (relu && !y && !mask))) || !weight || !save_mean || !save_invstd || (sync && !norm_fct) ||
+      !grad_weight || !grad_bias)
+    return fail(B200C_EINVAL, "%s backward: null buffer", bn_site(sync));
+  const bn::BwdArgs a{dy, dy2, y, mask, x, dy_masked, dx, relu != 0, weight, save_mean, save_invstd, norm_fct, grad_weight, grad_bias,
+                      m, channels, scratch};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!sync) {
+    RT(bn::backward(a, s));
+    g_launches.fetch_add(2);
+    return B200C_OK;
+  }
+  rc = check_ready(comm);
+  if (rc) return rc;
+  DeviceGuard g(comm->device);
+  const int rows = m != 0;
+  RT(bn::sync_bwd_reduce(a, s));
+  g_launches.fetch_add(rows);
+  float* sums = bn::sync_rows(scratch, channels).sums;
+  rc = b200c_allreduce(comm, sums, sums, (size_t)2 * channels, B200C_FLOAT32, B200C_SUM, B200C_ALGO_AUTO, stream);
+  if (rc) return rc;
+  RT(bn::sync_bwd_elemt(a, s));
+  g_launches.fetch_add(rows);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward(const void* x, const void* identity, void* y, const float* weight, const float* bias,
+                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
+                                b200c_stream_t stream) {
+  return bn_forward(nullptr, false, x, identity, y, nullptr, 1, weight, bias, running_mean, running_var, num_batches_tracked, save_mean,
+                    save_invstd, nullptr, m, channels, momentum, eps, scratch, stream);
+}
+
+extern "C" int b200c_bn_forward_mask(const void* x, const void* identity, void* y, uint8_t* mask, const float* weight,
+                                     const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                                     float* save_mean, float* save_invstd, int m, int channels, float momentum, float eps,
+                                     void* scratch, b200c_stream_t stream) {
+  if (!mask) return fail(B200C_EINVAL, "batch norm mask: null mask");
+  return bn_forward(nullptr, false, x, identity, y, mask, 1, weight, bias, running_mean, running_var, num_batches_tracked, save_mean,
+                    save_invstd, nullptr, m, channels, momentum, eps, scratch, stream);
 }
 
 extern "C" int b200c_bn_sync_forward(b200c_comm_t* comm, const void* x, const void* identity, void* y, uint8_t* mask, int relu,
                                      const float* weight, const float* bias, float* running_mean, float* running_var,
                                      int64_t* num_batches_tracked, float* save_mean, float* save_invstd, float* norm_fct, int m,
                                      int channels, float momentum, float eps, void* scratch, b200c_stream_t stream) {
-  int rc = check_bn_sync(m, channels, scratch, relu, mask, identity, nullptr);
-  if (rc) return rc;
-  if ((m && (!x || !y)) || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !norm_fct)
-    return fail(B200C_EINVAL, "sync batch norm forward: null buffer");
-  rc = check_ready(comm);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  DeviceGuard g(comm->device);
-  bn::FwdArgs a{x, identity, y, mask, weight, bias, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked),
-                save_mean, save_invstd, m, channels, momentum, eps, scratch};
-  g_launches.fetch_add(bn::sync_stats(a, s));
-  RT(cudaGetLastError());
-  const bn::SyncRows r = bn::sync_rows(scratch, channels);
-  void* gathered[kMaxRanks];
-  for (int j = 0; j < comm->world; j++) gathered[j] = r.gathered + j * r.row_floats;
-  rc = b200c_allgather(comm, r.local, gathered, (size_t)2 * channels + 1, B200C_FLOAT32, stream);
-  if (rc) return rc;
-  g_launches.fetch_add(bn::sync_apply(a, relu != 0, comm->world, norm_fct, s));
-  RT(cudaGetLastError());
-  return B200C_OK;
+  return bn_forward(comm, true, x, identity, y, mask, relu, weight, bias, running_mean, running_var, num_batches_tracked, save_mean,
+                    save_invstd, norm_fct, m, channels, momentum, eps, scratch, stream);
+}
+
+extern "C" int b200c_bn_backward(const void* dy, const void* y, const void* x, void* dy_masked, void* dx, const float* weight,
+                                 const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
+                                 int channels, void* scratch, b200c_stream_t stream) {
+  return bn_backward(nullptr, false, dy, nullptr, y, nullptr, 1, x, dy_masked, dx, weight, save_mean, save_invstd, nullptr, grad_weight,
+                     grad_bias, m, channels, scratch, stream);
+}
+
+extern "C" int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask, const void* x, void* dy_masked,
+                                      void* dx, const float* weight, const float* save_mean, const float* save_invstd,
+                                      float* grad_weight, float* grad_bias, int m, int channels, void* scratch,
+                                      b200c_stream_t stream) {
+  if (!mask) return fail(B200C_EINVAL, "batch norm mask: null mask");
+  return bn_backward(nullptr, false, dy, dy2, nullptr, mask, 1, x, dy_masked, dx, weight, save_mean, save_invstd, nullptr, grad_weight,
+                     grad_bias, m, channels, scratch, stream);
 }
 
 extern "C" int b200c_bn_sync_backward(b200c_comm_t* comm, const void* dy, const void* dy2, const void* y, const uint8_t* mask, int relu,
                                       const void* x, void* dy_masked, void* dx, const float* weight, const float* save_mean,
                                       const float* save_invstd, const float* norm_fct, float* grad_weight, float* grad_bias, int m,
                                       int channels, void* scratch, b200c_stream_t stream) {
-  int rc = check_bn_sync(m, channels, scratch, relu, mask, dy_masked, dy2);
-  if (rc) return rc;
-  if ((m && (!dy || !x || !dx || (relu && !y && !mask))) || !weight || !save_mean || !save_invstd || !norm_fct || !grad_weight ||
-      !grad_bias)
-    return fail(B200C_EINVAL, "sync batch norm backward: null buffer");
-  rc = check_ready(comm);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  DeviceGuard g(comm->device);
-  bn::BwdArgs a{dy, dy2, y, mask, x, dy_masked, dx, weight, save_mean, save_invstd, grad_weight, grad_bias, m, channels, scratch};
-  g_launches.fetch_add(bn::sync_bwd_reduce(a, relu != 0, s));
-  RT(cudaGetLastError());
-  float* sums = bn::sync_rows(scratch, channels).sums;
-  rc = b200c_allreduce(comm, sums, sums, (size_t)2 * channels, B200C_FLOAT32, B200C_SUM, B200C_ALGO_AUTO, stream);
-  if (rc) return rc;
-  g_launches.fetch_add(bn::sync_bwd_elemt(a, relu != 0, norm_fct, s));
-  RT(cudaGetLastError());
-  return B200C_OK;
+  return bn_backward(comm, true, dy, dy2, y, mask, relu, x, dy_masked, dx, weight, save_mean, save_invstd, norm_fct, grad_weight,
+                     grad_bias, m, channels, scratch, stream);
 }
 
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {

@@ -1,5 +1,7 @@
 // Launchers of the fused batch-norm kernels (norm_kernels.cuh); argument checking lives in b200coll.cu.
 #include <algorithm>
+#include <initializer_list>
+#include <type_traits>
 
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
@@ -78,115 +80,159 @@ static Scratch carve(void* scratch, int stride) {
   return s;
 }
 
-// The transform after the statistics: k_bn_transform (ReLU, optionally after `+= identity`) or, without relu,
-// k_bn_sync_transform.
-static void launch_transform(const FwdArgs& a, bool relu, cudaStream_t st) {
+// ---- the kernels, by their runtime keys ----
+// The launchers and load_kernels() both get their kernels from the *_kernel functions below, so what is preloaded is
+// what can launch; keys without a kernel give null, which a launcher reports and load_kernels() skips.
+//
+// with_const calls f(std::integral_constant<int, C>) for the candidate C that equals `key` (as with_world_t does in
+// launch_typed.cuh) and returns the kernel f returns, or null without such a candidate.
+template <int... Cs, typename F>
+static auto with_const(int key, F&& f) {
+  std::common_type_t<decltype(f(std::integral_constant<int, Cs>{}))...> kernel = nullptr;
+  ((key == Cs ? void(kernel = f(std::integral_constant<int, Cs>{})) : void()), ...);
+  return kernel;
+}
+
+using StatsKernel = void (*)(const bf16*, StatsOut, volatile float*, int*, int, int);
+using SyncStatsKernel = void (*)(const bf16*, float*, float, volatile float*, int*, int, int);
+using TransformKernel = void (*)(const bf16*, const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*, int, int);
+using BwdReduceKernel = void (*)(const bf16*, const bf16*, const bf16*, const bf16*, const uint8_t*, bf16*, const float*, const float*,
+                                 float*, float*, float*, float*, volatile float*, int*, int, int);
+using BwdElemtKernel = void (*)(const bf16*, const bf16*, const bf16*, const uint8_t*, const bf16*, bf16*, const float*, const float*,
+                                const float*, const float*, const float*, const float*, float, int, int);
+
+static StatsKernel stats_kernel(int vec) {
+  return with_const<1, kStatsVec>(vec, [](auto v) -> StatsKernel { return k_bn_stats<decltype(v)::value>; });
+}
+static SyncStatsKernel sync_stats_kernel(int vec) {
+  return with_const<1, kStatsVec>(vec, [](auto v) -> SyncStatsKernel { return k_bn_sync_stats<decltype(v)::value>; });
+}
+static TransformKernel transform_kernel(int vec, int tail) {
+  return with_const<1, kEwVec>(vec, [&](auto v) {
+    return with_const<kTailNone, kTailRelu, kTailAddRelu>(
+        tail, [](auto t) -> TransformKernel { return k_bn_transform<decltype(v)::value, (Tail) decltype(t)::value>; });
+  });
+}
+// the reduce kernel computes g, so it has no kGradMasked
+static BwdReduceKernel bwd_reduce_kernel(int src) {
+  return with_const<kGradY, kGradBits, kGradDy>(
+      src, [](auto g) -> BwdReduceKernel { return k_bn_bwd_reduce<(GradSrc) decltype(g)::value>; });
+}
+static BwdElemtKernel bwd_elemt_kernel(int vec, int src, bool fct_ptr) {
+  return with_const<1, kEwVec>(vec, [&](auto v) {
+    return with_const<kGradMasked, kGradY, kGradBits, kGradDy>(src, [&](auto g) {
+      return with_const<false, true>(fct_ptr, [](auto p) -> BwdElemtKernel {
+        return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, decltype(p)::value != 0>;
+      });
+    });
+  });
+}
+
+// Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
+// load a kernel lazily while a peer's collective waits): every key value goes through the functions above.
+cudaError_t load_kernels() {
+  cudaFuncAttributes attr;
+  cudaError_t e = cudaSuccess;
+  auto load = [&](auto kernel) { if (kernel && e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel); };
+  load(&k_bn_sync_merge);
+  for (int src = 0; src < kGradSrcs; src++) load(bwd_reduce_kernel(src));
+  for (int vec : {1, kStatsVec, kEwVec}) {
+    load(stats_kernel(vec));
+    load(sync_stats_kernel(vec));
+    for (int tail = 0; tail < kTails; tail++) load(transform_kernel(vec, tail));
+    for (int src = 0; src < kGradSrcs; src++) {
+      load(bwd_elemt_kernel(vec, src, false));
+      load(bwd_elemt_kernel(vec, src, true));
+    }
+  }
+  return e;
+}
+
+// ---- launchers, shared by the local site and the sync phases ----
+// Each returns the launch's error, or kNoKernel when the dispatch has no kernel for the site's keys.
+constexpr cudaError_t kNoKernel = cudaErrorInvalidDeviceFunction;
+
+// The statistics: with `sync_row` this rank's row for the allgather (k_bn_sync_stats), else the site's own save and
+// running statistics (k_bn_stats).
+static cudaError_t launch_stats(const FwdArgs& a, float* sync_row, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const int vec = vec_ok(a.c, &a.x, 1) ? kStatsVec : 1;
+  block.x /= vec;
+  const bf16* x = static_cast<const bf16*>(a.x);
+  if (sync_row) {
+    const SyncStatsKernel k = sync_stats_kernel(vec);
+    if (!k) return kNoKernel;
+    k<<<grid, block, 0, st>>>(x, sync_row, a.eps, s.staging, s.semaphores, a.m, a.c);
+  } else {
+    const StatsKernel k = stats_kernel(vec);
+    if (!k) return kNoKernel;
+    StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
+               (float)((double)a.m / (double)(a.m - 1)), a.eps};
+    k<<<grid, block, 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
+  }
+  return cudaGetLastError();
+}
+
+static cudaError_t launch_transform(const FwdArgs& a, cudaStream_t st) {
   const void* ptrs[3] = {a.x, a.y, a.identity ? a.identity : a.x};
   const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
   dim3 block, grid;
   ew_config(a.m, a.c, vec, &block, &grid);
-  const bf16* x = static_cast<const bf16*>(a.x);
-  const bf16* id = static_cast<const bf16*>(a.identity);
-  bf16* y = static_cast<bf16*>(a.y);
-  uint8_t* mask = static_cast<uint8_t*>(a.mask);
-  if (!relu) {
-    if (vec == kEwVec) k_bn_sync_transform<kEwVec><<<grid, block, 0, st>>>(x, y, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c);
-    else k_bn_sync_transform<1><<<grid, block, 0, st>>>(x, y, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c);
-    return;
-  }
-#define B200C_BN_TRANSFORM(V, R) \
-  k_bn_transform<V, R><<<grid, block, 0, st>>>(x, id, y, mask, a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c)
-  if (vec == kEwVec) {
-    if (id) B200C_BN_TRANSFORM(kEwVec, true); else B200C_BN_TRANSFORM(kEwVec, false);
-  } else {
-    if (id) B200C_BN_TRANSFORM(1, true); else B200C_BN_TRANSFORM(1, false);
-  }
-#undef B200C_BN_TRANSFORM
+  const TransformKernel k = transform_kernel(vec, !a.relu ? kTailNone : a.identity ? kTailAddRelu : kTailRelu);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.identity), static_cast<bf16*>(a.y),
+                            static_cast<uint8_t*>(a.mask), a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c);
+  return cudaGetLastError();
 }
 
 cudaError_t forward(const FwdArgs& a, cudaStream_t st) {
+  const cudaError_t e = launch_stats(a, nullptr, st);
+  return e == cudaSuccess ? launch_transform(a, st) : e;
+}
+
+// Where a backward kernel takes g from.  The elementwise kernel runs after the reduce kernel (`reduced`), which at a
+// residual site has written g to dy_masked.
+static GradSrc grad_src(const BwdArgs& a, bool reduced) {
+  if (!a.relu) return kGradDy;
+  if (reduced && a.dy_masked) return kGradMasked;
+  return a.mask ? kGradBits : kGradY;
+}
+
+static cudaError_t launch_bwd_reduce(const BwdArgs& a, cudaStream_t st) {
   Scratch s = carve(a.scratch, a.c);
   dim3 block, grid;
   reduce_config(a.m, a.c, &block, &grid);
-  StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
-             (float)((double)a.m / (double)(a.m - 1)), a.eps};
-  const bf16* x = static_cast<const bf16*>(a.x);
-  if (vec_ok(a.c, &a.x, 1)) {
-    k_bn_stats<kStatsVec><<<grid, dim3(block.x / kStatsVec, block.y), 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
-  } else {
-    k_bn_stats<1><<<grid, block, 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
-  }
-  launch_transform(a, true, st);
+  const BwdReduceKernel k = bwd_reduce_kernel(grad_src(a, false));
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
+                            static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(a.mask), static_cast<bf16*>(a.dy_masked),
+                            a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m,
+                            a.c);
   return cudaGetLastError();
 }
 
-// The reduce kernel for g from dy and the ReLU's mask or output, or (relu false) g = dy.
-static void launch_bwd_reduce(const BwdArgs& a, bool relu, float* sum_dy, float* sum_dy_xmu, const Scratch& s, cudaStream_t st) {
-  dim3 block, grid;
-  reduce_config(a.m, a.c, &block, &grid);
-  const bf16* x = static_cast<const bf16*>(a.x);
-  const bf16* dy = static_cast<const bf16*>(a.dy);
-  const bf16* dy2 = static_cast<const bf16*>(a.dy2);
-  const bf16* y = static_cast<const bf16*>(a.y);
-  const uint8_t* mask = static_cast<const uint8_t*>(a.mask);
-  bf16* masked = static_cast<bf16*>(a.dy_masked);
-  if (!relu)
-    k_bn_sync_bwd_reduce<<<grid, block, 0, st>>>(x, dy, dy2, y, mask, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu,
-                                                 a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m, a.c);
-  else if (mask)
-    k_bn_bwd_reduce<true><<<grid, block, 0, st>>>(x, dy, dy2, y, mask, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu,
-                                                  a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m, a.c);
-  else
-    k_bn_bwd_reduce<false><<<grid, block, 0, st>>>(x, dy, dy2, y, mask, masked, a.save_mean, a.save_invstd, sum_dy, sum_dy_xmu,
-                                                   a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m, a.c);
-}
-
-// The elementwise kernel after the reduce: k_bn_bwd_elemt with a norm_fct value, or with norm_fct_ptr set
-// k_bn_sync_bwd_elemt, which reads it from the device.
-static void launch_bwd_elemt(const BwdArgs& a, bool relu, const float* sum_dy, const float* sum_dy_xmu, float norm_fct,
-                             const float* norm_fct_ptr, cudaStream_t st) {
-  const bf16* x = static_cast<const bf16*>(a.x);
-  const bf16* dy = static_cast<const bf16*>(a.dy);
-  const bf16* dy2 = static_cast<const bf16*>(a.dy2);
-  const bf16* y = static_cast<const bf16*>(a.y);
-  const uint8_t* mask = static_cast<const uint8_t*>(a.mask);
-  const bf16* masked = static_cast<const bf16*>(a.dy_masked);
-  // g comes from the tensor the reduce kernel wrote (tail), else from dy and the mask or y, or is dy (no ReLU)
-  const GradSrc src = !relu ? kGradDy : masked ? kGradMasked : mask ? kGradBits : kGradY;
-  const void* ptrs[5] = {a.x, a.dx, masked ? a.dy_masked : a.dy, dy2 && !masked ? a.dy2 : a.dy, a.y};
+// norm_fct is this call's (float)(1.0 / m) unless the site brings a pointer to its own (a sync site's).
+static cudaError_t launch_bwd_elemt(const BwdArgs& a, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  const GradSrc src = grad_src(a, true);
+  const void* g = src == kGradMasked ? a.dy_masked : a.dy;
+  const void* ptrs[5] = {a.x, a.dx, g, a.dy2 && src != kGradMasked ? a.dy2 : a.dy, a.y};
   const int vec = vec_ok(a.c, ptrs, src == kGradY ? 5 : 4) ? kEwVec : 1;
   dim3 block, grid;
   ew_config(a.m, a.c, vec, &block, &grid);
-  bf16* dx = static_cast<bf16*>(a.dx);
-#define B200C_BN_ELEMT(V, S, G)                                                                                               \
-  if (norm_fct_ptr)                                                                                                          \
-    k_bn_sync_bwd_elemt<V, S><<<grid, block, 0, st>>>(G, dy2, y, mask, x, dx, a.save_mean, a.save_invstd, a.weight, sum_dy,  \
-                                                      sum_dy_xmu, norm_fct_ptr, a.m, a.c);                                   \
-  else                                                                                                                       \
-    k_bn_bwd_elemt<V, S><<<grid, block, 0, st>>>(G, dy2, y, mask, x, dx, a.save_mean, a.save_invstd, a.weight, sum_dy,       \
-                                                 sum_dy_xmu, norm_fct, a.m, a.c);
-#define B200C_BN_ELEMT_SRC(V)                                    \
-  if (src == kGradMasked) { B200C_BN_ELEMT(V, kGradMasked, masked) } \
-  else if (src == kGradBits) { B200C_BN_ELEMT(V, kGradBits, dy) }    \
-  else if (src == kGradY) { B200C_BN_ELEMT(V, kGradY, dy) }          \
-  else if (norm_fct_ptr) { k_bn_sync_bwd_elemt<V, kGradDy><<<grid, block, 0, st>>>(dy, dy2, y, mask, x, dx, a.save_mean, \
-                             a.save_invstd, a.weight, sum_dy, sum_dy_xmu, norm_fct_ptr, a.m, a.c); }
-  if (vec == kEwVec) {
-    B200C_BN_ELEMT_SRC(kEwVec)
-  } else {
-    B200C_BN_ELEMT_SRC(1)
-  }
-#undef B200C_BN_ELEMT_SRC
-#undef B200C_BN_ELEMT
+  const BwdElemtKernel k = bwd_elemt_kernel(vec, src, a.norm_fct != nullptr);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(g), static_cast<const bf16*>(a.dy2), static_cast<const bf16*>(a.y),
+                            static_cast<const uint8_t*>(a.mask), static_cast<const bf16*>(a.x), static_cast<bf16*>(a.dx), a.save_mean,
+                            a.save_invstd, a.weight, s.sums, s.sums + a.c, a.norm_fct, (float)(1.0 / a.m), a.m, a.c);
+  return cudaGetLastError();
 }
 
 cudaError_t backward(const BwdArgs& a, cudaStream_t st) {
-  Scratch s = carve(a.scratch, a.c);
-  float* sum_dy = s.sums;
-  float* sum_dy_xmu = s.sums + a.c;
-  launch_bwd_reduce(a, true, sum_dy, sum_dy_xmu, s, st);
-  launch_bwd_elemt(a, true, sum_dy, sum_dy_xmu, (float)(1.0 / a.m), nullptr, st);
-  return cudaGetLastError();
+  const cudaError_t e = launch_bwd_reduce(a, st);
+  return e == cudaSuccess ? launch_bwd_elemt(a, st) : e;
 }
 
 // ---- sync batch norm ----
@@ -206,90 +252,33 @@ SyncRows sync_rows(void* scratch, int c) {
   return r;
 }
 
-int sync_stats(const FwdArgs& a, cudaStream_t st) {
+cudaError_t sync_stats(const FwdArgs& a, cudaStream_t st) {
   SyncRows r = sync_rows(a.scratch, a.c);
-  if (a.m == 0) {
-    // an empty rank still sends a row: zeros, count 0, which every rank's merge skips
-    cudaMemsetAsync(r.local, 0, ((size_t)2 * a.c + 1) * 4, st);
-    return 0;
-  }
-  Scratch s = carve(a.scratch, a.c);
-  dim3 block, grid;
-  reduce_config(a.m, a.c, &block, &grid);
-  const bf16* x = static_cast<const bf16*>(a.x);
-  if (vec_ok(a.c, &a.x, 1))
-    k_bn_sync_stats<kStatsVec><<<grid, dim3(block.x / kStatsVec, block.y), 0, st>>>(x, r.local, a.eps, s.staging, s.semaphores, a.m, a.c);
-  else
-    k_bn_sync_stats<1><<<grid, block, 0, st>>>(x, r.local, a.eps, s.staging, s.semaphores, a.m, a.c);
-  return 1;
+  // an empty rank still sends a row: zeros, count 0, which every rank's merge skips
+  if (a.m == 0) return cudaMemsetAsync(r.local, 0, ((size_t)2 * a.c + 1) * 4, st);
+  return launch_stats(a, r.local, st);
 }
 
-int sync_apply(const FwdArgs& a, bool relu, int world, float* norm_fct, cudaStream_t st) {
+cudaError_t sync_apply(const FwdArgs& a, int world, float* norm_fct, cudaStream_t st) {
   SyncRows r = sync_rows(a.scratch, a.c);
   k_bn_sync_merge<<<ceil_div(a.c, kEwThreads), kEwThreads, 0, st>>>(r.gathered, (int)r.row_floats, world, a.save_mean, a.save_invstd,
                                                                     norm_fct, a.running_mean, a.running_var, a.num_batches_tracked,
                                                                     a.momentum, a.eps, a.c);
-  if (a.m == 0) return 1;
-  launch_transform(a, relu, st);
-  return 2;
+  return a.m == 0 ? cudaGetLastError() : launch_transform(a, st);
 }
 
-int sync_bwd_reduce(const BwdArgs& a, bool relu, cudaStream_t st) {
-  Scratch s = carve(a.scratch, a.c);
+cudaError_t sync_bwd_reduce(const BwdArgs& a, cudaStream_t st) {
   if (a.m == 0) {
     // nothing to sum: zero sums for the allreduce, zero dweight and dbias
-    cudaMemsetAsync(s.sums, 0, (size_t)2 * a.c * 4, st);
+    cudaMemsetAsync(carve(a.scratch, a.c).sums, 0, (size_t)2 * a.c * 4, st);
     cudaMemsetAsync(a.grad_weight, 0, (size_t)a.c * 4, st);
     cudaMemsetAsync(a.grad_bias, 0, (size_t)a.c * 4, st);
-    return 0;
+    return cudaGetLastError();
   }
-  launch_bwd_reduce(a, relu, s.sums, s.sums + a.c, s, st);
-  return 1;
+  return launch_bwd_reduce(a, st);
 }
 
-// Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
-// load a kernel lazily while a peer's collective waits).
-cudaError_t load_kernels() {
-  cudaFuncAttributes attr;
-  cudaError_t e = cudaSuccess;
-  auto load = [&](auto kernel) { if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel); };
-  load(k_bn_stats<1>);
-  load(k_bn_stats<kStatsVec>);
-  load(k_bn_sync_stats<1>);
-  load(k_bn_sync_stats<kStatsVec>);
-  load(k_bn_sync_merge);
-  load(k_bn_bwd_reduce<false>);
-  load(k_bn_bwd_reduce<true>);
-  load(k_bn_sync_bwd_reduce);
-  load(k_bn_transform<1, false>);
-  load(k_bn_transform<1, true>);
-  load(k_bn_transform<kEwVec, false>);
-  load(k_bn_transform<kEwVec, true>);
-  load(k_bn_sync_transform<1>);
-  load(k_bn_sync_transform<kEwVec>);
-  load(k_bn_bwd_elemt<1, kGradMasked>);
-  load(k_bn_bwd_elemt<1, kGradY>);
-  load(k_bn_bwd_elemt<1, kGradBits>);
-  load(k_bn_bwd_elemt<kEwVec, kGradMasked>);
-  load(k_bn_bwd_elemt<kEwVec, kGradY>);
-  load(k_bn_bwd_elemt<kEwVec, kGradBits>);
-  load(k_bn_sync_bwd_elemt<1, kGradMasked>);
-  load(k_bn_sync_bwd_elemt<1, kGradY>);
-  load(k_bn_sync_bwd_elemt<1, kGradBits>);
-  load(k_bn_sync_bwd_elemt<1, kGradDy>);
-  load(k_bn_sync_bwd_elemt<kEwVec, kGradMasked>);
-  load(k_bn_sync_bwd_elemt<kEwVec, kGradY>);
-  load(k_bn_sync_bwd_elemt<kEwVec, kGradBits>);
-  load(k_bn_sync_bwd_elemt<kEwVec, kGradDy>);
-  return e;
-}
-
-int sync_bwd_elemt(const BwdArgs& a, bool relu, const float* norm_fct, cudaStream_t st) {
-  if (a.m == 0) return 0;
-  Scratch s = carve(a.scratch, a.c);
-  launch_bwd_elemt(a, relu, s.sums, s.sums + a.c, 0.f, norm_fct, st);
-  return 1;
-}
+cudaError_t sync_bwd_elemt(const BwdArgs& a, cudaStream_t st) { return a.m == 0 ? cudaSuccess : launch_bwd_elemt(a, st); }
 
 }  // namespace bn
 }  // namespace b200c

@@ -339,44 +339,21 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_sync_merge(const float* __res
   running_var[i] = __fmaf_rn(unbiased_var, momentum, __fmul_rn(1 - momentum, running_var[i]));
 }
 
-// y = bf16(bn(x)) (torch.batch_norm_elemt): k_bn_transform's expression without the ReLU, for a batch norm that
-// nothing is fused after.
-template <int V>
-__global__ void __launch_bounds__(kEwThreads) k_bn_sync_transform(const bf16* __restrict__ input, bf16* __restrict__ out,
-                                                                  const float* __restrict__ mean, const float* __restrict__ inv_std,
-                                                                  const float* __restrict__ weight, const float* __restrict__ shift,
-                                                                  const int reduction_size, const int stride) {
-  const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
-  if (c0 >= stride) return;
-  float m_c[V], inv_std_c[V], w_c[V], s_c[V];
-#pragma unroll
-  for (int j = 0; j < V; j++) {
-    m_c[j] = mean[c0 + j];
-    inv_std_c[j] = inv_std[c0 + j];
-    w_c[j] = weight[c0 + j];
-    s_c[j] = shift[c0 + j];
-  }
-  const int row_step = blockDim.y * gridDim.y;
-  for (int m = blockIdx.y * blockDim.y + threadIdx.y; m < reduction_size; m += row_step) {
-    const int a = m * stride + c0;
-    const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
-    BVec<V> yv;
-#pragma unroll
-    for (int j = 0; j < V; j++) yv.v[j] = __float2bfloat16(w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j]);
-    *reinterpret_cast<BVec<V>*>(out + a) = yv;
-  }
-}
+// What is fused after the batch norm: nothing, a ReLU, or `+= identity` and a ReLU (a block's tail).
+enum Tail { kTailNone, kTailRelu, kTailAddRelu };
+constexpr int kTails = 3;
 
-// y = relu(bn(x)) (RESID false) or y = relu(bf16(bn(x)) + identity) (RESID true), rounded where eager torch
-// rounds: the batch-norm output to bf16, the bf16 sum of the residual add to bf16.  `t <= 0 ? 0 : bf16(t)` is
-// relu(bf16(t)) because rounding keeps the sign; NaN passes through as in torch's relu.
+// y = bf16(bn(x)) (kTailNone: torch.batch_norm_elemt), y = relu(bn(x)) (kTailRelu) or y = relu(bf16(bn(x)) +
+// identity) (kTailAddRelu), rounded where eager torch rounds: the batch-norm output to bf16, the bf16 sum of the
+// residual add to bf16.  `t <= 0 ? 0 : bf16(t)` is relu(bf16(t)) because rounding keeps the sign; NaN passes
+// through as in torch's relu.
 //
-// With `mask` set (C % 8 == 0) the kernel also writes the ReLU's backward predicate !(y <= 0), computed from the
-// stored bf16 y, as one bit per element: element a = m * C + c is bit a % 8 of byte a / 8.  V = 8 threads write
-// one byte each per row.  V = 1 threads pack a byte with a ballot over the 8 lanes of one 8-channel group: block.x
-// = min(C, 256) is then a multiple of 8, so those lanes share a row and are all in or all out of range, and they
-// reach the ballot together or return together.
-template <int V, bool RESID>
+// With `mask` set (C % 8 == 0) a kernel with a ReLU also writes the ReLU's backward predicate !(y <= 0), computed
+// from the stored bf16 y, as one bit per element: element a = m * C + c is bit a % 8 of byte a / 8.  V = 8 threads
+// write one byte each per row.  V = 1 threads pack a byte with a ballot over the 8 lanes of one 8-channel group:
+// block.x = min(C, 256) is then a multiple of 8, so those lanes share a row and are all in or all out of range, and
+// they reach the ballot together or return together.
+template <int V, Tail TAIL>
 __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restrict__ input, const bf16* __restrict__ identity,
                                                              bf16* __restrict__ out, uint8_t* __restrict__ mask,
                                                              const float* __restrict__ mean, const float* __restrict__ inv_std,
@@ -400,22 +377,24 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
     const int a = m * stride + c0;
     const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
     BVec<V> zv;
-    if (RESID) zv = *reinterpret_cast<const BVec<V>*>(identity + a);
+    if (TAIL == kTailAddRelu) zv = *reinterpret_cast<const BVec<V>*>(identity + a);
     BVec<V> yv;
     unsigned bits = 0;
 #pragma unroll
     for (int j = 0; j < V; j++) {
       auto tmp = w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j];
-      if (RESID) {
+      if (TAIL == kTailAddRelu) {
         const bf16 r = __float2bfloat16(__bfloat162float(__float2bfloat16(tmp)) + __bfloat162float(zv.v[j]));
         yv.v[j] = __bfloat162float(r) <= 0.f ? __float2bfloat16(0.f) : r;
-      } else {
+      } else if (TAIL == kTailRelu) {
         yv.v[j] = tmp <= 0.f ? __float2bfloat16(0.f) : __float2bfloat16(tmp);
+      } else {
+        yv.v[j] = __float2bfloat16(tmp);
       }
       bits |= (unsigned)!(__bfloat162float(yv.v[j]) <= 0.f) << j;
     }
     *reinterpret_cast<BVec<V>*>(out + a) = yv;
-    if (mask) {
+    if (TAIL != kTailNone && mask) {
       if (V == 1) bits = (__ballot_sync(group, bits) >> (lane & ~7u)) & 0xffu;
       if (V == 8 || lane % 8 == 0) mask[a >> 3] = (uint8_t)bits;
     }
@@ -433,6 +412,7 @@ __device__ __forceinline__ bf16 add_grads(bf16 a, bf16 b) { return __float2bfloa
 // (kGradMasked), relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits), or dy itself, for
 // a batch norm without a ReLU after it (kGradDy).
 enum GradSrc { kGradMasked, kGradY, kGradBits, kGradDy };
+constexpr int kGradSrcs = 4;
 
 // Per-channel sums of g and g * (x - mean) with g from G (torch: batch_norm_backward_reduce_channels_last_kernel<4>),
 // and dweight / dbias.  kGradBits reads the ReLU's predicate from `mask` (k_bn_transform's bits) instead of y from
@@ -441,14 +421,12 @@ enum GradSrc { kGradMasked, kGradY, kGradBits, kGradDy };
 // tail, where g is also the identity branch's gradient) g is written there as well.  As in k_bn_stats, all rows of
 // an iteration are loaded before the first sum uses one.
 template <GradSrc G>
-__device__ __forceinline__ void bn_bwd_reduce_body(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
-                                                   const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
-                                                   const uint8_t* __restrict__ mask, bf16* __restrict__ masked,
-                                                   const float* __restrict__ mean, const float* __restrict__ inv_std,
-                                                   float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
-                                                   float* __restrict__ grad_weight, float* __restrict__ grad_bias,
-                                                   volatile float* staging_data, int* semaphores, const int reduction_size,
-                                                   const int stride) {
+__global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
+                                const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
+                                const uint8_t* __restrict__ mask, bf16* __restrict__ masked, const float* __restrict__ mean,
+                                const float* __restrict__ inv_std, float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
+                                float* __restrict__ grad_weight, float* __restrict__ grad_bias, volatile float* staging_data,
+                                int* semaphores, const int reduction_size, const int stride) {
   static_assert(G != kGradMasked, "the reduce kernel computes g");
   constexpr bool BITS = G == kGradBits;
   constexpr int PARALLEL_LOADS = kParallelLoads;
@@ -562,38 +540,25 @@ __device__ __forceinline__ void bn_bwd_reduce_body(const bf16* __restrict__ inpu
   }
 }
 
-#define B200C_BN_BWD_REDUCE_PARAMS                                                                                        \
-  const bf16 *__restrict__ input, const bf16 *__restrict__ grad_output, const bf16 *__restrict__ grad_output2,           \
-      const bf16 *__restrict__ output, const uint8_t *__restrict__ mask, bf16 *__restrict__ masked,                      \
-      const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy_o,                   \
-      float *__restrict__ sum_dy_xmu_o, float *__restrict__ grad_weight, float *__restrict__ grad_bias,                  \
-      volatile float *staging_data, int *semaphores, const int reduction_size, const int stride
-#define B200C_BN_BWD_REDUCE_ARGS                                                                                          \
-  input, grad_output, grad_output2, output, mask, masked, mean, inv_std, sum_dy_o, sum_dy_xmu_o, grad_weight, grad_bias, \
-      staging_data, semaphores, reduction_size, stride
-
-// g = relu_grad(dy, y), or with BITS relu_grad_bit(dy, mask)
-template <bool BITS>
-__global__ void k_bn_bwd_reduce(B200C_BN_BWD_REDUCE_PARAMS) {
-  bn_bwd_reduce_body<BITS ? kGradBits : kGradY>(B200C_BN_BWD_REDUCE_ARGS);
-}
-
-// g = dy: a batch norm without a ReLU after it
-__global__ void k_bn_sync_bwd_reduce(B200C_BN_BWD_REDUCE_PARAMS) { bn_bwd_reduce_body<kGradDy>(B200C_BN_BWD_REDUCE_ARGS); }
-
-#undef B200C_BN_BWD_REDUCE_ARGS
-#undef B200C_BN_BWD_REDUCE_PARAMS
-
-// dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g from G; dy is summed with `grad_output2`
-// when that is set, as in k_bn_bwd_reduce.
-template <int V, GradSrc G>
-__device__ __forceinline__ void bn_bwd_elemt_body(const bf16* __restrict__ grad_output, const bf16* __restrict__ grad_output2,
-                                                  const bf16* __restrict__ output, const uint8_t* __restrict__ mask,
-                                                  const bf16* __restrict__ input, bf16* __restrict__ grad_input,
-                                                  const float* __restrict__ mean, const float* __restrict__ inv_std,
-                                                  const float* __restrict__ weight, const float* __restrict__ sum_dy,
-                                                  const float* __restrict__ sum_dy_xmu, const float norm_fct,
-                                                  const int reduction_size, const int stride) {
+// dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g from G (kGradMasked: `grad_output` is the
+// tensor the reduce kernel wrote); dy is summed with `grad_output2` when that is set, as in k_bn_bwd_reduce.
+//
+// norm_fct is torch's 1 / rows.  A local site passes the value, (float)(1.0 / m) computed by the launcher from this
+// call's rows (FCT_PTR false); a sync site passes a pointer to what k_bn_sync_merge wrote, 1 / float(rows of all
+// ranks) (FCT_PTR true).  The choice is a template parameter because the two round differently, as torch's two
+// kernels do: with norm_fct a kernel parameter nvcc contracts `g - sum_dy * norm_fct` into one FMA per element,
+// with norm_fct loaded from memory it multiplies once per channel and subtracts.  One kernel that selects between
+// value and pointer at run time rounds a local site's dx like a sync site's, which is not eager torch's.
+template <int V, GradSrc G, bool FCT_PTR>
+__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restrict__ grad_output, const bf16* __restrict__ grad_output2,
+                                                             const bf16* __restrict__ output, const uint8_t* __restrict__ mask,
+                                                             const bf16* __restrict__ input, bf16* __restrict__ grad_input,
+                                                             const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                             const float* __restrict__ weight, const float* __restrict__ sum_dy,
+                                                             const float* __restrict__ sum_dy_xmu,
+                                                             const float* __restrict__ norm_fct_ptr, const float norm_fct_value,
+                                                             const int reduction_size, const int stride) {
+  const float norm_fct = FCT_PTR ? *norm_fct_ptr : norm_fct_value;
   const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   if (c0 >= stride) return;
   float m_c[V], m_dy_c[V], factor_1_c[V], factor_2_c[V];
@@ -626,30 +591,6 @@ __device__ __forceinline__ void bn_bwd_elemt_body(const bf16* __restrict__ grad_
     *reinterpret_cast<BVec<V>*>(grad_input + a) = dxv;
   }
 }
-
-#define B200C_BN_BWD_ELEMT_PARAMS                                                                                          \
-  const bf16 *__restrict__ grad_output, const bf16 *__restrict__ grad_output2, const bf16 *__restrict__ output,           \
-      const uint8_t *__restrict__ mask, const bf16 *__restrict__ input, bf16 *__restrict__ grad_input,                    \
-      const float *__restrict__ mean, const float *__restrict__ inv_std, const float *__restrict__ weight,                 \
-      const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xmu
-#define B200C_BN_BWD_ELEMT_ARGS grad_output, grad_output2, output, mask, input, grad_input, mean, inv_std, weight, sum_dy, sum_dy_xmu
-
-// norm_fct = (float)(1.0 / m), computed by the launcher from this call's rows
-template <int V, GradSrc G>
-__global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(B200C_BN_BWD_ELEMT_PARAMS, const float norm_fct, const int reduction_size,
-                                                             const int stride) {
-  bn_bwd_elemt_body<V, G>(B200C_BN_BWD_ELEMT_ARGS, norm_fct, reduction_size, stride);
-}
-
-// norm_fct read from k_bn_sync_merge's output: 1 / float(rows of all ranks)
-template <int V, GradSrc G>
-__global__ void __launch_bounds__(kEwThreads) k_bn_sync_bwd_elemt(B200C_BN_BWD_ELEMT_PARAMS, const float* __restrict__ norm_fct,
-                                                                  const int reduction_size, const int stride) {
-  bn_bwd_elemt_body<V, G>(B200C_BN_BWD_ELEMT_ARGS, *norm_fct, reduction_size, stride);
-}
-
-#undef B200C_BN_BWD_ELEMT_ARGS
-#undef B200C_BN_BWD_ELEMT_PARAMS
 
 }  // namespace bn
 }  // namespace b200c

@@ -11,6 +11,7 @@ struct FwdArgs {
   const void* identity;  // bf16 [m][c], or null: no residual add
   void* y;               // bf16 [m][c]
   void* mask;            // uint8 [m * c / 8], or null: receives the ReLU's predicate, one bit per element (c % 8 == 0)
+  bool relu;             // a ReLU follows the batch norm (and the residual add); without one, no identity and no mask
   const float* weight;
   const float* bias;
   float* running_mean;
@@ -31,9 +32,11 @@ struct BwdArgs {
   const void* x;         // bf16 [m][c], the batch norm's input
   void* dy_masked;       // bf16 [m][c], or null: receives the ReLU's input gradient (residual site)
   void* dx;              // bf16 [m][c]
+  bool relu;             // as in FwdArgs; without one, dy is the batch norm's output gradient: no y, mask, dy2 or dy_masked
   const float* weight;
   const float* save_mean;
   const float* save_invstd;
+  const float* norm_fct;  // device, 1 / float(rows of all ranks) of a sync site, or null: 1 / m
   float* grad_weight;
   float* grad_bias;
   int m, c;
@@ -51,7 +54,7 @@ cudaError_t backward(const BwdArgs& a, cudaStream_t s);  // 2 kernels
 //   forward:  sync_stats -> allgather of `local` (2c + 1 floats) into the W `gathered` rows -> sync_apply
 //   backward: sync_bwd_reduce -> allreduce SUM of `sums` (2c floats, in place) -> sync_bwd_elemt
 // FwdArgs.save_mean / save_invstd receive the global statistics, which the backward reads.  m may be 0: the rank
-// then sends zeros and launches only the merge.  Each phase returns the number of kernels it launched.
+// then sends zeros and launches only the merge; otherwise each phase launches one kernel, and sync_apply two.
 struct SyncRows {
   float* local;       // [mean (c) | invstd (c) | count], 16-byte aligned
   float* gathered;    // W rows like `local`, row_floats apart (16-byte aligned)
@@ -60,11 +63,11 @@ struct SyncRows {
 };
 size_t sync_scratch_bytes(int c, int world);
 SyncRows sync_rows(void* scratch, int c);
-int sync_stats(const FwdArgs& a, cudaStream_t s);
-int sync_apply(const FwdArgs& a, bool relu, int world, float* norm_fct, cudaStream_t s);
-int sync_bwd_reduce(const BwdArgs& a, bool relu, cudaStream_t s);
-int sync_bwd_elemt(const BwdArgs& a, bool relu, const float* norm_fct, cudaStream_t s);
-cudaError_t load_kernels();   // every kernel above, into the current context
+cudaError_t sync_stats(const FwdArgs& a, cudaStream_t s);
+cudaError_t sync_apply(const FwdArgs& a, int world, float* norm_fct, cudaStream_t s);
+cudaError_t sync_bwd_reduce(const BwdArgs& a, cudaStream_t s);
+cudaError_t sync_bwd_elemt(const BwdArgs& a, cudaStream_t s);
+cudaError_t load_kernels();   // every batch-norm kernel, into the current context
 
 }  // namespace bn
 }  // namespace b200c

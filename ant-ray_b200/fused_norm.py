@@ -38,7 +38,7 @@ _lib = None
 # channel count (the library keeps its semaphores in a region no call's staging overlaps); calls on one stream
 # are ordered.
 _scratch = {}
-_scratch_need = {}   # channels -> b200c_bn_scratch_bytes(channels); 0: more channels than the kernels take
+_scratch_need = {}   # (channels, world or None) -> the library's scratch bytes; 0: more channels than the kernels take
 _NATIVE = torch._C._BatchNormBackend.Native
 # the current stream's handle without building a torch.cuda.Stream object: each step makes 98 fused calls
 _raw_stream = torch._C._cuda_getCurrentRawStream
@@ -51,18 +51,14 @@ def _native_lib():
     return _lib
 
 
-def _scratch_bytes(channels):
-    need = _scratch_need.get(channels)
-    if need is None:
-        need = _scratch_need[channels] = int(_native_lib().b200c_bn_scratch_bytes(channels))
-    return need
-
-
-def _sync_scratch_bytes(channels, world):
+def _scratch_bytes(channels, world=None):
+    """The scratch a site of `channels` needs: a local site's, or with `world` a sync site's over that many ranks."""
     key = (channels, world)
     need = _scratch_need.get(key)
     if need is None:
-        need = _scratch_need[key] = int(_native_lib().b200c_bn_sync_scratch_bytes(channels, world))
+        lib = _native_lib()
+        need = lib.b200c_bn_scratch_bytes(channels) if world is None else lib.b200c_bn_sync_scratch_bytes(channels, world)
+        need = _scratch_need[key] = int(need)
     return need
 
 
@@ -93,41 +89,33 @@ class _FusedBatchNorm(torch.autograd.Function):
         m = x.numel() // c
         y = torch.empty_like(x)
         nbt = bn.num_batches_tracked
-        nbt_ptr = nbt.data_ptr() if nbt is not None else None
         id_ptr = identity.data_ptr() if identity is not None else None
         ctx.residual = identity is not None
         ctx.comm, ctx.relu = comm, relu
         ctx.set_materialize_grads(False)
+        # what the backward reads of the ReLU: its mask (where C % 8 == 0), else y; nothing at a site without ReLU, whose
+        # output may then be modified in place (an inplace ReLU or `+= identity` after a SyncBatchNorm)
+        masked = relu and c % 8 == 0
+        relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if masked else y if relu else None
+        mask_ptr = relu_src.data_ptr() if masked else None
+        # stats = [save_mean (c) | save_invstd (c)], followed at a sync site by norm_fct: there the statistics are the
+        # global ones and norm_fct is the backward's 1 / rows of all ranks
+        stats = torch.empty(2 * c + (comm is not None), dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        params = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                  nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c)
         if comm is not None:
             stream = comm.stream().cuda_stream
-            # stats = [save_mean (c) | save_invstd (c) | norm_fct]: the global statistics and the backward's 1 / rows
-            stats = torch.empty(2 * c + 1, dtype=torch.float32, device=x.device)
-            mean = stats.data_ptr()
-            # what the backward reads of the ReLU: its mask, else y; nothing at a site without ReLU, whose output may
-            # then be modified in place (an inplace ReLU or `+= identity` after a SyncBatchNorm)
-            relu_src = None
-            if relu:
-                relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if c % 8 == 0 else y
-            mask_ptr = relu_src.data_ptr() if relu_src is not None and relu_src.dtype == torch.uint8 else None
-            scratch = _scratch_ptr(x.device, stream, _sync_scratch_bytes(c, comm.world_size))
-            N.check(lib.b200c_bn_sync_forward(comm._h(), x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, int(relu),
-                                              weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(),
-                                              bn.running_var.data_ptr(), nbt_ptr, mean, mean + 4 * c, mean + 8 * c, m, c,
-                                              bn.momentum, bn.eps, scratch, stream))
-            ctx.save_for_backward(x, relu_src, weight, stats)
-            return (y, y.view_as(y)) if pair else y
-        stats = torch.empty(2, c, dtype=torch.float32, device=x.device)
-        stream = _raw_stream(x.device.index)
-        mean = stats.data_ptr()   # stats = [save_mean; save_invstd]
-        args = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                nbt_ptr, mean, mean + 4 * c,
-                m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_need[c]), stream)
-        if c % 8 == 0:
-            relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device)
-            N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), relu_src.data_ptr(), *args))
+            scratch = _scratch_ptr(x.device, stream, _scratch_bytes(c, comm.world_size))
+            N.check(lib.b200c_bn_sync_forward(comm._h(), x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, int(relu), *params,
+                                              mean + 8 * c, m, c, bn.momentum, bn.eps, scratch, stream))
         else:
-            relu_src = y
-            N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *args))
+            stream = _raw_stream(x.device.index)
+            site = (m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream)
+            if masked:
+                N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, *params, *site))
+            else:
+                N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *params, *site))
         ctx.save_for_backward(x, relu_src, weight, stats)
         return (y, y.view_as(y)) if pair else y
 
@@ -136,8 +124,9 @@ class _FusedBatchNorm(torch.autograd.Function):
     def backward(ctx, *grads):
         grads = [g.contiguous(memory_format=torch.channels_last) for g in grads if g is not None]
         x, relu_src, weight, stats = ctx.saved_tensors
+        comm = ctx.comm
         if not grads:
-            if ctx.comm is None:
+            if comm is None:
                 return None, None, None, None, None, None, None, None
             # the other ranks wait in this site's all-reduce: join it with a zero gradient
             grads = [torch.zeros_like(x, memory_format=torch.channels_last)]
@@ -150,13 +139,13 @@ class _FusedBatchNorm(torch.autograd.Function):
         grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
         mean = stats.data_ptr()
         did_ptr = d_identity.data_ptr() if d_identity is not None else None
-        if ctx.comm is not None:
-            comm = ctx.comm
+        # the forward's relu_src: the mask, y, or nothing
+        mask = relu_src.data_ptr() if relu_src is not None and relu_src.dtype == torch.uint8 else None
+        y = relu_src.data_ptr() if relu_src is not None and mask is None else None
+        dy2 = grads[1].data_ptr() if len(grads) == 2 else None
+        if comm is not None:
             stream = comm.stream().cuda_stream
-            scratch = _scratch_ptr(x.device, stream, _sync_scratch_bytes(c, comm.world_size))
-            mask = relu_src.data_ptr() if ctx.relu and relu_src.dtype == torch.uint8 else None
-            y = relu_src.data_ptr() if ctx.relu and mask is None else None
-            dy2 = grads[1].data_ptr() if len(grads) == 2 else None
+            scratch = _scratch_ptr(x.device, stream, _scratch_bytes(c, comm.world_size))
             N.check(lib.b200c_bn_sync_backward(comm._h(), grads[0].data_ptr(), dy2, y, mask, int(ctx.relu), x.data_ptr(),
                                                did_ptr, dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, mean + 8 * c,
                                                grad_weight.data_ptr(), grad_bias.data_ptr(), m, c, scratch, stream))
@@ -165,15 +154,13 @@ class _FusedBatchNorm(torch.autograd.Function):
                 return None, d_identity, None, None, None, None, None, None
             return dx, d_identity, grad_weight, grad_bias, None, None, None, None
         stream = _raw_stream(x.device.index)
-        args = (x.data_ptr(), did_ptr, dx.data_ptr(), weight.data_ptr(),
-                mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c,
-                _scratch_ptr(x.device, stream, _scratch_need[c]), stream)
-        if relu_src.dtype == torch.uint8:
-            dy2 = grads[1].data_ptr() if len(grads) == 2 else None
-            N.check(lib.b200c_bn_backward_mask(grads[0].data_ptr(), dy2, relu_src.data_ptr(), *args))
+        site = (x.data_ptr(), did_ptr, dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
+                grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream)
+        if mask is not None:
+            N.check(lib.b200c_bn_backward_mask(grads[0].data_ptr(), dy2, mask, *site))
         else:
-            dy = grads[0] + grads[1] if len(grads) == 2 else grads[0]
-            N.check(lib.b200c_bn_backward(dy.data_ptr(), relu_src.data_ptr(), *args))
+            dy = grads[0] + grads[1] if dy2 is not None else grads[0]   # this call takes one gradient
+            N.check(lib.b200c_bn_backward(dy.data_ptr(), y, *site))
         return dx, d_identity, grad_weight, grad_bias, None, None, None, None
 
 
@@ -191,22 +178,31 @@ def _torch_syncs(bn):
     return dist.get_world_size(bn.process_group or dist.group.WORLD) > 1
 
 
+def _module_ok(bn):
+    """The module-side conditions of every fused site, local or sync: training mode, tracked running statistics, a
+    numeric momentum, and affine weight, bias and running statistics in contiguous fp32."""
+    if not bn.training or not bn.track_running_stats or not isinstance(bn.momentum, numbers.Real):
+        return False
+    return all(t is not None and t.dtype == torch.float32 and t.is_contiguous()
+               for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+
+
+def _relu_fusable(bn, relu):
+    return type(relu) is nn.ReLU and not bn._forward_hooks and not bn._forward_pre_hooks
+
+
 def _fusable(bn, relu, x):
-    """Whether this site can run fused: the conditions of the module docstring."""
+    """Whether this site can run fused as a local site: the conditions of the module docstring.  A site that cannot
+    falls back to the parent class's ops."""
     local = type(bn) is nn.BatchNorm2d or (isinstance(bn, nn.SyncBatchNorm) and not _torch_syncs(bn))
-    if not local or type(relu) is not nn.ReLU or not bn.training or not bn.track_running_stats:
+    if not local or not _relu_fusable(bn, relu) or not _module_ok(bn):
         return False
-    w, b, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
-    if w is None or b is None or rm is None or bn._forward_hooks or bn._forward_pre_hooks:
-        return False
-    if not isinstance(bn.momentum, numbers.Real) or not _activation(x) or x.numel() >= 2 ** 31:
+    if not _activation(x) or x.numel() >= 2 ** 31:
         return False
     # one value per channel: torch's batch_norm raises ("Expected more than 1 value per channel"), so must we
     if x.numel() // x.shape[1] <= 1 or not _scratch_bytes(x.shape[1]):
         return False
-    if any(t.dtype != torch.float32 or not t.is_contiguous() for t in (w, b, rm, rv)):
-        return False
-    return torch._C._select_batch_norm_backend(x, w, b, rm, rv, True, bn.eps) == _NATIVE
+    return torch._C._select_batch_norm_backend(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, True, bn.eps) == _NATIVE
 
 
 def _rows(t):
@@ -221,21 +217,12 @@ def _sync_comm(bn, x):
     every rank meets alike decide; an input the kernels cannot take raises instead of falling back, since the other
     ranks would wait in this site's collectives."""
     comm = getattr(bn, "b200_comm", None)
-    if comm is None or comm.world_size <= 1 or not bn.training or not bn.track_running_stats:
+    if comm is None or comm.world_size <= 1 or not _module_ok(bn) or not _rows(x):
         return None
-    w, b, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
-    if w is None or b is None or rm is None or not isinstance(bn.momentum, numbers.Real) or not _rows(x):
-        return None
-    if any(t.dtype != torch.float32 or not t.is_contiguous() for t in (w, b, rm, rv)):
-        return None
-    if x.numel() >= 2 ** 31 or not _sync_scratch_bytes(x.shape[1], comm.world_size):
+    if x.numel() >= 2 ** 31 or not _scratch_bytes(x.shape[1], comm.world_size):
         raise RuntimeError(f"sync batch norm: input of shape {tuple(x.shape)} exceeds the kernels' limits "
                            "(< 2^31 elements, at most 131072 channels)")
     return comm
-
-
-def _relu_fusable(bn, relu):
-    return type(relu) is nn.ReLU and not bn._forward_hooks and not bn._forward_pre_hooks
 
 
 def bn_relu(bn, relu, x):

@@ -44,7 +44,9 @@ def families(prof):
 
     from step_profile import FAMILIES
 
-    fams = [("bn_sync", r"k_bn_sync")] + FAMILIES
+    # bn_sync: the sync statistics and merge kernels only; a sync site's transform, backward reduce and backward
+    # elementwise kernels are the local sites' and count in their families
+    fams = [("bn_sync", r"k_bn_sync_(stats|merge)")] + FAMILIES
     out = {}
     for e in prof.key_averages():
         if e.device_type != torch.autograd.DeviceType.CUDA and not getattr(e, "self_device_time_total", 0):

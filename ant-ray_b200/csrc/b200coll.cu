@@ -1496,6 +1496,105 @@ extern "C" int b200c_bn_sync_backward(b200c_comm_t* comm, const void* dy, const 
                      grad_bias, m, channels, scratch, stream);
 }
 
+// A tail whose identity is a downsample branch's batch norm.
+extern "C" size_t b200c_bn_dual_scratch_bytes(int channels) {
+  return channels < 1 || channels > bn::kMaxChannels / 2 ? 0 : bn::dual_scratch_bytes(channels);
+}
+
+static int check_dual(int channels) {
+  if (channels > bn::kMaxChannels / 2) return fail(B200C_EINVAL, "batch norm dual: channels=%d above %d", channels, bn::kMaxChannels / 2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_dual(const void* x, const void* x_ds, void* y, uint8_t* mask, const float* weight, const float* bias,
+                                     float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                     float* save_invstd, float momentum, float eps, const float* weight_ds, const float* bias_ds,
+                                     float* running_mean_ds, float* running_var_ds, int64_t* num_batches_tracked_ds,
+                                     float* save_mean_ds, float* save_invstd_ds, float momentum_ds, float eps_ds, int m, int channels,
+                                     void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm dual", 1, m, channels, scratch, 1, mask, x_ds, nullptr);
+  if (!rc) rc = check_dual(channels);
+  if (rc) return rc;
+  if (!x || !x_ds || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !weight_ds ||
+      !bias_ds || !running_mean_ds || !running_var_ds || !save_mean_ds || !save_invstd_ds)
+    return fail(B200C_EINVAL, "batch norm dual forward: null buffer");
+  const bn::FwdArgs a{x, nullptr, y, mask, true, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  const bn::FwdArgs b{x_ds, nullptr, nullptr, nullptr, false, weight_ds, bias_ds, running_mean_ds, running_var_ds,
+                      reinterpret_cast<long long*>(num_batches_tracked_ds), save_mean_ds, save_invstd_ds, m, channels, momentum_ds,
+                      eps_ds, scratch};
+  RT(bn::forward_dual(a, b, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_dual(const void* dy, const void* dy2, const void* y, const uint8_t* mask, const void* x,
+                                      const void* x_ds, void* dx, void* dx_ds, const float* weight, const float* save_mean,
+                                      const float* save_invstd, float* grad_weight, float* grad_bias, const float* weight_ds,
+                                      const float* save_mean_ds, const float* save_invstd_ds, float* grad_weight_ds,
+                                      float* grad_bias_ds, int m, int channels, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm dual", 1, m, channels, scratch, 1, mask, nullptr, dy2);
+  if (!rc) rc = check_dual(channels);
+  if (rc) return rc;
+  if (!dy || (!y && !mask) || !x || !x_ds || !dx || !dx_ds || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias ||
+      !weight_ds || !save_mean_ds || !save_invstd_ds || !grad_weight_ds || !grad_bias_ds)
+    return fail(B200C_EINVAL, "batch norm dual backward: null buffer");
+  const bn::BwdArgs a{dy, dy2, mask ? nullptr : y, mask, x, nullptr, dx, true, weight, save_mean, save_invstd, nullptr, grad_weight,
+                      grad_bias, m, channels, scratch};
+  const bn::BwdArgs b{nullptr, nullptr, nullptr, nullptr, x_ds, nullptr, dx_ds, false, weight_ds, save_mean_ds, save_invstd_ds, nullptr,
+                      grad_weight_ds, grad_bias_ds, m, channels, scratch};
+  RT(bn::backward_dual(a, b, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+// The stem: n images of h x w rows.  The shape is checked in 64 bits before it becomes the site's m.
+static int check_pool(const char* dir, int n, int h, int w, int channels, int* m) {
+  if (n < 1 || h < 1 || w < 1 || (int64_t)n * h * w > INT32_MAX)
+    return fail(B200C_EINVAL, "batch norm pool %s: bad shape n=%d h=%d w=%d c=%d", dir, n, h, w, channels);
+  *m = n * h * w;
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_pool(const void* x, void* y, uint8_t* argmax, const float* weight, const float* bias,
+                                     float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                     float* save_invstd, int n, int h, int w, int channels, float momentum, float eps, void* scratch,
+                                     b200c_stream_t stream) {
+  int m = 0;
+  int rc = check_pool("forward", n, h, w, channels, &m);
+  if (!rc) rc = check_bn("batch norm pool", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (rc) return rc;
+  if (!x || !y || !argmax || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
+    return fail(B200C_EINVAL, "batch norm pool forward: null buffer");
+  bn::FwdArgs a{x, nullptr, y, nullptr, true, weight, bias, running_mean, running_var,
+                reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  a.argmax = argmax;
+  a.pool_h = h;
+  a.pool_w = w;
+  RT(bn::forward(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_pool(const void* dy, const uint8_t* argmax, const void* x, void* g, void* dx, const float* weight,
+                                      const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
+                                      int h, int w, int channels, void* scratch, b200c_stream_t stream) {
+  int m = 0;
+  int rc = check_pool("backward", n, h, w, channels, &m);
+  if (!rc) rc = check_bn("batch norm pool", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (rc) return rc;
+  if (!dy || !argmax || !x || !g || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias)
+    return fail(B200C_EINVAL, "batch norm pool backward: null buffer");
+  bn::BwdArgs a{dy, nullptr, nullptr, nullptr, x, g, dx, true, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                m, channels, scratch};
+  a.argmax = argmax;
+  a.pool_h = h;
+  a.pool_w = w;
+  RT(bn::backward(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {
   int rc = check_ready(c);
   if (rc) return rc;

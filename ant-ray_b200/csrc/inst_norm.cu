@@ -95,34 +95,51 @@ static auto with_const(int key, F&& f) {
 
 using StatsKernel = void (*)(const bf16*, StatsOut, volatile float*, int*, int, int);
 using SyncStatsKernel = void (*)(const bf16*, float*, float, volatile float*, int*, int, int);
-using TransformKernel = void (*)(const bf16*, const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*, int, int);
+using StatsDualKernel = void (*)(const bf16*, const bf16*, StatsOut, StatsOut, volatile float*, volatile float*, int*, int, int);
+using TransformKernel = void (*)(const bf16*, const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*,
+                                 const float*, const float*, const float*, const float*, int, int);
+using PoolFwdKernel = void (*)(const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*, PoolDims, int, int);
 using BwdReduceKernel = void (*)(const bf16*, const bf16*, const bf16*, const bf16*, const uint8_t*, bf16*, const float*, const float*,
-                                 float*, float*, float*, float*, volatile float*, int*, int, int);
+                                 float*, float*, float*, float*, volatile float*, int*, PoolDims, const bf16*, const float*, const float*,
+                                 float*, float*, float*, int, int);
 using BwdElemtKernel = void (*)(const bf16*, const bf16*, const bf16*, const uint8_t*, const bf16*, bf16*, const float*, const float*,
-                                const float*, const float*, const float*, const float*, float, int, int);
+                                const float*, const float*, const float*, const float*, float, const bf16*, bf16*, const float*,
+                                const float*, const float*, const float*, int, int);
 
 static StatsKernel stats_kernel(int vec) {
   return with_const<1, kStatsVec>(vec, [](auto v) -> StatsKernel { return k_bn_stats<decltype(v)::value>; });
+}
+static StatsDualKernel stats_dual_kernel(int vec) {
+  return with_const<1, kStatsVec>(vec, [](auto v) -> StatsDualKernel { return k_bn_stats_dual<decltype(v)::value>; });
 }
 static SyncStatsKernel sync_stats_kernel(int vec) {
   return with_const<1, kStatsVec>(vec, [](auto v) -> SyncStatsKernel { return k_bn_sync_stats<decltype(v)::value>; });
 }
 static TransformKernel transform_kernel(int vec, int tail) {
   return with_const<1, kEwVec>(vec, [&](auto v) {
-    return with_const<kTailNone, kTailRelu, kTailAddRelu>(
+    return with_const<kTailNone, kTailRelu, kTailAddRelu, kTailBnAddRelu>(
         tail, [](auto t) -> TransformKernel { return k_bn_transform<decltype(v)::value, (Tail) decltype(t)::value>; });
   });
 }
-// the reduce kernel computes g, so it has no kGradMasked
-static BwdReduceKernel bwd_reduce_kernel(int src) {
-  return with_const<kGradY, kGradBits, kGradDy>(
-      src, [](auto g) -> BwdReduceKernel { return k_bn_bwd_reduce<(GradSrc) decltype(g)::value>; });
+static PoolFwdKernel pool_fwd_kernel(int vec) {
+  return with_const<1, kEwVec>(vec, [](auto v) -> PoolFwdKernel { return k_bn_pool_fwd<decltype(v)::value>; });
 }
-static BwdElemtKernel bwd_elemt_kernel(int vec, int src, bool fct_ptr) {
+// the reduce kernel computes g, so it has no kGradMasked; a dual tail (a local site) reads y or its mask bits
+static BwdReduceKernel bwd_reduce_kernel(int src, bool dual) {
+  if (dual)
+    return with_const<kGradY, kGradBits>(src, [](auto g) -> BwdReduceKernel { return k_bn_bwd_reduce<(GradSrc) decltype(g)::value, true>; });
+  return with_const<kGradY, kGradBits, kGradDy, kGradPool>(
+      src, [](auto g) -> BwdReduceKernel { return k_bn_bwd_reduce<(GradSrc) decltype(g)::value, false>; });
+}
+static BwdElemtKernel bwd_elemt_kernel(int vec, int src, bool fct_ptr, bool dual) {
   return with_const<1, kEwVec>(vec, [&](auto v) {
+    if (dual)
+      return with_const<kGradY, kGradBits>(src, [](auto g) -> BwdElemtKernel {
+        return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, false, true>;
+      });
     return with_const<kGradMasked, kGradY, kGradBits, kGradDy>(src, [&](auto g) {
       return with_const<false, true>(fct_ptr, [](auto p) -> BwdElemtKernel {
-        return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, decltype(p)::value != 0>;
+        return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, decltype(p)::value != 0, false>;
       });
     });
   });
@@ -135,15 +152,19 @@ cudaError_t load_kernels() {
   cudaError_t e = cudaSuccess;
   auto load = [&](auto kernel) { if (kernel && e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel); };
   load(&k_bn_sync_merge);
-  for (int src = 0; src < kGradSrcs; src++) load(bwd_reduce_kernel(src));
+  for (int src = 0; src < kGradSrcs; src++) {
+    load(bwd_reduce_kernel(src, false));
+    load(bwd_reduce_kernel(src, true));
+  }
   for (int vec : {1, kStatsVec, kEwVec}) {
     load(stats_kernel(vec));
+    load(stats_dual_kernel(vec));
     load(sync_stats_kernel(vec));
+    load(pool_fwd_kernel(vec));
     for (int tail = 0; tail < kTails; tail++) load(transform_kernel(vec, tail));
-    for (int src = 0; src < kGradSrcs; src++) {
-      load(bwd_elemt_kernel(vec, src, false));
-      load(bwd_elemt_kernel(vec, src, true));
-    }
+    for (int src = 0; src < kGradSrcs; src++)
+      for (bool fct_ptr : {false, true})
+        for (bool dual : {false, true}) load(bwd_elemt_kernel(vec, src, fct_ptr, dual));
   }
   return e;
 }
@@ -183,20 +204,40 @@ static cudaError_t launch_transform(const FwdArgs& a, cudaStream_t st) {
   const TransformKernel k = transform_kernel(vec, !a.relu ? kTailNone : a.identity ? kTailAddRelu : kTailRelu);
   if (!k) return kNoKernel;
   k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.identity), static_cast<bf16*>(a.y),
-                            static_cast<uint8_t*>(a.mask), a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c);
+                            static_cast<uint8_t*>(a.mask), a.save_mean, a.save_invstd, a.weight, a.bias, nullptr, nullptr, nullptr,
+                            nullptr, a.m, a.c);
+  return cudaGetLastError();
+}
+
+static PoolDims pool_dims(int h, int w) { return PoolDims{h, w, (h - 1) / 2 + 1, (w - 1) / 2 + 1}; }
+
+// The stem's pooling: one thread per pooled element and 8 (or 1) channels.
+static cudaError_t launch_pool_fwd(const FwdArgs& a, cudaStream_t st) {
+  const PoolDims d = pool_dims(a.pool_h, a.pool_w);
+  const int pooled_rows = a.m / (a.pool_h * a.pool_w) * d.oh * d.ow;
+  const void* ptrs[3] = {a.x, a.y, a.argmax};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(pooled_rows, a.c, vec, &block, &grid);
+  const PoolFwdKernel k = pool_fwd_kernel(vec);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), static_cast<uint8_t*>(a.argmax), a.save_mean,
+                            a.save_invstd, a.weight, a.bias, d, pooled_rows, a.c);
   return cudaGetLastError();
 }
 
 cudaError_t forward(const FwdArgs& a, cudaStream_t st) {
   const cudaError_t e = launch_stats(a, nullptr, st);
-  return e == cudaSuccess ? launch_transform(a, st) : e;
+  if (e != cudaSuccess) return e;
+  return a.pool_h ? launch_pool_fwd(a, st) : launch_transform(a, st);
 }
 
 // Where a backward kernel takes g from.  The elementwise kernel runs after the reduce kernel (`reduced`), which at a
-// residual site has written g to dy_masked.
+// residual site and at the stem has written g to dy_masked.
 static GradSrc grad_src(const BwdArgs& a, bool reduced) {
   if (!a.relu) return kGradDy;
   if (reduced && a.dy_masked) return kGradMasked;
+  if (a.pool_h) return kGradPool;
   return a.mask ? kGradBits : kGradY;
 }
 
@@ -204,12 +245,14 @@ static cudaError_t launch_bwd_reduce(const BwdArgs& a, cudaStream_t st) {
   Scratch s = carve(a.scratch, a.c);
   dim3 block, grid;
   reduce_config(a.m, a.c, &block, &grid);
-  const BwdReduceKernel k = bwd_reduce_kernel(grad_src(a, false));
+  const GradSrc src = grad_src(a, false);
+  const BwdReduceKernel k = bwd_reduce_kernel(src, false);
   if (!k) return kNoKernel;
+  const void* mask = src == kGradPool ? a.argmax : a.mask;
   k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
-                            static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(a.mask), static_cast<bf16*>(a.dy_masked),
-                            a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m,
-                            a.c);
+                            static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(mask), static_cast<bf16*>(a.dy_masked),
+                            a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores,
+                            pool_dims(a.pool_h, a.pool_w), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.m, a.c);
   return cudaGetLastError();
 }
 
@@ -222,17 +265,86 @@ static cudaError_t launch_bwd_elemt(const BwdArgs& a, cudaStream_t st) {
   const int vec = vec_ok(a.c, ptrs, src == kGradY ? 5 : 4) ? kEwVec : 1;
   dim3 block, grid;
   ew_config(a.m, a.c, vec, &block, &grid);
-  const BwdElemtKernel k = bwd_elemt_kernel(vec, src, a.norm_fct != nullptr);
+  const BwdElemtKernel k = bwd_elemt_kernel(vec, src, a.norm_fct != nullptr, false);
   if (!k) return kNoKernel;
   k<<<grid, block, 0, st>>>(static_cast<const bf16*>(g), static_cast<const bf16*>(a.dy2), static_cast<const bf16*>(a.y),
                             static_cast<const uint8_t*>(a.mask), static_cast<const bf16*>(a.x), static_cast<bf16*>(a.dx), a.save_mean,
-                            a.save_invstd, a.weight, s.sums, s.sums + a.c, a.norm_fct, (float)(1.0 / a.m), a.m, a.c);
+                            a.save_invstd, a.weight, s.sums, s.sums + a.c, a.norm_fct, (float)(1.0 / a.m), nullptr, nullptr, nullptr,
+                            nullptr, nullptr, nullptr, a.m, a.c);
   return cudaGetLastError();
 }
 
 cudaError_t backward(const BwdArgs& a, cudaStream_t st) {
   const cudaError_t e = launch_bwd_reduce(a, st);
   return e == cudaSuccess ? launch_bwd_elemt(a, st) : e;
+}
+
+// ---- a tail whose identity is a downsample branch's batch norm (two batch norms of one shape) ----
+// The dual scratch is the local one followed by the second statistics plane's staging and the second batch norm's
+// sum of g * (x - mean); the semaphores stay in the fixed region at the start, plane 1's after plane 0's, which is
+// why a dual site takes at most kMaxChannels / 2 channels.
+static size_t dual_extra_offset(int c) { return (scratch_bytes(c) + 15) / 16 * 16; }
+size_t dual_scratch_bytes(int c) { return dual_extra_offset(c) + (size_t)3 * c * kMaxHBlock * 4 + (size_t)c * 4; }
+static float* dual_staging(void* scratch, int c) { return reinterpret_cast<float*>(static_cast<char*>(scratch) + dual_extra_offset(c)); }
+static float* dual_sum_xmu2(void* scratch, int c) { return dual_staging(scratch, c) + (size_t)3 * c * kMaxHBlock; }
+
+// `a` is the tail's batch norm (y, mask), `b` the downsample branch's (its x, weight, bias, statistics); b's y and
+// mask are unused.
+cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const void* xs[2] = {a.x, b.x};
+  const int svec = vec_ok(a.c, xs, 2) ? kStatsVec : 1;
+  block.x /= svec;
+  grid.z = 2;
+  const StatsDualKernel ks = stats_dual_kernel(svec);
+  if (!ks) return kNoKernel;
+  StatsOut oa{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
+              (float)((double)a.m / (double)(a.m - 1)), a.eps};
+  StatsOut ob{b.save_mean, b.save_invstd, b.running_mean, b.running_var, b.num_batches_tracked, b.momentum,
+              (float)((double)b.m / (double)(b.m - 1)), b.eps};
+  ks<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(b.x), oa, ob, s.staging,
+                             dual_staging(a.scratch, a.c), s.semaphores, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const void* ptrs[3] = {a.x, a.y, b.x};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const TransformKernel kt = transform_kernel(vec, kTailBnAddRelu);
+  if (!kt) return kNoKernel;
+  kt<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(b.x), static_cast<bf16*>(a.y),
+                             static_cast<uint8_t*>(a.mask), a.save_mean, a.save_invstd, a.weight, a.bias, b.save_mean, b.save_invstd,
+                             b.weight, b.bias, a.m, a.c);
+  return cudaGetLastError();
+}
+
+// `a` is the tail's batch norm (dy, dy2, y or mask, x, dx), `b` the downsample branch's (x, dx, weight, statistics,
+// grad_weight, grad_bias).  Neither writes g: the elementwise kernel derives it again.
+cudaError_t backward_dual(const BwdArgs& a, const BwdArgs& b, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  float* sum2 = dual_sum_xmu2(a.scratch, a.c);
+  const GradSrc src = a.mask ? kGradBits : kGradY;
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const BwdReduceKernel kr = bwd_reduce_kernel(src, true);
+  if (!kr) return kNoKernel;
+  kr<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
+                             static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(a.mask), nullptr, a.save_mean, a.save_invstd,
+                             s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, pool_dims(0, 0),
+                             static_cast<const bf16*>(b.x), b.save_mean, b.save_invstd, sum2, b.grad_weight, b.grad_bias, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const void* ptrs[7] = {a.x, a.dx, a.dy, a.dy2 ? a.dy2 : a.dy, b.x, b.dx, a.y};
+  const int vec = vec_ok(a.c, ptrs, src == kGradY ? 7 : 6) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const BwdElemtKernel ke = bwd_elemt_kernel(vec, src, false, true);
+  if (!ke) return kNoKernel;
+  ke<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2), static_cast<const bf16*>(a.y),
+                             static_cast<const uint8_t*>(a.mask), static_cast<const bf16*>(a.x), static_cast<bf16*>(a.dx), a.save_mean,
+                             a.save_invstd, a.weight, s.sums, s.sums + a.c, nullptr, (float)(1.0 / a.m), static_cast<const bf16*>(b.x),
+                             static_cast<bf16*>(b.dx), b.save_mean, b.save_invstd, b.weight, sum2, a.m, a.c);
+  return cudaGetLastError();
 }
 
 // ---- sync batch norm ----

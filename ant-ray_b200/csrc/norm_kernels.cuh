@@ -274,6 +274,25 @@ __global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats(const bf16* __restri
                    [&](int c, float mean, float m2n, int count) { finish_stats(o, c, mean, m2n, count); });
 }
 
+// Two batch norms of one shape (a block tail's and its downsample branch's): grid.z = 2, z selecting the input and
+// the outputs.  Each z plane is k_bn_stats over its input with the launch shape torch uses for it, so the bits are
+// those of two k_bn_stats launches; plane 1 stages in its own region and counts on semaphores[gridDim.x + x].
+template <int V>
+__global__ void __launch_bounds__(kMaxBlock / V) k_bn_stats_dual(const bf16* __restrict__ input0, const bf16* __restrict__ input1,
+                                                                 StatsOut o0, StatsOut o1, volatile float* staging0,
+                                                                 volatile float* staging1, int* semaphores, const int reduction_size,
+                                                                 const int stride) {
+  const bool z = blockIdx.z != 0;
+  // field by field: a reference to either parameter would put both on the stack
+  const StatsOut o{z ? o1.save_mean : o0.save_mean, z ? o1.save_invstd : o0.save_invstd, z ? o1.running_mean : o0.running_mean,
+                   z ? o1.running_var : o0.running_var, z ? o1.num_batches_tracked : o0.num_batches_tracked,
+                   z ? o1.momentum : o0.momentum, z ? o1.bessel : o0.bessel, z ? o1.eps : o0.eps};
+  if (o.num_batches_tracked && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0)
+    *o.num_batches_tracked += 1;
+  bn_stats_body<V>(z ? input1 : input0, z ? staging1 : staging0, semaphores + (z ? gridDim.x : 0), reduction_size, stride,
+                   [&](int c, float mean, float m2n, int count) { finish_stats(o, c, mean, m2n, count); });
+}
+
 // ---- sync batch norm (torch.nn.SyncBatchNorm's autograd function) ----
 // A rank's statistics travel as one row [mean (C) | invstd (C) | count] of fp32, as in torch's all_gather.
 
@@ -339,14 +358,17 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_sync_merge(const float* __res
   running_var[i] = __fmaf_rn(unbiased_var, momentum, __fmul_rn(1 - momentum, running_var[i]));
 }
 
-// What is fused after the batch norm: nothing, a ReLU, or `+= identity` and a ReLU (a block's tail).
-enum Tail { kTailNone, kTailRelu, kTailAddRelu };
-constexpr int kTails = 3;
+// What is fused after the batch norm: nothing, a ReLU, `+= identity` and a ReLU (a block's tail), or `+=` a second
+// batch norm's output and a ReLU (a tail whose identity is a downsample branch's batch norm).
+enum Tail { kTailNone, kTailRelu, kTailAddRelu, kTailBnAddRelu };
+constexpr int kTails = 4;
 
 // y = bf16(bn(x)) (kTailNone: torch.batch_norm_elemt), y = relu(bn(x)) (kTailRelu) or y = relu(bf16(bn(x)) +
 // identity) (kTailAddRelu), rounded where eager torch rounds: the batch-norm output to bf16, the bf16 sum of the
 // residual add to bf16.  `t <= 0 ? 0 : bf16(t)` is relu(bf16(t)) because rounding keeps the sign; NaN passes
-// through as in torch's relu.
+// through as in torch's relu.  kTailBnAddRelu reads the downsample branch's input from `identity` and applies its
+// batch norm (mean2 .. shift2) first: y = relu(bf16(bn(x)) + bf16(bn2(identity))), each rounded as eager torch
+// rounds the two batch norms' outputs; that output is never written.
 //
 // With `mask` set (C % 8 == 0) a kernel with a ReLU also writes the ReLU's backward predicate !(y <= 0), computed
 // from the stored bf16 y, as one bit per element: element a = m * C + c is bit a % 8 of byte a / 8.  V = 8 threads
@@ -358,17 +380,26 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
                                                              bf16* __restrict__ out, uint8_t* __restrict__ mask,
                                                              const float* __restrict__ mean, const float* __restrict__ inv_std,
                                                              const float* __restrict__ weight, const float* __restrict__ shift,
+                                                             const float* __restrict__ mean2, const float* __restrict__ inv_std2,
+                                                             const float* __restrict__ weight2, const float* __restrict__ shift2,
                                                              const int reduction_size, const int stride) {
   static_assert(V == 1 || V == 8, "a thread writes a whole mask byte (V = 8) or one bit of a ballot (V = 1)");
+  constexpr bool BN2 = TAIL == kTailBnAddRelu;
   const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   if (c0 >= stride) return;
-  float m_c[V], inv_std_c[V], w_c[V], s_c[V];
+  float m_c[V], inv_std_c[V], w_c[V], s_c[V], m2_c[V], inv_std2_c[V], w2_c[V], s2_c[V];
 #pragma unroll
   for (int j = 0; j < V; j++) {
     m_c[j] = mean[c0 + j];
     inv_std_c[j] = inv_std[c0 + j];
     w_c[j] = weight[c0 + j];
     s_c[j] = shift[c0 + j];
+    if (BN2) {
+      m2_c[j] = mean2[c0 + j];
+      inv_std2_c[j] = inv_std2[c0 + j];
+      w2_c[j] = weight2[c0 + j];
+      s2_c[j] = shift2[c0 + j];
+    }
   }
   const unsigned lane = (threadIdx.x + threadIdx.y * blockDim.x) % 32;
   const unsigned group = 0xffu << (lane & ~7u);
@@ -377,13 +408,14 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
     const int a = m * stride + c0;
     const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
     BVec<V> zv;
-    if (TAIL == kTailAddRelu) zv = *reinterpret_cast<const BVec<V>*>(identity + a);
+    if (TAIL == kTailAddRelu || BN2) zv = *reinterpret_cast<const BVec<V>*>(identity + a);
     BVec<V> yv;
     unsigned bits = 0;
 #pragma unroll
     for (int j = 0; j < V; j++) {
       auto tmp = w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j];
-      if (TAIL == kTailAddRelu) {
+      if (TAIL == kTailAddRelu || BN2) {
+        if (BN2) zv.v[j] = __float2bfloat16(w2_c[j] * (__bfloat162float(zv.v[j]) - m2_c[j]) * inv_std2_c[j] + s2_c[j]);
         const bf16 r = __float2bfloat16(__bfloat162float(__float2bfloat16(tmp)) + __bfloat162float(zv.v[j]));
         yv.v[j] = __bfloat162float(r) <= 0.f ? __float2bfloat16(0.f) : r;
       } else if (TAIL == kTailRelu) {
@@ -401,6 +433,103 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_transform(const bf16* __restr
   }
 }
 
+// ---- the ResNet stem: batch norm -> ReLU -> max_pool2d(kernel 3, stride 2, padding 1) ----
+// Pooled rows are N * OH * OW with OH = (H - 1) / 2 + 1, OW = (W - 1) / 2 + 1.  Window (ph, pw) covers input rows
+// 2 * ph - 1 .. 2 * ph + 1 and columns 2 * pw - 1 .. 2 * pw + 1, clipped to the input; an element's position in it
+// is (ih - 2 * ph + 1) * 3 + (iw - 2 * pw + 1).
+struct PoolDims {
+  int h, w, oh, ow;
+};
+// The argmax byte of a window whose maximum is 0: the ReLU passes no gradient to any of its elements.
+constexpr uint8_t kPoolNoGrad = 0xff;
+
+// pooled = max over the window of y = relu(bf16(bn(x))) (y as k_bn_transform<V, kTailRelu> computes it), selected
+// as torch's channels-last max_pool2d selects it: rows first, then columns, and a y greater than the maximum so far
+// or NaN replaces it, so the first maximum wins a tie and the last NaN wins.  `argmax` receives the winner's
+// position, or kPoolNoGrad where the maximum is 0.  That one byte stands in for the ReLU mask: every element a
+// window selects holds that window's maximum, so the element's ReLU passes its gradient exactly when the maximum
+// is not <= 0.  The 112 x 112 y is never written.
+template <int V>
+__global__ void __launch_bounds__(kEwThreads) k_bn_pool_fwd(const bf16* __restrict__ input, bf16* __restrict__ out,
+                                                            uint8_t* __restrict__ argmax, const float* __restrict__ mean,
+                                                            const float* __restrict__ inv_std, const float* __restrict__ weight,
+                                                            const float* __restrict__ shift, const PoolDims d, const int pooled_rows,
+                                                            const int stride) {
+  const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
+  if (c0 >= stride) return;
+  float m_c[V], inv_std_c[V], w_c[V], s_c[V];
+#pragma unroll
+  for (int j = 0; j < V; j++) {
+    m_c[j] = mean[c0 + j];
+    inv_std_c[j] = inv_std[c0 + j];
+    w_c[j] = weight[c0 + j];
+    s_c[j] = shift[c0 + j];
+  }
+  const int row_step = blockDim.y * gridDim.y;
+  for (int p = blockIdx.y * blockDim.y + threadIdx.y; p < pooled_rows; p += row_step) {
+    const int pw = p % d.ow, ph = (p / d.ow) % d.oh, n = p / (d.ow * d.oh);
+    float best[V];
+    uint8_t pos[V];
+#pragma unroll
+    for (int j = 0; j < V; j++) {
+      best[j] = -INFINITY;
+      pos[j] = 0;
+    }
+    for (int ih = max(2 * ph - 1, 0); ih < min(2 * ph + 2, d.h); ih++) {
+      for (int iw = max(2 * pw - 1, 0); iw < min(2 * pw + 2, d.w); iw++) {
+        const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + ((size_t)(n * d.h + ih) * d.w + iw) * stride + c0);
+        const uint8_t at = (ih - 2 * ph + 1) * 3 + (iw - 2 * pw + 1);
+#pragma unroll
+        for (int j = 0; j < V; j++) {
+          const auto tmp = w_c[j] * (__bfloat162float(xv.v[j]) - m_c[j]) * inv_std_c[j] + s_c[j];
+          const float y = __bfloat162float(tmp <= 0.f ? __float2bfloat16(0.f) : __float2bfloat16(tmp));
+          if (y > best[j] || isnan(y)) {
+            best[j] = y;
+            pos[j] = at;
+          }
+        }
+      }
+    }
+    BVec<V> yv;
+    struct alignas(V) {
+      uint8_t v[V];
+    } av;   // one V-byte store (the launcher picks V = 8 only with argmax on the 16-byte grid and C % 8 == 0)
+#pragma unroll
+    for (int j = 0; j < V; j++) {
+      yv.v[j] = __float2bfloat16(best[j]);
+      av.v[j] = best[j] <= 0.f ? kPoolNoGrad : pos[j];
+    }
+    const size_t a = (size_t)p * stride + c0;
+    *reinterpret_cast<BVec<V>*>(out + a) = yv;
+    *reinterpret_cast<decltype(av)*>(argmax + a) = av;
+  }
+}
+
+// g of input row m, channel c: torch's channels-last max_pool2d backward followed by threshold_backward.  An element
+// inside one window only takes that window's gradient as it is (-0.0 stays -0.0); one inside several sums the
+// gradients of the windows that selected it in fp32 from 0, in (ph, pw) order, and rounds once.  An element no
+// window selected, or whose ReLU stops the gradient (kPoolNoGrad), gets +0.
+__device__ __forceinline__ bf16 pool_grad(const bf16* __restrict__ dpool, const uint8_t* __restrict__ argmax, const PoolDims& d,
+                                          const int m, const int c, const int stride) {
+  const int iw = m % d.w, ih = (m / d.w) % d.h, n = m / (d.w * d.h);
+  const int ph0 = ih >> 1, ph1 = min((ih + 1) >> 1, d.oh - 1);
+  const int pw0 = iw >> 1, pw1 = min((iw + 1) >> 1, d.ow - 1);
+  // the (up to) four windows' bytes and gradients are loaded together, none waiting for another's compare; a
+  // missing second row or column repeats the first, whose slot is then never selected
+  const int o = ((n * d.oh + ph0) * d.ow + pw0) * stride + c;
+  const int dr = (ph1 - ph0) * d.ow * stride, dc = (pw1 - pw0) * stride;
+  const uint8_t a[4] = {argmax[o], argmax[o + dc], argmax[o + dr], argmax[o + dr + dc]};
+  const bf16 v[4] = {dpool[o], dpool[o + dc], dpool[o + dr], dpool[o + dr + dc]};
+  const int at = (ih - 2 * ph0 + 1) * 3 + (iw - 2 * pw0 + 1);   // position in window (ph0, pw0); -2 per later row / column
+  if (ph0 == ph1 && pw0 == pw1) return a[0] == at ? v[0] : __float2bfloat16(0.f);
+  float sum = 0.f;
+  if (a[0] == at) sum += __bfloat162float(v[0]);
+  if (pw1 != pw0 && a[1] == at - 2) sum += __bfloat162float(v[1]);
+  if (ph1 != ph0 && a[2] == at - 6) sum += __bfloat162float(v[2]);
+  if (ph1 != ph0 && pw1 != pw0 && a[3] == at - 8) sum += __bfloat162float(v[3]);
+  return __float2bfloat16(sum);
+}
+
 // The ReLU's backward (threshold_backward: y <= 0 ? 0 : dy), read from dy and the saved output y, or from dy and
 // the predicate !(y <= 0) that k_bn_transform wrote as a bit.
 __device__ __forceinline__ bf16 relu_grad(bf16 dy, bf16 y) { return __bfloat162float(y) <= 0.f ? __float2bfloat16(0.f) : dy; }
@@ -409,33 +538,45 @@ __device__ __forceinline__ bf16 relu_grad_bit(bf16 dy, unsigned bit) { return bi
 __device__ __forceinline__ bf16 add_grads(bf16 a, bf16 b) { return __float2bfloat16(__bfloat162float(a) + __bfloat162float(b)); }
 
 // Where the backward kernels take g, the batch norm's output gradient, from: the tensor the reduce kernel wrote
-// (kGradMasked), relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits), or dy itself, for
-// a batch norm without a ReLU after it (kGradDy).
-enum GradSrc { kGradMasked, kGradY, kGradBits, kGradDy };
-constexpr int kGradSrcs = 4;
+// (kGradMasked), relu_grad of dy and y (kGradY) or of dy and k_bn_transform's bits (kGradBits), dy itself, for
+// a batch norm without a ReLU after it (kGradDy), or pool_grad of the pooled gradient dy and k_bn_pool_fwd's
+// argmax bytes (kGradPool, the stem; the reduce kernel only).
+enum GradSrc { kGradMasked, kGradY, kGradBits, kGradDy, kGradPool };
+constexpr int kGradSrcs = 5;
 
 // Per-channel sums of g and g * (x - mean) with g from G (torch: batch_norm_backward_reduce_channels_last_kernel<4>),
 // and dweight / dbias.  kGradBits reads the ReLU's predicate from `mask` (k_bn_transform's bits) instead of y from
 // `output`.  With `grad_output2` set, dy is the bf16 sum of the two gradients, as autograd rounds it when a tensor
 // has two consumers; without it dy is taken as it is, so a -0.0 gradient stays -0.0.  With `masked` set (the block
-// tail, where g is also the identity branch's gradient) g is written there as well.  As in k_bn_stats, all rows of
-// an iteration are loaded before the first sum uses one.
-template <GradSrc G>
+// tail, where g is also the identity branch's gradient, and the stem) g is written there as well.  kGradPool reads
+// the pooled gradient from `grad_output` and the argmax bytes from `mask`, over the input geometry `pool`.  As in
+// k_bn_stats, all rows of an iteration are loaded before the first sum uses one.
+//
+// DUAL (a tail whose identity is a downsample branch's batch norm, fed the same g): `input2` is that batch norm's
+// input, and the same walk also sums g * (x2 - mean2).  Each of the three sums is accumulated, merged over the block
+// and over the grid exactly as a k_bn_bwd_reduce launch for its own batch norm would, so Σg is both dbias values.
+template <GradSrc G, bool DUAL>
 __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
                                 const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
                                 const uint8_t* __restrict__ mask, bf16* __restrict__ masked, const float* __restrict__ mean,
                                 const float* __restrict__ inv_std, float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
                                 float* __restrict__ grad_weight, float* __restrict__ grad_bias, volatile float* staging_data,
-                                int* semaphores, const int reduction_size, const int stride) {
+                                int* semaphores, const PoolDims pool, const bf16* __restrict__ input2,
+                                const float* __restrict__ mean2, const float* __restrict__ inv_std2, float* __restrict__ sum_dy_xmu2_o,
+                                float* __restrict__ grad_weight2, float* __restrict__ grad_bias2, const int reduction_size,
+                                const int stride) {
   static_assert(G != kGradMasked, "the reduce kernel computes g");
   constexpr bool BITS = G == kGradBits;
+  constexpr bool POOL = G == kGradPool;
   constexpr int PARALLEL_LOADS = kParallelLoads;
   float sum_dy[PARALLEL_LOADS];
   float sum_dy_xmu[PARALLEL_LOADS];
+  float sum_dy_xmu2[PARALLEL_LOADS];
 #pragma unroll
   for (int i = 0; i < PARALLEL_LOADS; i++) {
     sum_dy[i] = float(0);
     sum_dy_xmu[i] = float(0);
+    sum_dy_xmu2[i] = float(0);
   }
   int inner_loop_stride = blockDim.y * gridDim.y;
   int m_offset = blockIdx.y * blockDim.y + threadIdx.y;
@@ -447,33 +588,39 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
   int address_increment = inner_loop_stride * stride;
   auto r_mean = mean[c_offset];
   auto factor = inv_std[c_offset];
+  const float r_mean2 = DUAL ? mean2[c_offset] : 0.f;
 
   for (int i = 0; i < loop_count; i++) {
-    bf16 dy_v[PARALLEL_LOADS], dy2_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS];
+    bf16 dy_v[PARALLEL_LOADS], dy2_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS], x2_v[PARALLEL_LOADS];
     uint8_t mask_v[PARALLEL_LOADS];
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (m_offset + j * inner_loop_stride < reduction_size) {
         const int a = address_base + j * address_increment;
-        dy_v[j] = grad_output[a];
+        if (POOL) dy_v[j] = pool_grad(grad_output, mask, pool, m_offset + j * inner_loop_stride, c_offset, stride);
+        else dy_v[j] = grad_output[a];
         if (grad_output2) dy2_v[j] = grad_output2[a];
         if (BITS) mask_v[j] = mask[a >> 3];
         else if (G == kGradY) y_v[j] = output[a];
         x_v[j] = input[a];
+        if (DUAL) x2_v[j] = input2[a];
       }
     }
     float x_input[PARALLEL_LOADS];
+    float x_input2[PARALLEL_LOADS];
     float x_grad_output[PARALLEL_LOADS];
 #pragma unroll
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       if (c_offset < stride && m_offset < reduction_size) {
-        const bf16 dy = grad_output2 ? add_grads(dy_v[j], dy2_v[j]) : dy_v[j];
+        const bf16 dy = !POOL && grad_output2 ? add_grads(dy_v[j], dy2_v[j]) : dy_v[j];
         const bf16 g = BITS ? relu_grad_bit(dy, (mask_v[j] >> (address_base & 7)) & 1u) : G == kGradY ? relu_grad(dy, y_v[j]) : dy;
         if (masked) masked[address_base] = g;
         x_input[j] = __bfloat162float(x_v[j]);
+        x_input2[j] = DUAL ? __bfloat162float(x2_v[j]) : 0.f;
         x_grad_output[j] = __bfloat162float(g);
       } else {
         x_input[j] = float(0);
+        x_input2[j] = float(0);
         x_grad_output[j] = float(0);
       }
       m_offset += inner_loop_stride;
@@ -483,27 +630,52 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
     for (int j = 0; j < PARALLEL_LOADS; j++) {
       sum_dy[j] += x_grad_output[j];
       sum_dy_xmu[j] = __fmaf_rn(x_grad_output[j], x_input[j] - r_mean, sum_dy_xmu[j]);   // += g * (x - mean)
+      if (DUAL) sum_dy_xmu2[j] = __fmaf_rn(x_grad_output[j], x_input2[j] - r_mean2, sum_dy_xmu2[j]);
     }
   }
 #pragma unroll
   for (int j = 1; j < PARALLEL_LOADS; j++) {
     sum_dy[0] += sum_dy[j];
     sum_dy_xmu[0] += sum_dy_xmu[j];
+    if (DUAL) sum_dy_xmu2[0] += sum_dy_xmu2[j];
   }
   auto sum_dy_th = sum_dy[0];
   auto sum_dy_xmu_th = sum_dy_xmu[0];
+  float sum_dy_xmu2_th = sum_dy_xmu2[0];
 
   __shared__ float shmem_sum_dy[kMaxBlock];
   __shared__ float shmem_sum_dy_xmu[kMaxBlock];
-  merge_block_vertical_backward(sum_dy_th, sum_dy_xmu_th, shmem_sum_dy, shmem_sum_dy_xmu);
+  // the third sum takes the same tree after the first two (each value's tree is independent of the others)
+  auto merge = [&]() {
+    merge_block_vertical_backward(sum_dy_th, sum_dy_xmu_th, shmem_sum_dy, shmem_sum_dy_xmu);
+    if (DUAL) {
+      __syncthreads();
+      float unused = 0.f;
+      merge_block_vertical_backward(sum_dy_xmu2_th, unused, shmem_sum_dy, shmem_sum_dy_xmu);
+    }
+  };
+  merge();
 
+  auto write_sums = [&]() {
+    grad_bias[c_offset] = sum_dy_th;
+    grad_weight[c_offset] = sum_dy_xmu_th * factor;
+    sum_dy_o[c_offset] = sum_dy_th;
+    sum_dy_xmu_o[c_offset] = sum_dy_xmu_th;
+    if (DUAL) {
+      grad_bias2[c_offset] = sum_dy_th;
+      grad_weight2[c_offset] = sum_dy_xmu2_th * inv_std2[c_offset];
+      sum_dy_xmu2_o[c_offset] = sum_dy_xmu2_th;
+    }
+  };
   if (gridDim.y > 1) {
     volatile float* staging_sum_dy = staging_data;
     volatile float* staging_sum_dy_xmu = &staging_data[stride * gridDim.y];
+    volatile float* staging_sum_dy_xmu2 = &staging_data[2 * stride * gridDim.y];
     address_base = c_offset + blockIdx.y * stride;
     if (threadIdx.y == 0 && c_offset < stride) {
       staging_sum_dy[address_base] = sum_dy_th;
       staging_sum_dy_xmu[address_base] = sum_dy_xmu_th;
+      if (DUAL) staging_sum_dy_xmu2[address_base] = sum_dy_xmu2_th;
     }
     __threadfence();
     __syncthreads();
@@ -517,26 +689,18 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
     if (is_last_block_done) {
       sum_dy_th = float(0.0);
       sum_dy_xmu_th = float(0.0);
+      sum_dy_xmu2_th = float(0.0);
       for (int y = threadIdx.y; y < gridDim.y; y += blockDim.y) {
         address_base = c_offset + y * stride;
         sum_dy_th += (c_offset < stride ? staging_sum_dy[address_base] : float(0.0));
         sum_dy_xmu_th += (c_offset < stride ? staging_sum_dy_xmu[address_base] : float(0.0));
+        if (DUAL) sum_dy_xmu2_th += (c_offset < stride ? staging_sum_dy_xmu2[address_base] : float(0.0));
       }
-      merge_block_vertical_backward(sum_dy_th, sum_dy_xmu_th, shmem_sum_dy, shmem_sum_dy_xmu);
-      if (threadIdx.y == 0 && c_offset < stride) {
-        grad_bias[c_offset] = sum_dy_th;
-        grad_weight[c_offset] = sum_dy_xmu_th * factor;
-        sum_dy_o[c_offset] = sum_dy_th;
-        sum_dy_xmu_o[c_offset] = sum_dy_xmu_th;
-      }
+      merge();
+      if (threadIdx.y == 0 && c_offset < stride) write_sums();
     }
   } else {
-    if (blockIdx.y == 0 && threadIdx.y == 0 && c_offset < stride) {
-      grad_bias[c_offset] = sum_dy_th;
-      grad_weight[c_offset] = sum_dy_xmu_th * factor;
-      sum_dy_o[c_offset] = sum_dy_th;
-      sum_dy_xmu_o[c_offset] = sum_dy_xmu_th;
-    }
+    if (blockIdx.y == 0 && threadIdx.y == 0 && c_offset < stride) write_sums();
   }
 }
 
@@ -549,7 +713,10 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
 // kernels do: with norm_fct a kernel parameter nvcc contracts `g - sum_dy * norm_fct` into one FMA per element,
 // with norm_fct loaded from memory it multiplies once per channel and subtracts.  One kernel that selects between
 // value and pointer at run time rounds a local site's dx like a sync site's, which is not eager torch's.
-template <int V, GradSrc G, bool FCT_PTR>
+//
+// DUAL: also dx2 of the downsample branch's batch norm (input2, mean2 .. sum_dy_xmu2), fed the same g, which the
+// kernel derives from dy (and dy2) and the mask or y; Σg is the same for both.
+template <int V, GradSrc G, bool FCT_PTR, bool DUAL>
 __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restrict__ grad_output, const bf16* __restrict__ grad_output2,
                                                              const bf16* __restrict__ output, const uint8_t* __restrict__ mask,
                                                              const bf16* __restrict__ input, bf16* __restrict__ grad_input,
@@ -557,11 +724,16 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restr
                                                              const float* __restrict__ weight, const float* __restrict__ sum_dy,
                                                              const float* __restrict__ sum_dy_xmu,
                                                              const float* __restrict__ norm_fct_ptr, const float norm_fct_value,
+                                                             const bf16* __restrict__ input2, bf16* __restrict__ grad_input2,
+                                                             const float* __restrict__ mean2, const float* __restrict__ inv_std2,
+                                                             const float* __restrict__ weight2, const float* __restrict__ sum_dy_xmu2,
                                                              const int reduction_size, const int stride) {
+  static_assert(!DUAL || (G == kGradY || G == kGradBits), "a dual tail derives g from dy and the ReLU");
   const float norm_fct = FCT_PTR ? *norm_fct_ptr : norm_fct_value;
   const int c0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   if (c0 >= stride) return;
   float m_c[V], m_dy_c[V], factor_1_c[V], factor_2_c[V];
+  float m2_c[V], factor2_1_c[V], factor2_2_c[V];
 #pragma unroll
   for (int j = 0; j < V; j++) {
     m_c[j] = mean[c0 + j];
@@ -569,6 +741,12 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restr
     factor_1_c[j] = inv_std[c0 + j];
     factor_2_c[j] = weight[c0 + j] * factor_1_c[j];
     factor_1_c[j] = factor_1_c[j] * factor_1_c[j] * sum_dy_xmu[c0 + j] * norm_fct;
+    if (DUAL) {
+      m2_c[j] = mean2[c0 + j];
+      factor2_1_c[j] = inv_std2[c0 + j];
+      factor2_2_c[j] = weight2[c0 + j] * factor2_1_c[j];
+      factor2_1_c[j] = factor2_1_c[j] * factor2_1_c[j] * sum_dy_xmu2[c0 + j] * norm_fct;
+    }
   }
   const int row_step = blockDim.y * gridDim.y;
   for (int m = blockIdx.y * blockDim.y + threadIdx.y; m < reduction_size; m += row_step) {
@@ -580,15 +758,19 @@ __global__ void __launch_bounds__(kEwThreads) k_bn_bwd_elemt(const bf16* __restr
     if (G == kGradY) yv = *reinterpret_cast<const BVec<V>*>(output + a);
     if (G == kGradBits) bits = mask[a >> 3] >> (a & 7);
     const BVec<V> xv = *reinterpret_cast<const BVec<V>*>(input + a);
-    BVec<V> dxv;
+    BVec<V> x2v, dxv, dx2v;
+    if (DUAL) x2v = *reinterpret_cast<const BVec<V>*>(input2 + a);
 #pragma unroll
     for (int j = 0; j < V; j++) {
       const bf16 dy = G != kGradMasked && grad_output2 ? add_grads(gv.v[j], gv2.v[j]) : gv.v[j];
       const float g = __bfloat162float(G == kGradMasked || G == kGradDy ? dy
                                        : G == kGradY ? relu_grad(dy, yv.v[j]) : relu_grad_bit(dy, (bits >> j) & 1u));
       dxv.v[j] = __float2bfloat16((g - m_dy_c[j] - (__bfloat162float(xv.v[j]) - m_c[j]) * factor_1_c[j]) * factor_2_c[j]);
+      if (DUAL)
+        dx2v.v[j] = __float2bfloat16((g - m_dy_c[j] - (__bfloat162float(x2v.v[j]) - m2_c[j]) * factor2_1_c[j]) * factor2_2_c[j]);
     }
     *reinterpret_cast<BVec<V>*>(grad_input + a) = dxv;
+    if (DUAL) *reinterpret_cast<BVec<V>*>(grad_input2 + a) = dx2v;
   }
 }
 

@@ -22,6 +22,10 @@ struct FwdArgs {
   int m, c;
   float momentum, eps;
   void* scratch;
+  // The stem (pool_h > 0): y is relu(bn(x)) max-pooled 3x3 / stride 2 / padding 1 over m / (pool_h * pool_w)
+  // images of pool_h x pool_w rows, and argmax receives one byte per pooled element; identity and mask are null.
+  void* argmax;
+  int pool_h, pool_w;
 };
 
 struct BwdArgs {
@@ -41,14 +45,24 @@ struct BwdArgs {
   float* grad_bias;
   int m, c;
   void* scratch;
+  // The stem (pool_h > 0): dy is the pooled output's gradient, argmax the forward's, and dy_masked receives g;
+  // y, mask and dy2 are null.
+  const void* argmax;
+  int pool_h, pool_w;
 };
 
 // Largest channel count the kernels take: it bounds the semaphore region at the start of every scratch buffer.
 constexpr int kMaxChannels = 1 << 17;
 
 size_t scratch_bytes(int c);
-cudaError_t forward(const FwdArgs& a, cudaStream_t s);   // 2 kernels
-cudaError_t backward(const BwdArgs& a, cudaStream_t s);  // 2 kernels
+cudaError_t forward(const FwdArgs& a, cudaStream_t s);   // 2 kernels, the stem's included
+cudaError_t backward(const BwdArgs& a, cudaStream_t s);  // 2 kernels, the stem's included
+
+// A tail whose identity is a downsample branch's batch norm: `a` the tail's batch norm, `b` the branch's, of the
+// same m and c (c <= kMaxChannels / 2).  2 kernels per direction; scratch of dual_scratch_bytes(c).
+size_t dual_scratch_bytes(int c);
+cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t s);
+cudaError_t backward_dual(const BwdArgs& a, const BwdArgs& b, cudaStream_t s);
 
 // Sync batch norm: the local phases around the two collectives, which b200coll.cu runs between them.
 //   forward:  sync_stats -> allgather of `local` (2c + 1 floats) into the W `gathered` rows -> sync_apply

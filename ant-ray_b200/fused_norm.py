@@ -5,7 +5,8 @@ by nothing (a downsample branch).  In bf16 training torch runs the first two kin
 passes: batch norm, ReLU and the residual add forward; threshold_backward and batch norm backward.
 `fuse_resnet` swaps a model's torchvision `ResNet`, `Bottleneck` and `BasicBlock` classes for subclasses whose
 forward runs each such site as one native call per direction, which writes its output once and folds the ReLU
-mask into the backward.  The kernels reproduce torch's own channels-last kernels, reduction order included, so
+mask into the backward.  A downsample branch's batch norm runs inside its block tail's call (`bn_add_relu_downsample`),
+and the stem's batch norm, ReLU and max-pool are one call (`bn_relu_maxpool`).  The kernels reproduce torch's own channels-last kernels, reduction order included, so
 outputs, gradients and running statistics are bit-identical to eager torch.
 
 A site runs fused when it is in training mode, its input is a bf16 channels-last CUDA tensor with more than one
@@ -52,12 +53,16 @@ def _native_lib():
 
 
 def _scratch_bytes(channels, world=None):
-    """The scratch a site of `channels` needs: a local site's, or with `world` a sync site's over that many ranks."""
+    """The scratch a site of `channels` needs: a local site's, with `world` a sync site's over that many ranks, or with
+    world "dual" a dual tail's (a tail and its downsample branch's batch norm)."""
     key = (channels, world)
     need = _scratch_need.get(key)
     if need is None:
         lib = _native_lib()
-        need = lib.b200c_bn_scratch_bytes(channels) if world is None else lib.b200c_bn_sync_scratch_bytes(channels, world)
+        if world == "dual":
+            need = lib.b200c_bn_dual_scratch_bytes(channels)
+        else:
+            need = lib.b200c_bn_scratch_bytes(channels) if world is None else lib.b200c_bn_sync_scratch_bytes(channels, world)
         need = _scratch_need[key] = int(need)
     return need
 
@@ -164,6 +169,103 @@ class _FusedBatchNorm(torch.autograd.Function):
         return dx, d_identity, grad_weight, grad_bias, None, None, None, None
 
 
+class _FusedBatchNormDual(torch.autograd.Function):
+    """relu(bn(x) + bn_ds(x_ds)) in training mode: a block tail whose identity is its downsample branch's batch norm.
+    bn_ds(x_ds) is never written, and the backward writes dx and dx_ds from one walk over g.  `pair` as in
+    _FusedBatchNorm."""
+
+    @staticmethod
+    def forward(ctx, x, x_ds, weight, bias, weight_ds, bias_ds, bn, bn_ds, pair):
+        lib = _native_lib()
+        c = x.shape[1]
+        m = x.numel() // c
+        y = torch.empty_like(x)
+        ctx.set_materialize_grads(False)
+        masked = c % 8 == 0
+        relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if masked else y
+        # [save_mean | save_invstd] of bn, then of bn_ds
+        stats = torch.empty(4 * c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        nbt, nbt_ds = bn.num_batches_tracked, bn_ds.num_batches_tracked
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_forward_dual(
+            x.data_ptr(), x_ds.data_ptr(), y.data_ptr(), relu_src.data_ptr() if masked else None,
+            weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+            nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, bn.momentum, bn.eps,
+            weight_ds.data_ptr(), bias_ds.data_ptr(), bn_ds.running_mean.data_ptr(), bn_ds.running_var.data_ptr(),
+            nbt_ds.data_ptr() if nbt_ds is not None else None, mean + 8 * c, mean + 12 * c, bn_ds.momentum, bn_ds.eps,
+            m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c, "dual")), stream))
+        ctx.save_for_backward(x, x_ds, relu_src, weight, weight_ds, stats)
+        return (y, y.view_as(y)) if pair else y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        grads = [g.contiguous(memory_format=torch.channels_last) for g in grads if g is not None]
+        if not grads:
+            return (None,) * 9
+        x, x_ds, relu_src, weight, weight_ds, stats = ctx.saved_tensors
+        lib = _native_lib()
+        c = x.shape[1]
+        m = x.numel() // c
+        dx, dx_ds = torch.empty_like(x), torch.empty_like(x_ds)
+        dw, db, dw_ds, db_ds = (torch.empty(c, dtype=torch.float32, device=x.device) for _ in range(4))
+        mean = stats.data_ptr()
+        masked = relu_src.dtype == torch.uint8
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_backward_dual(
+            grads[0].data_ptr(), grads[1].data_ptr() if len(grads) == 2 else None, None if masked else relu_src.data_ptr(),
+            relu_src.data_ptr() if masked else None, x.data_ptr(), x_ds.data_ptr(), dx.data_ptr(), dx_ds.data_ptr(),
+            weight.data_ptr(), mean, mean + 4 * c, dw.data_ptr(), db.data_ptr(), weight_ds.data_ptr(), mean + 8 * c,
+            mean + 12 * c, dw_ds.data_ptr(), db_ds.data_ptr(), m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c, "dual")),
+            stream))
+        return dx, dx_ds, dw, db, dw_ds, db_ds, None, None, None
+
+
+class _FusedBatchNormPool(torch.autograd.Function):
+    """maxpool(relu(bn(x))) in training mode, maxpool being nn.MaxPool2d(3, 2, 1): the ResNet stem.  The forward writes
+    the pooled output and one argmax byte per pooled element, never relu(bn(x)) itself; the backward takes the pooled
+    output's gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, bn):
+        lib = _native_lib()
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device,
+                        memory_format=torch.channels_last)
+        argmax = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)
+        nbt = bn.num_batches_tracked
+        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_forward_pool(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), weight.data_ptr(), bias.data_ptr(),
+                                          bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                          nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, n, h, w, c,
+                                          bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        ctx.save_for_backward(x, argmax, weight, stats)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None, None
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        x, argmax, weight, stats = ctx.saved_tensors
+        lib = _native_lib()
+        n, c, h, w = x.shape
+        g = torch.empty_like(x)
+        dx = torch.empty_like(x)
+        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
+        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_backward_pool(dy.data_ptr(), argmax.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(),
+                                           weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(),
+                                           n, h, w, c, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        return dx, grad_weight, grad_bias, None
+
+
 def _activation(t):
     # With one channel, NCHW strides also pass the channels-last check, but torch runs its NCHW statistics kernel
     # unless stride(1) == 1 (batch_norm_choose_impl), so the channel stride must be 1 as well.
@@ -235,6 +337,23 @@ def bn_relu(bn, relu, x):
     return relu(bn(x))
 
 
+def _pool_fusable(pool):
+    """Whether `pool` is exactly nn.MaxPool2d(3, 2, 1) (dilation 1, floor mode, no indices) and calling the kernel
+    instead of the module skips no hook."""
+    two = lambda v, k: v in (k, (k, k))  # noqa: E731
+    return (type(pool) is nn.MaxPool2d and two(pool.kernel_size, 3) and two(pool.stride, 2) and two(pool.padding, 1)
+            and two(pool.dilation, 1) and not pool.ceil_mode and not pool.return_indices and not _hooked(pool)
+            and not _global_hooks())
+
+
+def bn_relu_maxpool(bn, relu, pool, x):
+    """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) and the batch norm can run as a local
+    fused site; otherwise bn_relu and the module call."""
+    if _pool_fusable(pool) and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
+        return _FusedBatchNormPool.apply(x, bn.weight, bn.bias, bn)
+    return pool(bn_relu(bn, relu, x))
+
+
 def bn_add_relu(bn, relu, x, identity, pair=False):
     """`out = bn(x); out += identity; relu(out)`, fused when the site allows it.  With `pair`, returns `(out,
     out_id)`: the same values, whose gradients a fused site receives apart and sums in its backward kernel."""
@@ -248,6 +367,30 @@ def bn_add_relu(bn, relu, x, identity, pair=False):
     out += identity
     out = relu(out)
     return (out, out) if pair else out
+
+
+def _downsample_bn(ds):
+    """The batch norm of a downsample branch that a dual tail can run: `ds` exactly nn.Sequential(nn.Conv2d, batch
+    norm), where calling the convolution and the kernel instead of the two modules skips no hook; else None."""
+    if type(ds) is not nn.Sequential or len(ds) != 2 or type(ds[0]) is not nn.Conv2d or _global_hooks():
+        return None
+    if _hooked(ds) or _hooked(ds[1]):
+        return None
+    return ds[1]
+
+
+def bn_add_relu_downsample(bn, relu, x, downsample, x_id, pair=False):
+    """`out = bn(x); out += downsample(x_id); relu(out)`, with `pair` as in bn_add_relu.  Where the downsample branch is
+    a convolution and a batch norm that can run as a local fused site alongside this one, both batch norms run in
+    one native call per direction and the branch's output is never written; otherwise bn_add_relu."""
+    bn_ds = _downsample_bn(downsample)
+    if bn_ds is not None and bn_ds is not bn and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
+        x_ds = downsample[0](x_id)
+        if (x_ds.shape == x.shape and _sync_comm(bn_ds, x_ds) is None and _fusable(bn_ds, relu, x_ds)
+                and _scratch_bytes(x.shape[1], "dual")):
+            return _FusedBatchNormDual.apply(x, x_ds, bn.weight, bn.bias, bn_ds.weight, bn_ds.bias, bn, bn_ds, pair)
+        return bn_add_relu(bn, relu, x, bn_ds(x_ds), pair)
+    return bn_add_relu(bn, relu, x, downsample(x_id), pair)
 
 
 def _hooked(mod):
@@ -280,8 +423,9 @@ else:
         def forward_pair(self, x, x_id):
             out = bn_relu(self.bn1, self.relu, self.conv1(x))
             out = self.conv2(out)
-            identity = self.downsample(x_id) if self.downsample is not None else x_id
-            return bn_add_relu(self.bn2, self.relu, out, identity, pair=True)
+            if self.downsample is not None:
+                return bn_add_relu_downsample(self.bn2, self.relu, out, self.downsample, x_id, pair=True)
+            return bn_add_relu(self.bn2, self.relu, out, x_id, pair=True)
 
     class FusedBottleneck(Bottleneck):
         def forward(self, x):
@@ -293,8 +437,9 @@ else:
             out = bn_relu(self.bn1, self.relu, self.conv1(x))
             out = bn_relu(self.bn2, self.relu, self.conv2(out))
             out = self.conv3(out)
-            identity = self.downsample(x_id) if self.downsample is not None else x_id
-            return bn_add_relu(self.bn3, self.relu, out, identity, pair=True)
+            if self.downsample is not None:
+                return bn_add_relu_downsample(self.bn3, self.relu, out, self.downsample, x_id, pair=True)
+            return bn_add_relu(self.bn3, self.relu, out, x_id, pair=True)
 
     def _pairwise(layer):
         """Whether `layer`'s blocks can be chained through forward_pair: a plain Sequential of fused blocks, where
@@ -306,8 +451,7 @@ else:
         def forward(self, x):
             if not self.training:
                 return super().forward(x)
-            x = bn_relu(self.bn1, self.relu, self.conv1(x))
-            x = x_id = self.maxpool(x)   # the maxpool output's two gradients are summed by autograd
+            x = x_id = bn_relu_maxpool(self.bn1, self.relu, self.maxpool, self.conv1(x))   # two gradients, summed by autograd
             hooks = _global_hooks()
             for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
                 if not hooks and _pairwise(layer):

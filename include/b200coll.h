@@ -321,6 +321,46 @@ int b200c_bn_backward_mask(const void* dy, const void* dy2, const uint8_t* mask,
                            const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
                            float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream);
 
+/* A block tail whose identity is a downsample branch's batch norm: y = relu(bn(x) + bn_ds(x_ds)), the two batch
+ * norms' outputs each rounded to bf16 before the bf16 add, as eager torch computes
+ * `out = bn3(conv3); out += downsample(x); relu(out)`.  x and x_ds have the same m rows of `channels`; each batch
+ * norm has its own weight, bias, statistics, momentum and eps, with the results of b200c_bn_forward for each.
+ * bn_ds(x_ds) is never written.  `mask` (may be NULL; channels % 8 == 0) as in b200c_bn_forward_mask.
+ * Backward: both batch norms take g, the ReLU's gradient of dy (or of bf16(dy + dy2) with `dy2` set); writes dx,
+ * dx_ds and both dweight / dbias, reading the mask, or y where mask is NULL.  g is not written.
+ * `scratch` holds at least b200c_bn_dual_scratch_bytes(channels) bytes, with the contract of b200c_bn_scratch_bytes;
+ * channels <= 65536 (0 outside 1..65536).  2 kernels per direction; every argument is checked before the first
+ * launch. */
+size_t b200c_bn_dual_scratch_bytes(int channels);
+int b200c_bn_forward_dual(const void* x, const void* x_ds, void* y, uint8_t* mask, const float* weight, const float* bias,
+                          float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                          float* save_invstd, float momentum, float eps, const float* weight_ds, const float* bias_ds,
+                          float* running_mean_ds, float* running_var_ds, int64_t* num_batches_tracked_ds,
+                          float* save_mean_ds, float* save_invstd_ds, float momentum_ds, float eps_ds, int m, int channels,
+                          void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_dual(const void* dy, const void* dy2, const void* y, const uint8_t* mask, const void* x,
+                           const void* x_ds, void* dx, void* dx_ds, const float* weight, const float* save_mean,
+                           const float* save_invstd, float* grad_weight, float* grad_bias, const float* weight_ds,
+                           const float* save_mean_ds, const float* save_invstd_ds, float* grad_weight_ds,
+                           float* grad_bias_ds, int m, int channels, void* scratch, b200c_stream_t stream);
+
+/* The ResNet stem, maxpool(relu(bn(x))) with torch's nn.MaxPool2d(3, stride=2, padding=1), over n images of h x w
+ * rows (m = n * h * w), bit-identical to eager torch's batch norm, ReLU and channels-last max_pool2d.  Scratch,
+ * statistics and their contract are those of b200c_bn_forward; any channel count.
+ * Forward: y receives the pooled output, n * oh * ow rows with oh = (h - 1) / 2 + 1, ow = (w - 1) / 2 + 1, and
+ * `argmax` one byte per pooled element: the position (row * 3 + column) in its window of the element it selected
+ * (rows first, the first maximum and the last NaN win), or 255 where the maximum is 0 and the ReLU passes no
+ * gradient.  relu(bn(x)) itself is not written.  2 kernels.
+ * Backward: from dy (the gradient of y), argmax and x writes dx, grad_weight and grad_bias; `g` (m rows, required)
+ * receives the batch norm's output gradient, torch's max_pool2d backward followed by the ReLU's.  2 kernels. */
+int b200c_bn_forward_pool(const void* x, void* y, uint8_t* argmax, const float* weight, const float* bias,
+                          float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                          float* save_invstd, int n, int h, int w, int channels, float momentum, float eps, void* scratch,
+                          b200c_stream_t stream);
+int b200c_bn_backward_pool(const void* dy, const uint8_t* argmax, const void* x, void* g, void* dx, const float* weight,
+                           const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
+                           int h, int w, int channels, void* scratch, b200c_stream_t stream);
+
 /* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
  * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
  * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)

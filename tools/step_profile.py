@@ -33,6 +33,8 @@ FAMILIES = [
     ("bn_stats_torch", r"batch_norm_collect_statistics"),
     ("bn_update_invert", r"batch_norm_update_stats"),
     ("bn_transform", r"batch_norm_transform_input|k_bn_transform"),
+    ("bn_pool", r"k_bn_pool_fwd"),                        # ours: the stem's transform, ReLU and max-pool forward
+    ("max_pool", r"max_pool"),                            # torch's (before conv: its kernels' names say nhwc)
     ("bn_bwd_reduce", r"k_bn_bwd_reduce"),
     ("bn_bwd_reduce_torch", r"batch_norm_backward_reduce"),
     ("bn_bwd_elemt", r"batch_norm_backward_elemt|k_bn_bwd_elemt"),
@@ -43,26 +45,33 @@ FAMILIES = [
     ("optimizer", r"multi_tensor|sgd|SGD|foreach"),
 ]
 
-# bytes each family's kernels move per element of a batch-norm site, by site kind (relu: BN -> ReLU; tail:
-# BN -> += identity -> ReLU whose output feeds another block; last_tail: the tail that feeds the pooling; plain:
-# downsample BN, always torch's kernels)
+# bytes each family's kernels move per element of a batch-norm site, by site kind (stem: BN -> ReLU -> 3x3 / 2
+# max-pool, a quarter as many pooled elements; relu: BN -> ReLU; tail: BN -> += identity -> ReLU whose output feeds
+# another block; ds_tail: such a tail whose identity is a downsample branch; last_tail: the tail that feeds the
+# pooling; plain: the downsample branch's BN, which the fused build runs inside the ds_tail's kernels)
 TORCH_BYTES = {  # family -> {kind: bytes per element}
-    "bn_stats_torch": {"relu": 2, "tail": 2, "last_tail": 2, "plain": 2},
-    "bn_transform": {"relu": 4, "tail": 4, "last_tail": 4, "plain": 4},
-    "relu": {"relu": 4, "tail": 4, "last_tail": 4},
-    "add": {"tail": 6, "last_tail": 6},
-    "threshold_backward": {"relu": 6, "tail": 6, "last_tail": 6},
-    "bn_bwd_reduce_torch": {"relu": 4, "tail": 4, "last_tail": 4, "plain": 4},
-    "bn_bwd_elemt": {"relu": 6, "tail": 6, "last_tail": 6, "plain": 6},
+    "bn_stats_torch": {"stem": 2, "relu": 2, "tail": 2, "last_tail": 2, "plain": 2},
+    "bn_transform": {"stem": 4, "relu": 4, "tail": 4, "last_tail": 4, "plain": 4},
+    "relu": {"stem": 4, "relu": 4, "tail": 4, "last_tail": 4},
+    "max_pool": {"stem": 9},   # y -> pooled, int64 indices; indices, dpool -> dy
+    "add": {"tail": 6, "ds_tail": 6, "last_tail": 6},
+    "threshold_backward": {"stem": 6, "relu": 6, "tail": 6, "ds_tail": 6, "last_tail": 6},
+    "bn_bwd_reduce_torch": {"stem": 4, "relu": 4, "tail": 4, "ds_tail": 4, "last_tail": 4, "plain": 4},
+    "bn_bwd_elemt": {"stem": 6, "relu": 6, "tail": 6, "ds_tail": 6, "last_tail": 6, "plain": 6},
 }
-# the fused sites' ReLU mask is 1 bit (1/8 byte) per element
+for _fam in ("bn_stats_torch", "bn_transform", "relu"):
+    TORCH_BYTES[_fam]["ds_tail"] = TORCH_BYTES[_fam]["tail"]
+# the fused sites' ReLU mask is 1 bit (1/8 byte) per element; the stem's argmax is 1 byte per pooled element
+# (ds_tail: the identity read is the branch's input, and the backward writes no g: the elementwise kernel reads dy,
+# dy2 and the mask again; plain: the branch's input read by each kernel, its dx written)
 FUSED_BYTES = {
-    "bn_stats": {"relu": 2, "tail": 2, "last_tail": 2},
-    "bn_stats_torch": {"plain": 2},
-    "bn_transform": {"relu": 4.125, "tail": 6.125, "last_tail": 6.125, "plain": 4},   # x (, identity) -> y, mask
-    "bn_bwd_reduce": {"relu": 4.125, "tail": 8.125, "last_tail": 6.125},            # dy (, dy2), mask, x (tail: -> dy')
-    "bn_bwd_reduce_torch": {"plain": 4},
-    "bn_bwd_elemt": {"relu": 6.125, "tail": 6, "last_tail": 6, "plain": 6},         # dy, mask, x -> dx (tail: dy', x -> dx)
+    "bn_stats": {"stem": 2, "relu": 2, "tail": 2, "ds_tail": 2, "last_tail": 2, "plain": 2},
+    "bn_transform": {"relu": 4.125, "tail": 6.125, "ds_tail": 6.125, "last_tail": 6.125},   # x (, identity) -> y, mask
+    "bn_pool": {"stem": 2.75},                                                              # x -> pooled, argmax
+    # stem: dpool, argmax, x -> g; others: dy (, dy2), mask, x (tail: -> dy')
+    "bn_bwd_reduce": {"stem": 4.75, "relu": 4.125, "tail": 8.125, "ds_tail": 6.125, "last_tail": 6.125, "plain": 2},
+    # dy, mask, x -> dx (tail, stem: g, x -> dx; ds_tail: dy, dy2, mask, x -> dx)
+    "bn_bwd_elemt": {"stem": 6, "relu": 6.125, "tail": 6, "ds_tail": 8.125, "last_tail": 6, "plain": 4},
 }
 
 
@@ -72,12 +81,12 @@ def bn_sites(batch):
     import torchvision
 
     model = torchvision.models.resnet50(weights=None).eval()
-    kinds = {id(model.bn1): "relu"}
+    kinds = {id(model.bn1): "stem"}
     for mod in model.modules():
         if isinstance(mod, torchvision.models.resnet.Bottleneck):
             kinds.update({id(mod.bn1): "relu", id(mod.bn2): "relu", id(mod.bn3): "tail"})
             if mod.downsample is not None:
-                kinds[id(mod.downsample[1])] = "plain"
+                kinds.update({id(mod.bn3): "ds_tail", id(mod.downsample[1]): "plain"})
     kinds[id(model.layer4[-1].bn3)] = "last_tail"
     sites = []
     hooks = [m.register_forward_pre_hook(lambda m, a: sites.append((kinds[id(m)], a[0].numel() * batch)))
@@ -184,7 +193,7 @@ def main():
     out = {"mode": "unfused" if args.unfused else "fused", "batch": args.batch, "steps": args.steps,
            "ms_per_step": round(ms / args.steps, 3), "kernel_ms_per_step": round(total, 3),
            "images_per_sec": round(args.batch * args.steps / (ms / 1e3), 1), **gpu_identity(), "families": fams,
-           "bn_site_elements": {k: sum(e for kind, e in sites if kind == k) for k in ("relu", "tail", "last_tail", "plain")}}
+           "bn_site_elements": {k: sum(e for kind, e in sites if kind == k) for k in ("stem", "relu", "tail", "ds_tail", "last_tail", "plain")}}
     os.makedirs(args.out, exist_ok=True)
     path = os.path.join(args.out, f"step_profile_{out['mode']}.json")
     with open(path, "w") as f:

@@ -138,9 +138,12 @@ static BwdElemtKernel bwd_elemt_kernel(int vec, int src, bool fct_ptr, bool dual
         return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, false, true>;
       });
     return with_const<kGradMasked, kGradY, kGradBits, kGradDy>(src, [&](auto g) {
-      return with_const<false, true>(fct_ptr, [](auto p) -> BwdElemtKernel {
+      auto kernel = [](auto p) -> BwdElemtKernel {
         return k_bn_bwd_elemt<decltype(v)::value, (GradSrc) decltype(g)::value, decltype(p)::value != 0, false>;
-      });
+      };
+      // a batch norm without a ReLU after it runs only as a sync site, which brings its norm_fct pointer
+      if constexpr (decltype(g)::value == kGradDy) return with_const<true>(fct_ptr, kernel);
+      else return with_const<false, true>(fct_ptr, kernel);
     });
   });
 }

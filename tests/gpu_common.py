@@ -221,3 +221,8 @@ BN_REGIME_SHAPES = {
     (8, 4104, 8, 8): BnLaunch(32, 16, 129, 1),         # one column past a power of two
     (2, 131072, 32, 32): BnLaunch(32, 16, 4096, 8),    # the most channels, merged: the last semaphore (512 MiB per tensor)
 }
+# The same regimes for a dual tail (two batch norms of one shape in one grid.z = 2 launch), whose plane 1 counts on the
+# semaphores after plane 0's: at most half the channels.  The last entry is that limit on a merged grid, where plane 1
+# uses semaphores 2048 .. 4095.
+BN_DUAL_REGIME_SHAPES = {s: cfg for s, cfg in BN_REGIME_SHAPES.items() if s[1] != BN_MAX_CHANNELS}
+BN_DUAL_REGIME_SHAPES[(2, BN_MAX_CHANNELS // 2, 32, 32)] = BnLaunch(32, 16, 2048, 8)

@@ -69,6 +69,22 @@ def test_named_shapes_reach_their_launch_regimes():
     assert any(s[1] % 8 for s in BN_REGIME_SHAPES) and any(s[1] % 8 == 0 for s in BN_REGIME_SHAPES)
 
 
+def test_dual_shapes_reach_their_launch_regimes_within_half_the_semaphores():
+    # A dual tail's plane 1 counts on semaphores[grid_x + x], so both planes' columns must fit the region; the limit
+    # shape's plane 1 reaches its last semaphore.
+    from gpu_common import BN_DUAL_REGIME_SHAPES, BN_MAX_CHANNELS, BN_REGIME_SHAPES, BN_SEMAPHORES, BnLaunch, bn_launch_config
+
+    assert len(BN_DUAL_REGIME_SHAPES) == len(BN_REGIME_SHAPES)
+    assert {s: cfg for s, cfg in BN_DUAL_REGIME_SHAPES.items() if s[1] != BN_MAX_CHANNELS // 2} == \
+        {s: cfg for s, cfg in BN_REGIME_SHAPES.items() if s[1] != BN_MAX_CHANNELS}
+    assert BN_DUAL_REGIME_SHAPES[(2, 65536, 32, 32)] == BnLaunch(32, 16, 2048, 8)
+    for (n, c, h, w), want in BN_DUAL_REGIME_SHAPES.items():
+        assert bn_launch_config(n * h * w, c) == want, (n, c, h, w)
+        assert 2 * want.grid_x <= BN_SEMAPHORES, (n, c, h, w)
+    last = max(cfg.grid_x + cfg.grid_x - 1 for cfg in BN_DUAL_REGIME_SHAPES.values() if cfg.grid_y > 1)
+    assert last == BN_SEMAPHORES - 1 == 4095
+
+
 def test_merged_grids_fit_the_semaphore_region():
     # Each column of a merged grid owns one semaphore of the fixed region at the start of the scratch buffer, so no
     # shape the kernels take may merge over more columns than the region holds.  The largest channel count uses

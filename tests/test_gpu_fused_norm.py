@@ -79,12 +79,30 @@ def test_fused_site_is_bit_identical_to_eager_torch(n, c, h, w, residual):
 
 def test_one_scratch_serves_every_channel_count():
     # A narrow site whose grid merge spans many rows stages its partial sums in the scratch buffer that the
-    # semaphores of a later wide site share (one buffer per stream); every site must still merge correctly.
+    # semaphores of a later wide site share (one buffer per stream); every site must still merge correctly.  Local,
+    # dual and stem sites interleave on the stream: the buffer grows at the first dual site, which needs more than
+    # the sites before it; a wide dual site (plane 1 on semaphores 512 .. 1023) is followed by narrow local sites,
+    # and a dual site's plane 1 counts on semaphores a wider local site used before it.
+    from test_gpu_fused_dual import check_dual, inputs as dual_inputs
+    from test_gpu_fused_stem import check_stem, gauss_inputs
+
     fused_norm._scratch.clear()
-    for n, c, h, w in [(256, 16, 56, 56), (256, 2048, 7, 7), (256, 32, 56, 56), (256, 2048, 7, 7), (3, 100, 9, 9)]:
-        for residual in (False, True):
-            check_site(n, c, h, w, residual)
-    assert len(fused_norm._scratch) == 1
+    sites = [("local", (256, 16, 56, 56)), ("stem", (8, 16, 56, 56)), ("dual", (32, 512, 28, 28)), ("local", (256, 2048, 7, 7)),
+             ("local", (256, 32, 56, 56)), ("dual", (2, 16384, 32, 32)), ("local", (256, 16, 56, 56)), ("local", (3, 100, 9, 9)),
+             ("local", (256, 2048, 7, 7)), ("dual", (32, 1024, 14, 14)), ("stem", (3, 100, 9, 9)), ("local", (256, 32, 56, 56))]
+    sizes = []
+    for kind, (n, c, h, w) in sites:
+        if kind == "local":
+            for residual in (False, True):
+                check_site(n, c, h, w, residual)
+        elif kind == "dual":
+            x3, x_ds, dy1, dy2 = dual_inputs(n, c, h, w, c + n)
+            check_dual(x3, x_ds, dy1, dy2, "pair", make_bn(c, 1), make_bn(c, 2))
+        else:
+            check_stem(*gauss_inputs(n, c, h, w, c + n), make_bn(c, 3))
+        assert len(fused_norm._scratch) == 1
+        sizes.append(next(iter(fused_norm._scratch.values()))[0])
+    assert sizes[2] > sizes[1] == sizes[0], sizes
 
 
 def test_one_value_per_channel_raises_as_torch_does():
@@ -339,10 +357,10 @@ def check_stats_against_float64(x, got):
         assert ((var_got - var64).abs() <= 8 * k * u * (x64 ** 2).mean(0)).all()
 
 
-@pytest.mark.parametrize("m,c", [(65536, 16), (32768, 100), (32768, 2048), (2048, 131072)])
-def test_scratch_stays_in_bounds_and_semaphores_return_to_zero(m, c):
-    assert bn_launch_config(m, c).grid_y == (8 if c == 131072 else 128)
-    x, dy, w, b, rm, rv = site_inputs(m, c, c)
+def check_native_site(m, c, seed):
+    """One ReLU site through b200c_bn_forward / b200c_bn_backward (y read, no mask) on a scratch with guard bytes,
+    against torch bit for bit.  Returns (x, native results)."""
+    x, dy, w, b, rm, rv = site_inputs(m, c, seed)
     want = torch_site(x, dy, w, b, rm, rv)
     buf, need = scratch_with_guard(c)
     launch, got = native_site(x, dy, w, b, rm, rv, buf, torch.cuda.current_stream())
@@ -351,7 +369,13 @@ def test_scratch_stays_in_bounds_and_semaphores_return_to_zero(m, c):
     check_scratch(buf, need)
     for k in want:
         assert same_bits(got[k], want[k]), k
-    check_stats_against_float64(x, got)
+    return x, got
+
+
+@pytest.mark.parametrize("m,c", [(65536, 16), (32768, 100), (32768, 2048), (2048, 131072)])
+def test_scratch_stays_in_bounds_and_semaphores_return_to_zero(m, c):
+    assert bn_launch_config(m, c).grid_y == (8 if c == 131072 else 128)
+    check_stats_against_float64(*check_native_site(m, c, c))
 
 
 def test_two_streams_with_their_own_scratch():

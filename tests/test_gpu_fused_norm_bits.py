@@ -2,7 +2,7 @@
 
 A tail called with `pair=True` returns its output twice; autograd hands the backward each consumer's gradient
 apart and the kernel sums them as autograd's bf16 accumulation does.  Checked for every tail shape of ResNet-50 at
-batch 256, with only one of the two outputs used, with a channel count that has no mask (C % 8 != 0), and at
+batch 256 and one shape per launch regime of the reducing kernels (gpu_common.BN_REGIME_SHAPES), with only one of the two outputs used, with a channel count that has no mask (C % 8 != 0), and at
 value edges of the two gradients.  Through the C-ABI: the mask's bits and layout for the vector and the scalar
 transform (a guard past the mask stays untouched), and the mask backward against the backward that reads y.  In a
 fused resnet50 training step, the blocks chained in pairs leave one elementwise add in the backward, the maxpool
@@ -20,7 +20,7 @@ import torch.nn.functional as F
 
 from ant_ray_b200 import _native as N
 from ant_ray_b200 import fused_norm
-from gpu_common import assert_same_values
+from gpu_common import BN_REGIME_SHAPES, assert_same_values
 from test_gpu_fused_norm import make_bn, misaligned
 
 pytestmark = pytest.mark.gpu
@@ -82,7 +82,7 @@ def check_two_gradients(n, c, h, w, used, edges=False):
         assert_same_values(got[k], want[k], k)
 
 
-@pytest.mark.parametrize("n,c,h,w", TAIL_SHAPES + [(3, 100, 9, 9)])
+@pytest.mark.parametrize("n,c,h,w", TAIL_SHAPES + [(3, 100, 9, 9)] + list(BN_REGIME_SHAPES))
 def test_two_gradients_match_eager_accumulation(n, c, h, w):
     check_two_gradients(n, c, h, w, "both")
 

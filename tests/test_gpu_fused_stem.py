@@ -4,7 +4,9 @@ autograd, bit for bit: the pooled output, dx, dweight, dbias, the running statis
 Eager torch runs the batch norm on its native channels-last kernels, the ReLU in place and max_pool2d on its
 channels-last kernels (argmax rows first, the first maximum and the last NaN win; the backward sums each input's
 gradient over the windows that selected it in fp32, in (ph, pw) order).  The fused site never writes relu(bn(x));
-it makes 4 native launches, as every other fused site."""
+it makes 4 native launches, as every other fused site.  Shapes: the ResNet stem's and odd ones, one shape per launch
+regime of the reducing kernels (gpu_common.BN_REGIME_SHAPES), inputs off the 16-byte grid; through the C-ABI, the
+argmax bytes against eager torch's indices, with every operand on and off the grid."""
 import copy
 import json
 import os
@@ -18,9 +20,9 @@ import torch.nn as nn
 
 from ant_ray_b200 import _native as N
 from ant_ray_b200 import fused_norm
-from gpu_common import same_bits
-from test_gpu_fused_norm import (CONST, ONE_NAN, ZERO, check_scratch, edge_bn_setup, edge_site_inputs, make_bn, misaligned,
-                                 scratch_with_guard)
+from gpu_common import BN_REGIME_SHAPES, same_bits
+from test_gpu_fused_norm import (CONST, ONE_NAN, ZERO, check_scratch, check_stats_against_float64, edge_bn_setup, edge_site_inputs,
+                                 make_bn, misaligned, scratch_with_guard)
 
 pytestmark = pytest.mark.gpu
 CL = torch.channels_last
@@ -38,6 +40,7 @@ def run(bn, x, dpool, fused, pool=None):
     if fused:
         before = N.launch_count()
         y = fused_norm.bn_relu_maxpool(bn, relu, pool, x)
+        assert type(y.grad_fn).__name__ == "_FusedBatchNormPoolBackward" or not fused_norm._pool_fusable(pool)
         y.backward(dpool)
         torch.cuda.synchronize()
         launches = N.launch_count() - before
@@ -74,6 +77,16 @@ STEM_SHAPES = [(256, 64, 112, 112), (32, 64, 112, 112), (4, 64, 113, 113), (2, 6
 def test_stem_is_bit_identical_to_eager_torch(n, c, h, w):
     x, dpool = gauss_inputs(n, c, h, w, n + c + h)
     check_stem(x, dpool, make_bn(c, 3))
+
+
+@pytest.mark.parametrize("n,c,h,w", list(BN_REGIME_SHAPES))
+def test_every_launch_regime_matches_eager_torch(n, c, h, w):
+    # the statistics kernel and the pooled-gradient reduce (kGradPool) at every launch regime; where C % 8 == 0 the
+    # misaligned copy takes the scalar statistics, pooling and elementwise kernels at the same launch shape
+    x, dpool = gauss_inputs(n, c, h, w, n + c + h)
+    check_stem(x, dpool, make_bn(c, 3))
+    if c % 8 == 0:
+        check_stem(misaligned(x), dpool, make_bn(c, 3))
 
 
 def test_misaligned_input_takes_the_scalar_kernels():
@@ -137,36 +150,77 @@ def test_four_window_gradients_sum_in_torch_order():
     assert (relu_out[:, :, 1, 1] > 0).all()
 
 
+def off_grid(numel, dtype):
+    """A flat buffer of `numel` elements whose data pointer is one element past a 16-byte boundary."""
+    return torch.empty(numel + 1, dtype=dtype, device="cuda")[1:]
+
+
+def expected_argmax(x, bn):
+    """Eager torch's window position of each pooled element's maximum, (ih - 2 ph + 1) * 3 + (iw - 2 pw + 1), or
+    255 where the maximum is 0: one byte per pooled element in NHWC order."""
+    n, c, h, w = x.shape
+    with torch.no_grad():
+        pooled, idx = nn.functional.max_pool2d(torch.relu(bn(x)), 3, 2, 1, return_indices=True)
+    _, _, oh, ow = pooled.shape
+    ph = torch.arange(oh, device="cuda").view(1, 1, oh, 1)
+    pw = torch.arange(ow, device="cuda").view(1, 1, 1, ow)
+    pos = (idx // w - 2 * ph + 1) * 3 + (idx % w - 2 * pw + 1)
+    pos = torch.where(pooled == 0, 255, pos)
+    assert ((pos >= 0) & (pos <= 8) | (pos == 255)).all()
+    return pooled, pos.to(torch.uint8).permute(0, 2, 3, 1).flatten()
+
+
 def test_through_the_c_abi_scratch_stays_in_bounds_and_semaphores_return_to_zero():
-    lib = N.load()
     for n, c, h, w in [(32, 64, 112, 112), (3, 100, 9, 9)]:
-        x, dpool = gauss_inputs(n, c, h, w, 14)
-        bn = make_bn(c, 15)
-        buf, need = scratch_with_guard(c)
-        _, _, oh, ow = pooled_shape(n, c, h, w)
-        y = torch.empty(n, c, oh, ow, dtype=torch.bfloat16, device="cuda", memory_format=CL)
-        argmax = torch.empty(y.numel(), dtype=torch.uint8, device="cuda")
-        g, dx = torch.empty_like(x), torch.empty_like(x)
-        mean, invstd, dw, db = (torch.empty(c, dtype=torch.float32, device="cuda") for _ in range(4))
-        s = torch.cuda.current_stream().cuda_stream
-        N.check(lib.b200c_bn_forward_pool(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), bn.weight.data_ptr(), bn.bias.data_ptr(),
-                                          bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.num_batches_tracked.data_ptr(),
-                                          mean.data_ptr(), invstd.data_ptr(), n, h, w, c, 0.1, 1e-5, buf.data_ptr(), s))
-        torch.cuda.synchronize()
-        check_scratch(buf, need)
-        assert ((argmax <= 8) | (argmax == 255)).all()
-        N.check(lib.b200c_bn_backward_pool(dpool.contiguous(memory_format=CL).data_ptr(), argmax.data_ptr(), x.data_ptr(),
-                                           g.data_ptr(), dx.data_ptr(), bn.weight.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
-                                           dw.data_ptr(), db.data_ptr(), n, h, w, c, buf.data_ptr(), s))
-        torch.cuda.synchronize()
-        check_scratch(buf, need)
-        # g is the batch norm's output gradient: what eager torch's max_pool2d and threshold backward give
-        xr = x.detach().clone().requires_grad_()
-        ref_bn = make_bn(c, 15)
-        t = ref_bn(xr)
-        t.retain_grad()
-        nn.MaxPool2d(3, 2, 1)(torch.relu(t)).backward(dpool)
-        assert same_bits(g, t.grad)
+        check_stem_through_the_c_abi(n, c, h, w, aligned=True)
+
+
+@pytest.mark.parametrize("aligned", [True, False], ids=["vector", "scalar"])
+@pytest.mark.parametrize("n,c,h,w", [(32, 64, 112, 112), (3, 100, 9, 9)] + [s for s in BN_REGIME_SHAPES if s[1] <= 2048])
+def test_through_the_c_abi_at_every_launch_regime_on_and_off_the_grid(n, c, h, w, aligned):
+    # Off the grid, x, y and argmax each sit one element past a 16-byte boundary (the fused module cannot misalign y
+    # and argmax): k_bn_pool_fwd<1> and the scalar kernels at C % 8 == 0 too.
+    check_stem_through_the_c_abi(n, c, h, w, aligned)
+
+
+def check_stem_through_the_c_abi(n, c, h, w, aligned):
+    """b200c_bn_forward_pool / b200c_bn_backward_pool on a scratch with guard bytes: the scratch stays in bounds and
+    its semaphores return to zero, the statistics are within rounding of float64, the pooled output and the argmax
+    bytes are eager torch's, and g is eager torch's max_pool2d and threshold backward."""
+    lib = N.load()
+    x, dpool = gauss_inputs(n, c, h, w, 14)
+    if not aligned:
+        x = misaligned(x)
+    bn = make_bn(c, 15)
+    buf, need = scratch_with_guard(c)
+    _, _, oh, ow = pooled_shape(n, c, h, w)
+    numel = n * oh * ow * c
+    y = torch.empty(numel, dtype=torch.bfloat16, device="cuda") if aligned else off_grid(numel, torch.bfloat16)
+    argmax = torch.empty(numel, dtype=torch.uint8, device="cuda") if aligned else off_grid(numel, torch.uint8)
+    g, dx = torch.empty_like(x), torch.empty_like(x)
+    mean, invstd, dw, db = (torch.empty(c, dtype=torch.float32, device="cuda") for _ in range(4))
+    s = torch.cuda.current_stream().cuda_stream
+    N.check(lib.b200c_bn_forward_pool(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), bn.weight.data_ptr(), bn.bias.data_ptr(),
+                                      bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.num_batches_tracked.data_ptr(),
+                                      mean.data_ptr(), invstd.data_ptr(), n, h, w, c, 0.1, 1e-5, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    check_stats_against_float64(x.permute(0, 2, 3, 1).reshape(n * h * w, c), {"mean": mean, "invstd": invstd})
+    pooled, want_argmax = expected_argmax(x, make_bn(c, 15))
+    assert same_bits(y.view(n, oh, ow, c), pooled.permute(0, 2, 3, 1)), "pooled output"
+    assert torch.equal(argmax, want_argmax), f"{int((argmax != want_argmax).sum())}/{numel} argmax bytes differ"
+    N.check(lib.b200c_bn_backward_pool(dpool.contiguous(memory_format=CL).data_ptr(), argmax.data_ptr(), x.data_ptr(),
+                                       g.data_ptr(), dx.data_ptr(), bn.weight.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
+                                       dw.data_ptr(), db.data_ptr(), n, h, w, c, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    # g is the batch norm's output gradient: what eager torch's max_pool2d and threshold backward give
+    xr = x.detach().clone().requires_grad_()
+    ref_bn = make_bn(c, 15)
+    t = ref_bn(xr)
+    t.retain_grad()
+    nn.MaxPool2d(3, 2, 1)(torch.relu(t)).backward(dpool)
+    assert same_bits(g, t.grad)
 
 
 def stem_trace_kernels():

@@ -9,8 +9,10 @@ statistics and num_batches_tracked must have the reference's bits.
 
 Sites: ReLU (stem / conv1 / conv2 positions), tails with one and with two output gradients, and plain sites (the
 module's own forward, e.g. a downsample branch).  Shapes: every batch-norm shape of ResNet-50 with a global batch
-split unevenly over the ranks, including an empty and a single-row rank; C = 100 (scalar kernels, no mask); an
-operand off the 16-byte grid; the value edges of test_gpu_fused_norm; and the sync scratch's guard bytes."""
+split unevenly over the ranks, including an empty and a single-row rank; one shape per launch regime of the reducing
+kernels on rank 0 with one image on every other rank (gpu_common.BN_REGIME_SHAPES); C = 100 (scalar kernels, no
+mask); an operand off the 16-byte grid; the value edges of test_gpu_fused_norm; through the C-ABI, a ReLU site that
+reads y instead of a mask at C % 8 == 0, and the sync scratch's guard bytes."""
 import copy
 
 import pytest
@@ -19,7 +21,7 @@ import torch.nn as nn
 
 from ant_ray_b200 import _native as N
 from ant_ray_b200 import fused_norm
-from gpu_common import assert_same_values
+from gpu_common import BN_MAX_CHANNELS, BN_REGIME_SHAPES, assert_same_values
 from test_gpu_fused_norm import RESNET50_BN_SHAPES, edge_bn_setup, edge_site_inputs, misaligned
 
 pytestmark = pytest.mark.gpu
@@ -186,7 +188,27 @@ def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=()):
     return got, launched
 
 
-def check_sites(world, n, c, h, w, kind, seed, inputs=None, bn_setup=None, misalign=(), sizes=None, **bn_args):
+def collective_launches(world, c):
+    """The launches of one sync site's two collectives over all ranks: the allgather of 2C + 1 statistics floats and
+    the all-reduce of 2C sums, each in as many pieces as the world's staging takes."""
+    W = world.world_size
+    rows = [torch.zeros(2 * c + 1, device="cuda") for _ in range(W)]
+    gathered = [[torch.empty(2 * c + 1, device="cuda") for _ in range(W)] for _ in range(W)]
+    sums = [torch.zeros(2 * c, device="cuda") for _ in range(W)]
+    before = N.launch_count()
+
+    def step(r, comm):
+        comm.allgather(rows[r].data_ptr(), [t.data_ptr() for t in gathered[r]], 2 * c + 1, N.FLOAT32)
+        comm.allreduce(sums[r].data_ptr(), sums[r].data_ptr(), 2 * c, N.FLOAT32, N.SUM)
+
+    world.run(step)
+    torch.cuda.synchronize()
+    world.check()
+    return N.launch_count() - before
+
+
+def check_sites(world, n, c, h, w, kind, seed, inputs=None, bn_setup=None, misalign=(), sizes=None, collectives=None,
+                **bn_args):
     W = world.world_size
     sizes = sizes or split_rows(n, W, seed)
     assert sum(sizes) == n
@@ -208,8 +230,10 @@ def check_sites(world, n, c, h, w, kind, seed, inputs=None, bn_setup=None, misal
     want = reference(bn, xs, ids, dys, dy2s, kind)
     got, launched = run_native(world, bn, xs, ids, dys, dy2s, kind, misalign)
     compare(got, want, sizes)
-    # per rank: 2 collectives (one launch each at these sizes), the merge, and 4 local kernels when it has rows
-    assert launched == sum(3 + (4 if s else 0) for s in sizes), launched
+    # per rank: 2 collectives (one launch each, unless `collectives` counts their pieces), the merge, and 4 local
+    # kernels when it has rows
+    collectives = 2 * W if collectives is None else collectives
+    assert launched == collectives + sum(1 + (4 if s else 0) for s in sizes), launched
 
 
 def compare(got, want, sizes):
@@ -232,6 +256,22 @@ def compare(got, want, sizes):
 def test_resnet50_sites_match_torch_sync_batch_norm(world, c, h, w, kind):
     n = 2 * world.world_size + 3
     check_sites(world, n, c, h, w, kind, seed=c * 7 + h + world.world_size)
+
+
+@pytest.mark.parametrize("kind", ["relu", "tail2", "plain"])
+@pytest.mark.parametrize("n,c,h,w", list(BN_REGIME_SHAPES))
+def test_every_launch_regime_matches_torch_sync_batch_norm(world, n, c, h, w, kind):
+    # rank 0 runs the regime's launch shape; every other rank holds one image, so the ranks' launch shapes differ
+    W = world.world_size
+    if W > 3:
+        pytest.skip("the regime sweep runs at W = 2 and W = 3")
+    sizes = [n] + [1] * (W - 1)
+    collectives = None
+    if c == BN_MAX_CHANNELS:
+        # 2C + 1 floats are more than the world's 1 MiB staging takes in one piece
+        collectives = collective_launches(world, c)
+        assert collectives > 2 * W, collectives
+    check_sites(world, sum(sizes), c, h, w, kind, seed=n + c + h + W, sizes=sizes, collectives=collectives)
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -341,3 +381,44 @@ def test_sync_scratch_guard_and_semaphores(world):
     # every rank holds the same global statistics
     for s in st[1:]:
         assert_same_values(s["stats"], st[0]["stats"], "global statistics")
+
+
+@pytest.mark.parametrize("c", [64, 2048])
+def test_relu_site_reading_y_through_the_c_abi(world, c):
+    check_relu_site_reading_y(world, c)
+
+
+def check_relu_site_reading_y(world, c):
+    """b200c_bn_sync_forward with relu = 1 and no mask, then b200c_bn_sync_backward from y: the vector elementwise
+    backward that reads y and the device's 1 / rows of all ranks (the fused module passes a mask at C % 8 == 0).  The
+    ranks hold different batch sizes, so a rank's own 1 / rows would differ from the global one."""
+    W, h, w = world.world_size, 5, 5
+    sizes = [2 + r for r in range(W)]
+    lib = N.load()
+    g = torch.Generator(device="cuda").manual_seed(c + W)
+    xs = [cl((torch.randn(m, c, h, w, device="cuda", generator=g) * 2 + 0.5).to(torch.bfloat16)) for m in sizes]
+    dys = [cl(torch.randn(m, c, h, w, device="cuda", generator=g).to(torch.bfloat16)) for m in sizes]
+    bn = make_sync_bn(c, c + W)
+    want = reference(bn, xs, [None] * W, dys, [None] * W, "relu")
+    need = int(lib.b200c_bn_sync_scratch_bytes(c, W))
+    w_, b_ = bn.weight.detach(), bn.bias.detach()
+    st = [dict(rm=bn.running_mean.clone(), rv=bn.running_var.clone(), nbt=bn.num_batches_tracked.clone(), y=torch.empty_like(x),
+               dx=torch.empty_like(x), stats=torch.empty(2 * c + 1, device="cuda"), dw=torch.empty(c, device="cuda"),
+               db=torch.empty(c, device="cuda"), scratch=torch.zeros(need, dtype=torch.uint8, device="cuda")) for x in xs]
+
+    def step(r, comm):
+        s, m, p = st[r], sizes[r] * h * w, st[r]["stats"].data_ptr()
+        stream = torch.cuda.current_stream().cuda_stream
+        N.check(lib.b200c_bn_sync_forward(comm._h(), xs[r].data_ptr(), None, s["y"].data_ptr(), None, 1, w_.data_ptr(),
+                                          b_.data_ptr(), s["rm"].data_ptr(), s["rv"].data_ptr(), s["nbt"].data_ptr(), p, p + 4 * c,
+                                          p + 8 * c, m, c, 0.1, 1e-5, s["scratch"].data_ptr(), stream))
+        N.check(lib.b200c_bn_sync_backward(comm._h(), dys[r].data_ptr(), None, s["y"].data_ptr(), None, 1, xs[r].data_ptr(), None,
+                                           s["dx"].data_ptr(), w_.data_ptr(), p, p + 4 * c, p + 8 * c, s["dw"].data_ptr(),
+                                           s["db"].data_ptr(), m, c, s["scratch"].data_ptr(), stream))
+
+    world.run(step)
+    torch.cuda.synchronize()
+    world.check()
+    got = [{"y": s["y"], "dx": s["dx"], "dweight": s["dw"], "dbias": s["db"], "running_mean": s["rm"], "running_var": s["rv"],
+            "num_batches_tracked": s["nbt"]} for s in st]
+    compare(got, want, sizes)

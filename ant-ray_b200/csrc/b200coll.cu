@@ -1595,6 +1595,54 @@ extern "C" int b200c_bn_backward_pool(const void* dy, const uint8_t* argmax, con
   return B200C_OK;
 }
 
+// Eval mode (norm_infer.cuh): one kernel per site.  An eval batch norm takes one value per channel (m >= 1).
+static int check_infer(const char* site, int param_bf16, int m, int c) {
+  if (m < 1 || c < 1 || (int64_t)m * c > INT32_MAX) return fail(B200C_EINVAL, "%s: bad shape m=%d c=%d", site, m, c);
+  if (param_bf16 != 0 && param_bf16 != 1) return fail(B200C_EINVAL, "%s: param_bf16=%d is neither 0 nor 1", site, param_bf16);
+  return B200C_OK;
+}
+
+static int run_infer(const bn::InferArgs& a, b200c_stream_t stream) {
+  RT(bn::infer(a, (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer(const void* x, const void* identity, void* y, const void* weight, const void* bias,
+                              const void* running_mean, const void* running_var, int param_bf16, float eps, int m, int channels,
+                              b200c_stream_t stream) {
+  int rc = check_infer("batch norm infer", param_bf16, m, channels);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer: null buffer");
+  return run_infer({x, identity, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0},
+                   stream);
+}
+
+extern "C" int b200c_bn_infer_dual(const void* x, const void* x_ds, void* y, const void* weight, const void* bias,
+                                   const void* running_mean, const void* running_var, float eps, const void* weight_ds,
+                                   const void* bias_ds, const void* running_mean_ds, const void* running_var_ds, float eps_ds,
+                                   int param_bf16, int m, int channels, b200c_stream_t stream) {
+  int rc = check_infer("batch norm infer dual", param_bf16, m, channels);
+  if (rc) return rc;
+  if (!x || !x_ds || !y || !weight || !bias || !running_mean || !running_var || !weight_ds || !bias_ds || !running_mean_ds ||
+      !running_var_ds)
+    return fail(B200C_EINVAL, "batch norm infer dual: null buffer");
+  return run_infer({x, x_ds, y, {weight, bias, running_mean, running_var, eps}, {weight_ds, bias_ds, running_mean_ds, running_var_ds, eps_ds},
+                    true, param_bf16 != 0, m, channels, 0, 0},
+                   stream);
+}
+
+extern "C" int b200c_bn_infer_pool(const void* x, void* y, const void* weight, const void* bias, const void* running_mean,
+                                   const void* running_var, int param_bf16, float eps, int n, int h, int w, int channels,
+                                   b200c_stream_t stream) {
+  int m = 0;
+  int rc = check_pool("infer", n, h, w, channels, &m);
+  if (!rc) rc = check_infer("batch norm infer pool", param_bf16, m, channels);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer pool: null buffer");
+  return run_infer({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, h, w}, stream);
+}
+
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {
   int rc = check_ready(c);
   if (rc) return rc;

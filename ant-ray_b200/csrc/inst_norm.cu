@@ -3,6 +3,7 @@
 #include <initializer_list>
 #include <type_traits>
 
+#include "norm_infer.cuh"
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
 
@@ -148,6 +149,26 @@ static BwdElemtKernel bwd_elemt_kernel(int vec, int src, bool fct_ptr, bool dual
   });
 }
 
+// the eval-mode kernels, one pointer type per parameter type P (float or bf16)
+template <typename P>
+using InferTransformKernel = void (*)(const bf16*, const bf16*, bf16*, const P*, const P*, const P*, const P*, float, const P*, const P*,
+                                      const P*, const P*, float, int, int);
+template <typename P>
+using InferPoolKernel = void (*)(const bf16*, bf16*, const P*, const P*, const P*, const P*, float, PoolDims, int, int);
+
+template <typename P>
+static InferTransformKernel<P> infer_transform_kernel(int vec, int tail) {
+  return with_const<1, kEwVec>(vec, [&](auto v) {
+    return with_const<kTailRelu, kTailAddRelu, kTailBnAddRelu>(tail, [](auto t) -> InferTransformKernel<P> {
+      return bn_infer::k_infer_transform<decltype(v)::value, (Tail) decltype(t)::value, P>;
+    });
+  });
+}
+template <typename P>
+static InferPoolKernel<P> infer_pool_kernel(int vec) {
+  return with_const<1, kEwVec>(vec, [](auto v) -> InferPoolKernel<P> { return bn_infer::k_infer_pool<decltype(v)::value, P>; });
+}
+
 // Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
 // load a kernel lazily while a peer's collective waits): every key value goes through the functions above.
 cudaError_t load_kernels() {
@@ -168,6 +189,12 @@ cudaError_t load_kernels() {
     for (int src = 0; src < kGradSrcs; src++)
       for (bool fct_ptr : {false, true})
         for (bool dual : {false, true}) load(bwd_elemt_kernel(vec, src, fct_ptr, dual));
+    load(infer_pool_kernel<float>(vec));
+    load(infer_pool_kernel<bf16>(vec));
+    for (int tail = 0; tail < kTails; tail++) {
+      load(infer_transform_kernel<float>(vec, tail));
+      load(infer_transform_kernel<bf16>(vec, tail));
+    }
   }
   return e;
 }
@@ -349,6 +376,38 @@ cudaError_t backward_dual(const BwdArgs& a, const BwdArgs& b, cudaStream_t st) {
                              static_cast<bf16*>(b.dx), b.save_mean, b.save_invstd, b.weight, sum2, a.m, a.c);
   return cudaGetLastError();
 }
+
+// ---- eval mode: one kernel per site, launched as the training transform / pool kernels are ----
+template <typename P>
+static cudaError_t launch_infer(const InferArgs& a, cudaStream_t st) {
+  auto p = [](const void* q) { return static_cast<const P*>(q); };
+  const bf16* x = static_cast<const bf16*>(a.x);
+  bf16* y = static_cast<bf16*>(a.y);
+  const InferParams& b = a.bn;
+  dim3 block, grid;
+  if (a.pool_h) {
+    const PoolDims d = pool_dims(a.pool_h, a.pool_w);
+    const int pooled_rows = a.m / (a.pool_h * a.pool_w) * d.oh * d.ow;
+    const void* ptrs[2] = {a.x, a.y};
+    const int vec = vec_ok(a.c, ptrs, 2) ? kEwVec : 1;
+    ew_config(pooled_rows, a.c, vec, &block, &grid);
+    const InferPoolKernel<P> k = infer_pool_kernel<P>(vec);
+    if (!k) return kNoKernel;
+    k<<<grid, block, 0, st>>>(x, y, p(b.running_mean), p(b.running_var), p(b.weight), p(b.bias), b.eps, d, pooled_rows, a.c);
+    return cudaGetLastError();
+  }
+  const void* ptrs[3] = {a.x, a.y, a.identity ? a.identity : a.x};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const InferTransformKernel<P> k = infer_transform_kernel<P>(vec, a.dual ? kTailBnAddRelu : a.identity ? kTailAddRelu : kTailRelu);
+  if (!k) return kNoKernel;
+  const InferParams& ds = a.ds;
+  k<<<grid, block, 0, st>>>(x, static_cast<const bf16*>(a.identity), y, p(b.running_mean), p(b.running_var), p(b.weight), p(b.bias), b.eps,
+                            p(ds.running_mean), p(ds.running_var), p(ds.weight), p(ds.bias), ds.eps, a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer(const InferArgs& a, cudaStream_t st) { return a.param_bf16 ? launch_infer<bf16>(a, st) : launch_infer<float>(a, st); }
 
 // ---- sync batch norm ----
 // The sync scratch is the local one followed, from a 16-byte boundary, by W + 1 rows of [mean | invstd | count]:

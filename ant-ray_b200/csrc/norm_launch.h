@@ -83,5 +83,26 @@ cudaError_t sync_bwd_reduce(const BwdArgs& a, cudaStream_t s);
 cudaError_t sync_bwd_elemt(const BwdArgs& a, cudaStream_t s);
 cudaError_t load_kernels();   // every batch-norm kernel, into the current context
 
+// Eval-mode sites (norm_infer.cuh): one kernel each, no scratch, nothing written but y.  Weight, bias and running
+// statistics of each batch norm are [c] of fp32, or of bf16 with param_bf16.
+struct InferParams {
+  const void* weight;
+  const void* bias;
+  const void* running_mean;
+  const void* running_var;
+  float eps;
+};
+struct InferArgs {
+  const void* x;         // bf16 [m][c]
+  const void* identity;  // bf16 [m][c], or null: no residual add; with `ds`, the downsample branch's batch-norm input
+  void* y;               // bf16 [m][c], or the pooled rows of the stem
+  InferParams bn;
+  InferParams ds;        // the downsample branch's batch norm (dual), else unused
+  bool dual, param_bf16;
+  int m, c;
+  int pool_h, pool_w;    // the stem (pool_h > 0): y = max_pool2d(relu(bn(x)), 3, 2, 1) over m / (pool_h * pool_w) images
+};
+cudaError_t infer(const InferArgs& a, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

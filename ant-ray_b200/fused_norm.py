@@ -1,4 +1,4 @@
-"""Fused batch norm for the ResNet training step (libb200coll.so, norm_kernels.cuh).
+"""Fused batch norm for the ResNet training step and eval forward (libb200coll.so, norm_kernels.cuh, norm_infer.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
 by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
@@ -14,6 +14,17 @@ value per channel, a channel stride of 1 and at most 131072 channels, its batch 
 a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum, and
 torch would run it on its native kernels (`torch._C._select_batch_norm_backend`).  Otherwise the block runs the
 parent class's ops, so the choice never changes a result.
+
+Eval mode: where no gradient is recorded (`torch.no_grad()`, `torch.inference_mode()`, or nothing the site reads
+requires grad), the same four kinds of site run as one native launch each on the eval kernels, which read the
+running statistics and write only the site's output (no running statistic, no `num_batches_tracked`), with the bits
+of eager torch's eval batch norm and the ReLU, add and max-pool after it.  A site runs there when its batch norm is
+a `BatchNorm2d`, or a SyncBatchNorm (which torch does not synchronise in eval), in eval mode with running
+statistics and a positive eps; its weight, bias and running statistics are contiguous on the input's device and
+all fp32 or all bf16 (a model cast to bf16); the input is a non-empty bf16 channels-last CUDA tensor with a channel
+stride of 1 and fewer than 2^31 elements; torch would run it on its native kernels; and no hook of the batch norm,
+the ReLU or the global registry would be skipped.  Otherwise the site runs torch's ops.  With gradients recorded,
+eval runs the parent classes' forward.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -307,6 +318,43 @@ def _fusable(bn, relu, x):
     return torch._C._select_batch_norm_backend(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, True, bn.eps) == _NATIVE
 
 
+_PARAM_DTYPES = ({torch.float32}, {torch.bfloat16})
+
+
+def _infer_ok(bn, relu, x, *operands):
+    """Whether this site can run as an eval site (the module docstring's conditions): `operands` are the other tensors
+    the kernel reads (the identity), which must not require grad either."""
+    # eps <= 0 stays on torch, whose F.batch_norm raises for it
+    if bn.training or not (type(bn) is nn.BatchNorm2d or isinstance(bn, nn.SyncBatchNorm)) or not bn.eps > 0:
+        return False
+    if type(relu) is not nn.ReLU or _hooked(bn) or _hooked(relu) or _global_hooks():
+        return False
+    params = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
+    if any(t is None or not t.is_contiguous() or t.device != x.device for t in params) or {t.dtype for t in params} not in _PARAM_DTYPES:
+        return False
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (x, bn.weight, bn.bias, *operands)):
+        return False
+    if not _activation(x) or x.numel() == 0 or x.numel() >= 2 ** 31:
+        return False
+    return torch._C._select_batch_norm_backend(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, False, bn.eps) == _NATIVE
+
+
+def _infer_params(bn):
+    """weight, bias, running_mean and running_var of an eval site's batch norm, and its param_bf16 flag."""
+    return (bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+            int(bn.weight.dtype == torch.bfloat16))
+
+
+def _infer(bn, x, identity=None):
+    """relu(bn(x)) or relu(bn(x) + identity) of an eval site, in one native launch."""
+    y = torch.empty_like(x)
+    c = x.shape[1]
+    N.check(_native_lib().b200c_bn_infer(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
+                                         *_infer_params(bn), bn.eps, x.numel() // c, c,
+                                         _raw_stream(x.device.index)))
+    return y
+
+
 def _rows(t):
     """_activation, where a tensor without elements (a rank with an empty batch) passes on its device, dtype and rank
     alone: its strides say nothing (a convolution over an empty batch returns default strides whatever its input's
@@ -329,6 +377,8 @@ def _sync_comm(bn, x):
 
 def bn_relu(bn, relu, x):
     """relu(bn(x)), fused when the site allows it."""
+    if _infer_ok(bn, relu, x):
+        return _infer(bn, x)
     comm = _sync_comm(bn, x)
     if comm is not None and _relu_fusable(bn, relu):
         return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, comm, True)
@@ -349,6 +399,13 @@ def _pool_fusable(pool):
 def bn_relu_maxpool(bn, relu, pool, x):
     """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) and the batch norm can run as a local
     fused site; otherwise bn_relu and the module call."""
+    if _pool_fusable(pool) and _infer_ok(bn, relu, x):
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device,
+                        memory_format=torch.channels_last)
+        N.check(_native_lib().b200c_bn_infer_pool(x.data_ptr(), y.data_ptr(), *_infer_params(bn), bn.eps, n, h, w, c,
+                                                  _raw_stream(x.device.index)))
+        return y
     if _pool_fusable(pool) and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
         return _FusedBatchNormPool.apply(x, bn.weight, bn.bias, bn)
     return pool(bn_relu(bn, relu, x))
@@ -357,6 +414,9 @@ def bn_relu_maxpool(bn, relu, pool, x):
 def bn_add_relu(bn, relu, x, identity, pair=False):
     """`out = bn(x); out += identity; relu(out)`, fused when the site allows it.  With `pair`, returns `(out,
     out_id)`: the same values, whose gradients a fused site receives apart and sums in its backward kernel."""
+    if _infer_ok(bn, relu, x, identity) and _activation(identity) and identity.shape == x.shape and identity.device == x.device:
+        out = _infer(bn, x, identity)
+        return (out, out) if pair else out
     comm = _sync_comm(bn, x)
     if comm is not None:
         if _relu_fusable(bn, relu) and _rows(identity) and identity.shape == x.shape:
@@ -382,8 +442,20 @@ def _downsample_bn(ds):
 def bn_add_relu_downsample(bn, relu, x, downsample, x_id, pair=False):
     """`out = bn(x); out += downsample(x_id); relu(out)`, with `pair` as in bn_add_relu.  Where the downsample branch is
     a convolution and a batch norm that can run as a local fused site alongside this one, both batch norms run in
-    one native call per direction and the branch's output is never written; otherwise bn_add_relu."""
+    one native call per direction (in eval, one launch) and the branch's output is never written; otherwise
+    bn_add_relu."""
     bn_ds = _downsample_bn(downsample)
+    if bn_ds is not None and bn_ds is not bn and _infer_ok(bn, relu, x):
+        x_ds = downsample[0](x_id)
+        if x_ds.shape == x.shape and _infer_ok(bn_ds, relu, x_ds) and bn_ds.weight.dtype == bn.weight.dtype:
+            y = torch.empty_like(x)
+            c = x.shape[1]
+            ptrs, ptrs_ds = _infer_params(bn)[:4], _infer_params(bn_ds)[:4]
+            N.check(_native_lib().b200c_bn_infer_dual(x.data_ptr(), x_ds.data_ptr(), y.data_ptr(), *ptrs, bn.eps, *ptrs_ds, bn_ds.eps,
+                                                      int(bn.weight.dtype == torch.bfloat16), x.numel() // c, c,
+                                                      _raw_stream(x.device.index)))
+            return (y, y) if pair else y
+        return bn_add_relu(bn, relu, x, bn_ds(x_ds), pair)
     if bn_ds is not None and bn_ds is not bn and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
         x_ds = downsample[0](x_id)
         if (x_ds.shape == x.shape and _sync_comm(bn_ds, x_ds) is None and _fusable(bn_ds, relu, x_ds)
@@ -414,9 +486,12 @@ else:
     # as separate tensors and returns its output twice, so that chained blocks hand each tail's backward the two
     # gradients of its output apart, to be summed inside the kernel instead of by a separate add.
 
+    # In eval mode without autograd recording the same helpers run each site on the eval kernels (one launch per
+    # site); with autograd recording, eval keeps the parent class's ops.
+
     class FusedBasicBlock(BasicBlock):
         def forward(self, x):
-            if not self.training:
+            if not self.training and torch.is_grad_enabled():
                 return super().forward(x)
             return self.forward_pair(x, x)[0]
 
@@ -429,7 +504,7 @@ else:
 
     class FusedBottleneck(Bottleneck):
         def forward(self, x):
-            if not self.training:
+            if not self.training and torch.is_grad_enabled():
                 return super().forward(x)
             return self.forward_pair(x, x)[0]
 
@@ -449,12 +524,12 @@ else:
 
     class FusedResNet(ResNet):
         def forward(self, x):
-            if not self.training:
+            if not self.training and torch.is_grad_enabled():
                 return super().forward(x)
             x = x_id = bn_relu_maxpool(self.bn1, self.relu, self.maxpool, self.conv1(x))   # two gradients, summed by autograd
             hooks = _global_hooks()
             for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
-                if not hooks and _pairwise(layer):
+                if self.training and not hooks and _pairwise(layer):
                     for block in layer:
                         x, x_id = block.forward_pair(x, x_id)
                 else:
@@ -502,7 +577,12 @@ def sync_batch_norm(model, comm):
 
 def fuse_resnet(model):
     """Rewrite `model` in place: every module whose class is exactly torchvision's ResNet, Bottleneck or BasicBlock
-    gets the fused subclass.  Parameters, buffers, state_dict keys, hooks and the object itself are unchanged."""
+    gets the fused subclass.  Parameters, buffers, state_dict keys, hooks and the object itself are unchanged.
+
+    This is also the entry point for inference: after `model.eval()`, a forward under `torch.inference_mode()` or
+    `torch.no_grad()` on bf16 channels-last input (autocast with fp32 parameters, or a model cast to bf16) runs every
+    batch norm of the model, with the ReLU, residual add and stem max-pool after it, as one native launch per site,
+    bit-identical to the untouched model."""
     for mod in model.modules():
         cls = _SWAP.get(type(mod))
         if cls is not None:

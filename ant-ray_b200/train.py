@@ -127,7 +127,9 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
     torchvision ResNet is first rewritten in place by `fused_norm.fuse_resnet`, and with more than one rank the
     model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
-    communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.
+    communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten ResNet's
+    eval forward under `torch.no_grad()` or `torch.inference_mode()` (validation) runs each batch-norm site as one
+    native eval launch with eager torch's bits; SyncBatchNorm does not synchronise in eval, so those run locally.
     """
     parallel_strategy_kwargs = dict(parallel_strategy_kwargs or {})
     device = move_to_device if isinstance(move_to_device, torch.device) else get_device()

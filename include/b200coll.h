@@ -361,6 +361,28 @@ int b200c_bn_backward_pool(const void* dy, const uint8_t* argmax, const void* x,
                            const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
                            int h, int w, int channels, void* scratch, b200c_stream_t stream);
 
+/* ---- fused batch norm (eval) over channels-last bf16 activations ----
+ * An eval-mode batch norm with its running statistics and what follows it in a ResNet, in one kernel, bit-identical
+ * to eager torch's batch_norm (train = false: invstd = rsqrt(float(running_var) + eps), then w * (x - mean) * invstd
+ * + bias) followed by the bf16 ops after it.  weight, bias, running_mean and running_var are [channels] of fp32, or of
+ * bf16 with param_bf16 = 1 (widened to fp32, as torch widens them).  Only y is written: no running statistic, no
+ * num_batches_tracked, no mask and no scratch.  m >= 1 rows of `channels` (NHWC memory order), fewer than 2^31
+ * elements; every argument is checked before the launch.  1 kernel each.
+ *
+ * b200c_bn_infer: y = relu(bn(x)), or with `identity` (may be NULL) y = relu(bn(x) + identity).
+ * b200c_bn_infer_dual: y = relu(bn(x) + bn_ds(x_ds)), a block tail whose identity is a downsample branch's batch norm;
+ * each batch norm has its own parameters and eps, of the one parameter type.
+ * b200c_bn_infer_pool: the stem, y = max_pool2d(relu(bn(x)), 3, stride 2, padding 1) over n images of h x w rows,
+ * selected as b200c_bn_forward_pool selects; writes the pooled rows only (no argmax). */
+int b200c_bn_infer(const void* x, const void* identity, void* y, const void* weight, const void* bias, const void* running_mean,
+                   const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
+int b200c_bn_infer_dual(const void* x, const void* x_ds, void* y, const void* weight, const void* bias, const void* running_mean,
+                        const void* running_var, float eps, const void* weight_ds, const void* bias_ds, const void* running_mean_ds,
+                        const void* running_var_ds, float eps_ds, int param_bf16, int m, int channels, b200c_stream_t stream);
+int b200c_bn_infer_pool(const void* x, void* y, const void* weight, const void* bias, const void* running_mean,
+                        const void* running_var, int param_bf16, float eps, int n, int h, int w, int channels,
+                        b200c_stream_t stream);
+
 /* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
  * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
  * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)

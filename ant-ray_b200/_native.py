@@ -35,6 +35,8 @@ SUM, PROD, MAX, MIN, AVG = range(5)
 ALGO_AUTO, ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS, ALGO_NVLS_PIPE, ALGO_LL, ALGO_NVLS_LANES, ALGO_NVLS_STREAMS = range(8)
 # b200c_share_mode_t
 SHARE_VMM_FD, SHARE_LEGACY_IPC = 0, 1
+# b200c_act_t: the activation of a b200c_bn_*_act site
+ACT_RELU6, ACT_SILU, ACT_HARDSWISH = 1, 2, 3
 MAX_RANKS = 8
 
 
@@ -116,6 +118,9 @@ SYMBOLS = {
     "b200c_bn_infer": (c_int, [c_void_p] * 7 + [c_int, c_float, c_int, c_int, c_void_p]),
     "b200c_bn_infer_dual": (c_int, [c_void_p] * 7 + [c_float] + [c_void_p] * 4 + [c_float, c_int, c_int, c_int, c_void_p]),
     "b200c_bn_infer_pool": (c_int, [c_void_p] * 6 + [c_int, c_float] + [c_int] * 4 + [c_void_p]),
+    "b200c_bn_forward_act": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "b200c_bn_backward_act": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_infer_act": (c_int, [c_void_p] * 6 + [c_int, c_float, c_int, c_int, c_int, c_void_p]),
     "b200c_bn_sync_scratch_bytes": (c_size_t, [c_int, c_int]),
     "b200c_bn_sync_forward": (c_int, [c_void_p] * 5 + [c_int] + [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_sync_backward": (c_int, [c_void_p] * 5 + [c_int] + [c_void_p] * 9 + [c_int, c_int, c_void_p, c_void_p]),

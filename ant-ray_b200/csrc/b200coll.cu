@@ -1643,6 +1643,57 @@ extern "C" int b200c_bn_infer_pool(const void* x, void* y, const void* weight, c
   return run_infer({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, h, w}, stream);
 }
 
+// A batch norm followed by ReLU6, SiLU or Hardswish (norm_act.cuh): the local site's checks, an activation the kernels
+// have, and (the eval site too) at most kMaxChannels channels.
+static int check_act(const char* site, int act, int c) {
+  if (!bn::act_ok(act)) return fail(B200C_EINVAL, "%s: unknown act=%d", site, act);
+  if (c > bn::kMaxChannels) return fail(B200C_EINVAL, "%s: channels=%d above %d", site, c, bn::kMaxChannels);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_act(const void* x, void* y, const float* weight, const float* bias, float* running_mean,
+                                    float* running_var, int64_t* num_batches_tracked, float* save_mean, float* save_invstd, int act,
+                                    int m, int channels, float momentum, float eps, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm act", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (!rc) rc = check_act("batch norm act", act, channels);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
+    return fail(B200C_EINVAL, "batch norm act forward: null buffer");
+  const bn::FwdArgs a{x, nullptr, y, nullptr, false, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  RT(bn::forward_act(a, act, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_act(const void* dy, const void* x, void* g, void* dx, const float* weight, const float* bias,
+                                     const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int act,
+                                     int m, int channels, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm act", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (!rc) rc = check_act("batch norm act", act, channels);
+  if (rc) return rc;
+  if (!dy || !x || !g || !dx || !weight || !bias || !save_mean || !save_invstd || !grad_weight || !grad_bias)
+    return fail(B200C_EINVAL, "batch norm act backward: null buffer");
+  const bn::BwdArgs a{dy, nullptr, nullptr, nullptr, x, g, dx, false, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                      m, channels, scratch};
+  RT(bn::backward_act(a, bias, act, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_act(const void* x, void* y, const void* weight, const void* bias, const void* running_mean,
+                                  const void* running_var, int param_bf16, float eps, int act, int m, int channels,
+                                  b200c_stream_t stream) {
+  int rc = check_infer("batch norm infer act", param_bf16, m, channels);
+  if (!rc) rc = check_act("batch norm infer act", act, channels);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer act: null buffer");
+  RT(bn::infer_act({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0}, act,
+                   (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {
   int rc = check_ready(c);
   if (rc) return rc;

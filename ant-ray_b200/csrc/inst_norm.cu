@@ -1,8 +1,10 @@
-// Launchers of the fused batch-norm kernels (norm_kernels.cuh); argument checking lives in b200coll.cu.
+// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh); argument checking lives
+// in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
 
+#include "norm_act.cuh"
 #include "norm_infer.cuh"
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
@@ -169,6 +171,35 @@ static InferPoolKernel<P> infer_pool_kernel(int vec) {
   return with_const<1, kEwVec>(vec, [](auto v) -> InferPoolKernel<P> { return bn_infer::k_infer_pool<decltype(v)::value, P>; });
 }
 
+// the kernels of a batch norm followed by ReLU6, SiLU or Hardswish (norm_act.cuh), by b200c_act_t
+using bn_act::Act;
+using ActTransformKernel = void (*)(const bf16*, bf16*, const float*, const float*, const float*, const float*, int, int);
+using ActBwdReduceKernel = void (*)(const bf16*, const bf16*, const float*, const float*, const float*, const float*, float*, float*,
+                                    float*, float*, volatile float*, int*, bf16*, int, int);
+template <typename P>
+using ActInferKernel = void (*)(const bf16*, bf16*, const P*, const P*, const P*, const P*, float, int, int);
+
+template <typename F>
+static auto with_act(int act, F&& f) {
+  return with_const<bn_act::kActRelu6, bn_act::kActSilu, bn_act::kActHardswish>(act, f);
+}
+bool act_ok(int act) { return act == bn_act::kActRelu6 || act == bn_act::kActSilu || act == bn_act::kActHardswish; }
+
+static ActTransformKernel act_transform_kernel(int vec, int act) {
+  return with_const<1, kEwVec>(vec, [&](auto v) {
+    return with_act(act, [](auto a) -> ActTransformKernel { return bn_act::k_act_transform<decltype(v)::value, (Act) decltype(a)::value>; });
+  });
+}
+static ActBwdReduceKernel act_bwd_reduce_kernel(int act) {
+  return with_act(act, [](auto a) -> ActBwdReduceKernel { return bn_act::k_act_bwd_reduce<(Act) decltype(a)::value>; });
+}
+template <typename P>
+static ActInferKernel<P> act_infer_kernel(int vec, int act) {
+  return with_const<1, kEwVec>(vec, [&](auto v) {
+    return with_act(act, [](auto a) -> ActInferKernel<P> { return bn_act::k_act_infer<decltype(v)::value, (Act) decltype(a)::value, P>; });
+  });
+}
+
 // Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
 // load a kernel lazily while a peer's collective waits): every key value goes through the functions above.
 cudaError_t load_kernels() {
@@ -194,6 +225,12 @@ cudaError_t load_kernels() {
     for (int tail = 0; tail < kTails; tail++) {
       load(infer_transform_kernel<float>(vec, tail));
       load(infer_transform_kernel<bf16>(vec, tail));
+    }
+    for (int act : {bn_act::kActRelu6, bn_act::kActSilu, bn_act::kActHardswish}) {
+      if (vec == 1) load(act_bwd_reduce_kernel(act));
+      load(act_transform_kernel(vec, act));
+      load(act_infer_kernel<float>(vec, act));
+      load(act_infer_kernel<bf16>(vec, act));
     }
   }
   return e;
@@ -408,6 +445,64 @@ static cudaError_t launch_infer(const InferArgs& a, cudaStream_t st) {
 }
 
 cudaError_t infer(const InferArgs& a, cudaStream_t st) { return a.param_bf16 ? launch_infer<bf16>(a, st) : launch_infer<float>(a, st); }
+
+// ---- batch norm followed by ReLU6, SiLU or Hardswish ----
+// The statistics are the local site's (k_bn_stats); the transform, like k_bn_transform, then writes act(t).
+cudaError_t forward_act(const FwdArgs& a, int act, cudaStream_t st) {
+  const cudaError_t e = launch_stats(a, nullptr, st);
+  if (e != cudaSuccess) return e;
+  const void* ptrs[2] = {a.x, a.y};
+  const int vec = vec_ok(a.c, ptrs, 2) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const ActTransformKernel k = act_transform_kernel(vec, act);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), a.save_mean, a.save_invstd, a.weight, a.bias, a.m, a.c);
+  return cudaGetLastError();
+}
+
+// The reduce recomputes t, derives g from dy and writes it to a.dy_masked, with k_bn_bwd_reduce's launch shape; the
+// local site's elementwise kernel then reads g (kGradMasked) with this call's norm_fct = (float)(1.0 / m).
+cudaError_t backward_act(const BwdArgs& a, const float* bias, int act, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const ActBwdReduceKernel kr = act_bwd_reduce_kernel(act);
+  if (!kr) return kNoKernel;
+  const bf16* x = static_cast<const bf16*>(a.x);
+  bf16* g = static_cast<bf16*>(a.dy_masked);
+  kr<<<grid, block, 0, st>>>(x, static_cast<const bf16*>(a.dy), a.save_mean, a.save_invstd, a.weight, bias, s.sums, s.sums + a.c,
+                             a.grad_weight, a.grad_bias, s.staging, s.semaphores, g, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const void* ptrs[3] = {a.x, a.dx, g};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const BwdElemtKernel ke = bwd_elemt_kernel(vec, kGradMasked, false, false);
+  if (!ke) return kNoKernel;
+  ke<<<grid, block, 0, st>>>(g, nullptr, nullptr, nullptr, x, static_cast<bf16*>(a.dx), a.save_mean, a.save_invstd, a.weight, s.sums,
+                             s.sums + a.c, nullptr, (float)(1.0 / a.m), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.m, a.c);
+  return cudaGetLastError();
+}
+
+template <typename P>
+static cudaError_t launch_infer_act(const InferArgs& a, int act, cudaStream_t st) {
+  const void* ptrs[2] = {a.x, a.y};
+  const int vec = vec_ok(a.c, ptrs, 2) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const ActInferKernel<P> k = act_infer_kernel<P>(vec, act);
+  if (!k) return kNoKernel;
+  const InferParams& b = a.bn;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), static_cast<const P*>(b.running_mean),
+                            static_cast<const P*>(b.running_var), static_cast<const P*>(b.weight), static_cast<const P*>(b.bias), b.eps,
+                            a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_act(const InferArgs& a, int act, cudaStream_t st) {
+  return a.param_bf16 ? launch_infer_act<bf16>(a, act, st) : launch_infer_act<float>(a, act, st);
+}
 
 // ---- sync batch norm ----
 // The sync scratch is the local one followed, from a 16-byte boundary, by W + 1 rows of [mean | invstd | count]:

@@ -104,5 +104,15 @@ struct InferArgs {
 };
 cudaError_t infer(const InferArgs& a, cudaStream_t s);
 
+// Batch norm followed by ReLU6, SiLU or Hardswish (norm_act.cuh; act is b200c_act_t).  A local training site: the
+// forward reads FwdArgs without identity, mask or stem (2 kernels), the backward BwdArgs.dy / x / dx / weight, the
+// statistics, sums and scratch, and `bias` to recompute the batch norm's output, and writes the activation's gradient g
+// to BwdArgs.dy_masked (2 kernels).  The eval site reads
+// InferArgs without identity, downsample or stem (1 kernel).
+bool act_ok(int act);
+cudaError_t forward_act(const FwdArgs& a, int act, cudaStream_t s);
+cudaError_t backward_act(const BwdArgs& a, const float* bias, int act, cudaStream_t s);
+cudaError_t infer_act(const InferArgs& a, int act, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

@@ -1,4 +1,5 @@
-"""Fused batch norm for the ResNet training step and eval forward (libb200coll.so, norm_kernels.cuh, norm_infer.cuh).
+"""Fused batch norm for the training step and eval forward of ResNets and of torchvision's Conv2dNormActivation blocks
+(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
 by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
@@ -25,6 +26,13 @@ all fp32 or all bf16 (a model cast to bf16); the input is a non-empty bf16 chann
 stride of 1 and fewer than 2^31 elements; torch would run it on its native kernels; and no hook of the batch norm,
 the ReLU or the global registry would be skipped.  Otherwise the site runs torch's ops.  With gradients recorded,
 eval runs the parent classes' forward.
+
+Conv2dNormActivation: `fuse_model` also swaps every torchvision `Conv2dNormActivation` that ends in an nn.ReLU6,
+nn.SiLU or nn.Hardswish (MobileNetV2 / V3, EfficientNet) for `FusedConv2dNormActivation`, whose batch norm and
+activation run as one site per direction (`bn_act`, norm_act.cuh): the forward writes act(bn(x)) with eager torch's
+bits, and the backward recomputes bn(x) from x instead of saving it.  `bn_act` runs nn.ReLU on the ReLU sites above.  The
+conditions are those above, with no hook on the batch norm or the activation; in eval without autograd recording the
+site is one launch.  A sync site with one of those activations runs the sync batch norm alone, then the activation.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -277,6 +285,66 @@ class _FusedBatchNormPool(torch.autograd.Function):
         return dx, grad_weight, grad_bias, None
 
 
+# eager torch's backward of each activation, g of (dy, t)
+_ACT_BACKWARD = {N.ACT_RELU6: lambda dy, t: torch.ops.aten.hardtanh_backward(dy, t, 0.0, 6.0),
+                 N.ACT_SILU: torch.ops.aten.silu_backward, N.ACT_HARDSWISH: torch.ops.aten.hardswish_backward}
+
+
+class _FusedBatchNormAct(torch.autograd.Function):
+    """act(bn(x)) in training mode, act being ReLU6, SiLU or Hardswish (`code`, the library's b200c_act_t).  The
+    batch norm's output is never written: the backward recomputes it from x, the saved statistics, weight and bias, and
+    writes the activation's gradient g for the batch norm's elementwise backward.
+
+    A gradient that arrives in another layout than channels-last (at the last block before a model's average pool)
+    makes eager torch's activation backward write g in that layout, and its batch-norm backward then runs its NCHW
+    kernels, whose sums round differently.  There the backward runs those torch ops on t recomputed by torch's own
+    transform, so the bits stay eager torch's."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, bn, code):
+        lib = _native_lib()
+        c = x.shape[1]
+        m = x.numel() // c
+        y = torch.empty_like(x)
+        nbt = bn.num_batches_tracked
+        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_forward_act(x.data_ptr(), y.data_ptr(), weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(),
+                                         bn.running_var.data_ptr(), nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c,
+                                         code, m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        ctx.code, ctx.eps = code, bn.eps
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, weight, bias, stats)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None, None, None
+        x, weight, bias, stats = ctx.saved_tensors
+        c = x.shape[1]
+        m = x.numel() // c
+        if not dy.is_contiguous(memory_format=torch.channels_last):
+            mean, invstd = stats[:c], stats[c:]
+            t = torch.batch_norm_elemt(x, weight, bias, mean, invstd, ctx.eps)
+            g = _ACT_BACKWARD[ctx.code](dy, t)
+            # the running statistics are not read in training mode
+            return (*torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, mean, invstd, True, ctx.eps,
+                                                               [True, True, True]), None, None)
+        lib = _native_lib()
+        g, dx = torch.empty_like(x), torch.empty_like(x)
+        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
+        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_backward_act(dy.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(), weight.data_ptr(), bias.data_ptr(), mean,
+                                          mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), ctx.code, m, c,
+                                          _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        return dx, grad_weight, grad_bias, None, None
+
+
 def _activation(t):
     # With one channel, NCHW strides also pass the channels-last check, but torch runs its NCHW statistics kernel
     # unless stride(1) == 1 (batch_norm_choose_impl), so the channel stride must be 1 as well.
@@ -307,8 +375,13 @@ def _relu_fusable(bn, relu):
 def _fusable(bn, relu, x):
     """Whether this site can run fused as a local site: the conditions of the module docstring.  A site that cannot
     falls back to the parent class's ops."""
+    return _relu_fusable(bn, relu) and _local_ok(bn, x)
+
+
+def _local_ok(bn, x):
+    """_fusable's conditions on the batch norm and its input."""
     local = type(bn) is nn.BatchNorm2d or (isinstance(bn, nn.SyncBatchNorm) and not _torch_syncs(bn))
-    if not local or not _relu_fusable(bn, relu) or not _module_ok(bn):
+    if not local or not _module_ok(bn):
         return False
     if not _activation(x) or x.numel() >= 2 ** 31:
         return False
@@ -324,10 +397,18 @@ _PARAM_DTYPES = ({torch.float32}, {torch.bfloat16})
 def _infer_ok(bn, relu, x, *operands):
     """Whether this site can run as an eval site (the module docstring's conditions): `operands` are the other tensors
     the kernel reads (the identity), which must not require grad either."""
+    return type(relu) is nn.ReLU and not _skips_hooks(bn, relu) and _infer_bn_ok(bn, x, *operands)
+
+
+def _skips_hooks(bn, act):
+    """Whether calling a kernel instead of `bn` and `act` would skip a hook: theirs or the global registry's."""
+    return _hooked(bn) or _hooked(act) or _global_hooks()
+
+
+def _infer_bn_ok(bn, x, *operands):
+    """_infer_ok's conditions on the batch norm and its input."""
     # eps <= 0 stays on torch, whose F.batch_norm raises for it
     if bn.training or not (type(bn) is nn.BatchNorm2d or isinstance(bn, nn.SyncBatchNorm)) or not bn.eps > 0:
-        return False
-    if type(relu) is not nn.ReLU or _hooked(bn) or _hooked(relu) or _global_hooks():
         return False
     params = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
     if any(t is None or not t.is_contiguous() or t.device != x.device for t in params) or {t.dtype for t in params} not in _PARAM_DTYPES:
@@ -385,6 +466,31 @@ def bn_relu(bn, relu, x):
     if comm is None and _fusable(bn, relu, x):
         return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False)
     return relu(bn(x))
+
+
+# activations with native batch-norm sites of their own, by their b200c_act_t (ReLU runs on bn_relu's sites)
+_ACT_CODES = {nn.ReLU6: N.ACT_RELU6, nn.SiLU: N.ACT_SILU, nn.Hardswish: N.ACT_HARDSWISH}
+
+
+def bn_act(bn, act, x):
+    """act(bn(x)) for `act` an nn.ReLU, nn.ReLU6, nn.SiLU or nn.Hardswish (exactly those classes), fused when the site
+    allows it: ReLU through bn_relu (its sync sites included); for the others an eval site, else a local training
+    site, with the conditions of bn_relu's and no hook on `act`.  A sync site with another activation runs the
+    batch norm's own forward (FusedSyncBatchNorm's sync site) and then `act`; anything else runs `act(bn(x))`."""
+    if type(act) is nn.ReLU:
+        return bn_relu(bn, act, x)
+    code = _ACT_CODES.get(type(act))
+    if code is None or _skips_hooks(bn, act):
+        return act(bn(x))
+    if _infer_bn_ok(bn, x):
+        y = torch.empty_like(x)
+        c = x.shape[1]
+        N.check(_native_lib().b200c_bn_infer_act(x.data_ptr(), y.data_ptr(), *_infer_params(bn), bn.eps, code, x.numel() // c, c,
+                                                 _raw_stream(x.device.index)))
+        return y
+    if _sync_comm(bn, x) is None and _local_ok(bn, x):
+        return _FusedBatchNormAct.apply(x, bn.weight, bn.bias, bn, code)
+    return act(bn(x))
 
 
 def _pool_fusable(pool):
@@ -572,6 +678,45 @@ def sync_batch_norm(model, comm):
         if type(mod) in (nn.SyncBatchNorm, FusedSyncBatchNorm) and _world_group(mod.process_group):
             mod.__class__ = FusedSyncBatchNorm
             mod.b200_comm = comm
+    return model
+
+
+try:
+    from torchvision.ops.misc import Conv2dNormActivation
+except ImportError:  # without torchvision there is nothing to rewrite
+    Conv2dNormActivation = None
+else:
+
+    class FusedConv2dNormActivation(Conv2dNormActivation):
+        """torchvision's Conv2dNormActivation whose batch norm and activation run as one site (`bn_act`) when the block
+        is exactly an nn.Conv2d, a BatchNorm2d or SyncBatchNorm, and an nn.ReLU6, SiLU or Hardswish, and calling the
+        kernels instead of those two modules skips no hook.  The convolution is still called as a module, and the
+        block's own hooks run as before.  Anything else, and eval with gradients recorded, runs the parent's forward."""
+
+        def forward(self, x):
+            if len(self) != 3 or (not self.training and torch.is_grad_enabled()):
+                return super().forward(x)
+            conv, bn, act = self[0], self[1], self[2]
+            if (type(conv) is not nn.Conv2d or not (type(bn) is nn.BatchNorm2d or isinstance(bn, nn.SyncBatchNorm))
+                    or type(act) not in _ACT_CODES):
+                return super().forward(x)
+            return bn_act(bn, act, conv(x))
+
+def fuse_model(model):
+    """Rewrite `model` in place: `fuse_resnet`, and every module whose class is exactly torchvision's
+    Conv2dNormActivation and whose last module is an nn.ReLU6, SiLU or Hardswish (MobileNetV2 / V3, EfficientNet)
+    becomes a FusedConv2dNormActivation.  Parameters, buffers, state_dict keys, hooks and the object itself are
+    unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in training and in eval
+    (see `fuse_resnet` for inference).
+
+    Blocks ending in nn.ReLU (MobileNetV3, RegNet) keep torchvision's forward: bn_act would run them on bn_relu's sites,
+    but a regnet_y_400mf training step with them fused took about 11 ms more host time than the untouched model (DESIGN.md
+    section 10), more than the kernel time they save."""
+    fuse_resnet(model)
+    if Conv2dNormActivation is not None:
+        for mod in model.modules():
+            if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
+                mod.__class__ = FusedConv2dNormActivation
     return model
 
 

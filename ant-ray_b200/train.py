@@ -125,9 +125,11 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     Same arguments as the reference (v2/torch/train_loop_utils.py:166-248); `grad_wire` overrides
     the backend config's wire type, `wrap_single` wraps in DDP / FSDP even at world size 1 (the
     reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
-    torchvision ResNet is first rewritten in place by `fused_norm.fuse_resnet`, and with more than one rank the
+    torchvision ResNet, and every torchvision Conv2dNormActivation ending in ReLU6, SiLU or Hardswish (MobileNetV2 / V3,
+    EfficientNet), is first
+    rewritten in place by `fused_norm.fuse_model`, and with more than one rank the
     model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
-    communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten ResNet's
+    communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten blocks'
     eval forward under `torch.no_grad()` or `torch.inference_mode()` (validation) runs each batch-norm site as one
     native eval launch with eager torch's bits; SyncBatchNorm does not synchronise in eval, so those run locally.
     """
@@ -138,10 +140,11 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     if move_to_device:
         model = model.to(device)
     if device.type == "cuda":
-        # batch norm + ReLU (+ residual add) of torchvision ResNets as fused native sites; same bits as eager torch
+        # batch norm + ReLU (+ residual add) of torchvision ResNets, and batch norm + activation of Conv2dNormActivation
+        # blocks, as fused native sites; same bits as eager torch
         from . import fused_norm
 
-        fused_norm.fuse_resnet(model)
+        fused_norm.fuse_model(model)
     world_size = dist.get_world_size() if dist.is_initialized() else 1
     norm_comm = _attach_sync_norm(model, device, world_size)
     if parallel_strategy and (world_size > 1 or wrap_single):

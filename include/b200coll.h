@@ -383,6 +383,29 @@ int b200c_bn_infer_pool(const void* x, void* y, const void* weight, const void* 
                         const void* running_var, int param_bf16, float eps, int n, int h, int w, int channels,
                         b200c_stream_t stream);
 
+/* ---- fused batch norm followed by ReLU6, SiLU or Hardswish (torchvision's Conv2dNormActivation) ----
+ * y = act(bn(x)) over channels-last bf16 activations, bit-identical to eager torch's batch norm followed by its
+ * activation module: the batch norm's output t is rounded to bf16, the activation computed in fp32 as torch's CUDA
+ * kernels compute it and rounded to bf16.  t itself is never written.  `act` is a b200c_act_t; EINVAL for any other.
+ * Channels 1..131072, m >= 1 rows, fewer than 2^31 elements; every argument is checked before the first launch.
+ *
+ * b200c_bn_forward_act: the training forward of b200c_bn_forward (statistics, running statistics, num_batches_tracked,
+ * scratch of b200c_bn_scratch_bytes(channels)) without identity, writing act(t).  2 kernels.
+ * b200c_bn_backward_act: from dy (the gradient of y), x, weight, bias and the saved statistics, writes dx, grad_weight
+ * and grad_bias; the activation's gradient g is derived from dy and t recomputed from x, as torch's
+ * silu_backward / hardswish_backward / hardtanh_backward derive it from the saved t, rounded to bf16, and written to
+ * `g` (m rows, required), which the batch norm's elementwise backward reads.  2 kernels.
+ * b200c_bn_infer_act: the eval site of b200c_bn_infer without identity, writing act(t).  1 kernel. */
+typedef enum { B200C_ACT_RELU6 = 1, B200C_ACT_SILU = 2, B200C_ACT_HARDSWISH = 3 } b200c_act_t;
+int b200c_bn_forward_act(const void* x, void* y, const float* weight, const float* bias, float* running_mean, float* running_var,
+                         int64_t* num_batches_tracked, float* save_mean, float* save_invstd, int act, int m, int channels,
+                         float momentum, float eps, void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_act(const void* dy, const void* x, void* g, void* dx, const float* weight, const float* bias, const float* save_mean,
+                          const float* save_invstd, float* grad_weight, float* grad_bias, int act, int m, int channels, void* scratch,
+                          b200c_stream_t stream);
+int b200c_bn_infer_act(const void* x, void* y, const void* weight, const void* bias, const void* running_mean, const void* running_var,
+                       int param_bf16, float eps, int act, int m, int channels, b200c_stream_t stream);
+
 /* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
  * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
  * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)

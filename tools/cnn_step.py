@@ -1,0 +1,181 @@
+#!/usr/bin/env python
+"""Training step and eval forward of torchvision CNNs whose batch norms sit in Conv2dNormActivation blocks
+(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, regnet_y_400mf), with and without `fused_norm.fuse_model`.
+
+Batch `--batch` (256) at 224 x 224, bf16 autocast with fp32 parameters, channels-last, SGD with momentum.  Per model,
+alternating the two builds ("fused", "unfused") in one process, `--runs` times each, the order swapped every run:
+  train_images_per_sec   `--iters` training steps between device events, after `--warmup` steps
+  eval_images_per_sec    `--iters` forwards under inference_mode, the same way
+Both builds start from the same weights and train on the same batches, reseeded per step, so after the timed runs
+their parameters and eval logits must have identical bits ("identical").  Then the host's time per training step
+(forward and backward, no optimizer step): the wall time per step at batch `--host-batch` (4), where the GPU work is
+too small to set the pace.  Then, in a separate profiled run per build, the kernel time per step by family.
+
+Writes OUT/cnn_step.json; prints the summary.  The card's name and power limit are read in the same run.
+
+  python tools/cnn_step.py --out DIR [--models a,b] [--batch 256] [--runs 4] [--iters 10] [--warmup 3] [--host-batch 4]
+"""
+import argparse
+import copy
+import json
+import os
+import re
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for _p in (ROOT, os.path.join(ROOT, "tools")):
+    if _p not in sys.path:
+        sys.path.insert(0, _p)
+
+from step_profile import gpu_identity  # noqa: E402
+
+MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "regnet_y_400mf"]
+# first match wins
+FAMILIES = [
+    ("bn_stats", r"k_bn_stats|batch_norm_collect_statistics"),
+    ("bn_transform_act", r"k_act_transform|k_act_infer|k_bn_transform|k_infer_transform|batch_norm_transform_input"),
+    ("bn_bwd_reduce", r"k_act_bwd_reduce|k_bn_bwd_reduce|batch_norm_backward_reduce"),
+    ("bn_bwd_elemt", r"k_act_bwd_elemt|k_bn_bwd_elemt|batch_norm_backward_elemt"),
+    ("torch_act", r"silu|hardswish|hardsigmoid|clamp|hardtanh|threshold|relu"),
+    ("conv", r"conv|cudnn|xmma|gemm|nvjet|cutlass|fprop|dgrad|wgrad|implicit_|nhwc|nchw|sm90_"),
+]
+
+
+def family_of(name):
+    for fam, pat in FAMILIES:
+        if re.search(pat, name):
+            return fam
+    return "other"
+
+
+def main():
+    p = argparse.ArgumentParser()
+    p.add_argument("--out", required=True)
+    p.add_argument("--models", default=",".join(MODELS))
+    p.add_argument("--batch", type=int, default=256)
+    p.add_argument("--runs", type=int, default=4)
+    p.add_argument("--iters", type=int, default=10)
+    p.add_argument("--warmup", type=int, default=3)
+    p.add_argument("--host-batch", type=int, default=4)
+    args = p.parse_args()
+
+    import torch
+    import torch.nn.functional as F
+    import torchvision
+    from torch.profiler import ProfilerActivity, profile
+
+    from ant_ray_b200 import fused_norm
+
+    if not torch.cuda.is_available():
+        raise SystemExit("cnn_step.py measures the GPU step: it needs a CUDA device")
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True   # the two builds' results are compared bit for bit
+    device = torch.device("cuda", 0)
+    g = torch.Generator(device=device).manual_seed(3)
+    x = torch.randn(args.batch, 3, 224, 224, device=device, generator=g).contiguous(memory_format=torch.channels_last)
+    y = torch.randint(0, 1000, (args.batch,), device=device, generator=g)
+    out = {**gpu_identity(), "batch": args.batch, "runs": args.runs, "iters": args.iters, "models": {}}
+
+    for arch in args.models.split(","):
+        torch.manual_seed(0)
+        base = getattr(torchvision.models, arch)(weights=None).to(device).to(memory_format=torch.channels_last)
+        models = {"fused": fused_norm.fuse_model(copy.deepcopy(base)), "unfused": base}
+        opts = {b: torch.optim.SGD(m.parameters(), lr=0.01, momentum=0.9) for b, m in models.items()}
+        steps = {b: 0 for b in models}
+
+        def train_step(b):
+            torch.manual_seed(1000 + steps[b])   # dropout and stochastic depth draw the same masks in both builds
+            steps[b] += 1
+            with torch.autocast("cuda", dtype=torch.bfloat16):
+                loss = F.cross_entropy(models[b](x).float(), y)
+            opts[b].zero_grad(set_to_none=True)
+            loss.backward()
+            opts[b].step()
+
+        def forward(b):
+            with torch.inference_mode(), torch.autocast("cuda", dtype=torch.bfloat16):
+                return models[b](x)
+
+        def timed(b, fn):
+            for _ in range(args.warmup):
+                fn(b)
+            torch.cuda.synchronize()
+            start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            start.record()
+            for _ in range(args.iters):
+                fn(b)
+            end.record()
+            torch.cuda.synchronize()
+            return round(args.batch * args.iters / (start.elapsed_time(end) / 1e3), 1)
+
+        res = {b: {"train_images_per_sec": [], "eval_images_per_sec": []} for b in models}
+        for r in range(args.runs):
+            for b in (["fused", "unfused"] if r % 2 == 0 else ["unfused", "fused"]):   # alternating builds, ABBA
+                models[b].train()
+                res[b]["train_images_per_sec"].append(timed(b, train_step))
+                models[b].eval()
+                res[b]["eval_images_per_sec"].append(timed(b, forward))
+        ints = {2: torch.int16, 4: torch.int32}
+        same = lambda a, c: a.dtype == c.dtype and bool(torch.equal(a.view(ints[a.element_size()]), c.view(ints[c.element_size()])))  # noqa: E731
+        entry = {"builds": res, "act_sites": len([m for m in models["fused"].modules() if type(m) is fused_norm.FusedConv2dNormActivation and len(m) == 3]),
+                 "identical": {"parameters": all(same(a, c) for a, c in zip(models["fused"].parameters(), models["unfused"].parameters())),
+                               "buffers": all(same(a, c) for a, c in zip(models["fused"].buffers(), models["unfused"].buffers())
+                                              if a.is_floating_point()),
+                               "eval_logits": same(forward("fused"), forward("unfused"))}}
+        # host time: at batch `--host-batch` the GPU work is small, so a step's wall time is what the host needs to issue it
+        xs, ys = x[:args.host_batch].clone(), y[:args.host_batch].clone()
+
+        def host_step(b):
+            torch.manual_seed(0)
+            with torch.autocast("cuda", dtype=torch.bfloat16):
+                loss = F.cross_entropy(models[b](xs).float(), ys)
+            opts[b].zero_grad(set_to_none=True)
+            loss.backward()
+
+        host = {b: [] for b in models}
+        for r in range(args.runs):
+            for b in (["fused", "unfused"] if r % 2 == 0 else ["unfused", "fused"]):
+                models[b].train()
+                for _ in range(args.warmup):
+                    host_step(b)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                for _ in range(args.iters):
+                    host_step(b)
+                torch.cuda.synchronize()
+                host[b].append(round((time.perf_counter() - t0) / args.iters * 1e3, 2))
+        entry["host_ms_per_step"] = {"batch": args.host_batch, **host}
+        profiled = {}
+        for b in models:
+            models[b].train()
+            for _ in range(args.warmup):
+                train_step(b)
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(args.iters):
+                    train_step(b)
+                torch.cuda.synchronize()
+            fams = {}
+            for ev in prof.key_averages():
+                t = getattr(ev, "self_device_time_total", None)
+                if t is None:
+                    t = ev.self_cuda_time_total
+                if t > 0:
+                    fam = family_of(ev.key)
+                    fams[fam] = fams.get(fam, 0.0) + t / args.iters / 1e3
+            profiled[b] = {"kernel_ms_per_step": round(sum(fams.values()), 3),
+                           "families_ms_per_step": {k: round(v, 3) for k, v in sorted(fams.items(), key=lambda kv: -kv[1])}}
+        entry["profile"] = profiled
+        out["models"][arch] = entry
+        del models, opts, base
+        torch.cuda.empty_cache()
+
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "cnn_step.json"), "w") as f:
+        json.dump(out, f, indent=1)
+    print(json.dumps(out, indent=1))
+
+
+if __name__ == "__main__":
+    main()

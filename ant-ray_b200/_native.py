@@ -121,6 +121,9 @@ SYMBOLS = {
     "b200c_bn_forward_act": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_backward_act": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200c_bn_infer_act": (c_int, [c_void_p] * 6 + [c_int, c_float, c_int, c_int, c_int, c_void_p]),
+    "b200c_bn_forward_res": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "b200c_bn_backward_res": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 8 + [c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_infer_res": (c_int, [c_void_p] * 7 + [c_int, c_float, c_int, c_int, c_void_p]),
     "b200c_bn_sync_scratch_bytes": (c_size_t, [c_int, c_int]),
     "b200c_bn_sync_forward": (c_int, [c_void_p] * 5 + [c_int] + [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_sync_backward": (c_int, [c_void_p] * 5 + [c_int] + [c_void_p] * 9 + [c_int, c_int, c_void_p, c_void_p]),

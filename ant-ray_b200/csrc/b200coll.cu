@@ -1694,6 +1694,62 @@ extern "C" int b200c_bn_infer_act(const void* x, void* y, const void* weight, co
   return B200C_OK;
 }
 
+// A batch norm followed by a residual add, with or without stochastic depth (norm_res.cuh): the local site's checks,
+// at most kMaxChannels channels, noise only with an identity (forward) and rows_per_sample >= 1 dividing m with noise.
+static int check_res(const char* site, int m, int c, const void* identity, const void* noise, int rows_per_sample) {
+  if (c > bn::kMaxChannels) return fail(B200C_EINVAL, "%s: channels=%d above %d", site, c, bn::kMaxChannels);
+  if (noise && !identity) return fail(B200C_EINVAL, "%s: noise without an identity", site);
+  if (noise && (rows_per_sample < 1 || m % rows_per_sample))
+    return fail(B200C_EINVAL, "%s: rows_per_sample=%d does not divide m=%d", site, rows_per_sample, m);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_res(const void* x, const void* identity, const void* noise, int rows_per_sample, void* y,
+                                    const float* weight, const float* bias, float* running_mean, float* running_var,
+                                    int64_t* num_batches_tracked, float* save_mean, float* save_invstd, int m, int channels,
+                                    float momentum, float eps, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm res", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (!rc) rc = check_res("batch norm res", m, channels, identity, noise, rows_per_sample);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd)
+    return fail(B200C_EINVAL, "batch norm res forward: null buffer");
+  const bn::FwdArgs a{x, identity, y, nullptr, false, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  RT(bn::forward_res(a, noise, rows_per_sample, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+// The identity's gradient is dy itself, so the backward takes no identity; the noise check stands in for it.
+extern "C" int b200c_bn_backward_res(const void* dy, const void* noise, int rows_per_sample, const void* x, void* g, void* dx,
+                                     const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
+                                     float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream) {
+  int rc = check_bn("batch norm res", 1, m, channels, scratch, 1, nullptr, nullptr, nullptr);
+  if (!rc) rc = check_res("batch norm res", m, channels, noise, noise, rows_per_sample);
+  if (rc) return rc;
+  if (!dy || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias || (noise && !g))
+    return fail(B200C_EINVAL, "batch norm res backward: null buffer");
+  if (g && !noise) return fail(B200C_EINVAL, "batch norm res backward: g without noise (g is dy)");
+  const bn::BwdArgs a{dy, nullptr, nullptr, nullptr, x, g, dx, false, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                      m, channels, scratch};
+  RT(bn::backward_res(a, noise, rows_per_sample, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_res(const void* x, const void* identity, void* y, const void* weight, const void* bias,
+                                  const void* running_mean, const void* running_var, int param_bf16, float eps, int m, int channels,
+                                  b200c_stream_t stream) {
+  int rc = check_infer("batch norm infer res", param_bf16, m, channels);
+  if (!rc) rc = check_res("batch norm infer res", m, channels, identity, nullptr, 0);
+  if (rc) return rc;
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer res: null buffer");
+  RT(bn::infer_res({x, identity, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0},
+                   (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
 extern "C" int b200c_broadcast(b200c_comm_t* c, void* buf, size_t count, int dtype, int root, b200c_stream_t stream) {
   int rc = check_ready(c);
   if (rc) return rc;

@@ -1,5 +1,5 @@
-// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh); argument checking lives
-// in b200coll.cu.
+// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh); argument
+// checking lives in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
@@ -8,6 +8,7 @@
 #include "norm_infer.cuh"
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
+#include "norm_res.cuh"
 
 namespace b200c {
 namespace bn {
@@ -200,6 +201,28 @@ static ActInferKernel<P> act_infer_kernel(int vec, int act) {
   });
 }
 
+// the kernels of a batch norm followed by a residual add, with or without stochastic depth (norm_res.cuh)
+using bn_res::Res;
+using ResTransformKernel = void (*)(const bf16*, const bf16*, const bf16*, bf16*, const float*, const float*, const float*, const float*,
+                                    int, int, int);
+using ResBwdReduceKernel = void (*)(const bf16*, const bf16*, const bf16*, const float*, const float*, float*, float*, float*, float*,
+                                    volatile float*, int*, bf16*, int, int, int);
+template <typename P>
+using ResInferKernel = void (*)(const bf16*, const bf16*, bf16*, const P*, const P*, const P*, const P*, float, int, int);
+
+static ResTransformKernel res_transform_kernel(int vec, bool drop) {
+  return with_const<1, kEwVec>(vec, [&](auto v) -> ResTransformKernel {
+    return drop ? bn_res::k_res_transform<decltype(v)::value, bn_res::kResDropAdd> : bn_res::k_res_transform<decltype(v)::value, bn_res::kResAdd>;
+  });
+}
+static ResBwdReduceKernel res_bwd_reduce_kernel() { return bn_res::k_res_bwd_reduce; }
+template <typename P>
+static ResInferKernel<P> res_infer_kernel(int vec, bool add) {
+  return with_const<1, kEwVec>(vec, [&](auto v) -> ResInferKernel<P> {
+    return add ? bn_res::k_res_infer<decltype(v)::value, bn_res::kResAdd, P> : bn_res::k_res_infer<decltype(v)::value, bn_res::kResPlain, P>;
+  });
+}
+
 // Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
 // load a kernel lazily while a peer's collective waits): every key value goes through the functions above.
 cudaError_t load_kernels() {
@@ -207,6 +230,7 @@ cudaError_t load_kernels() {
   cudaError_t e = cudaSuccess;
   auto load = [&](auto kernel) { if (kernel && e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel); };
   load(&k_bn_sync_merge);
+  load(res_bwd_reduce_kernel());
   for (int src = 0; src < kGradSrcs; src++) {
     load(bwd_reduce_kernel(src, false));
     load(bwd_reduce_kernel(src, true));
@@ -231,6 +255,11 @@ cudaError_t load_kernels() {
       load(act_transform_kernel(vec, act));
       load(act_infer_kernel<float>(vec, act));
       load(act_infer_kernel<bf16>(vec, act));
+    }
+    for (bool b : {false, true}) {
+      load(res_transform_kernel(vec, b));
+      load(res_infer_kernel<float>(vec, b));
+      load(res_infer_kernel<bf16>(vec, b));
     }
   }
   return e;
@@ -446,6 +475,22 @@ static cudaError_t launch_infer(const InferArgs& a, cudaStream_t st) {
 
 cudaError_t infer(const InferArgs& a, cudaStream_t st) { return a.param_bf16 ? launch_infer<bf16>(a, st) : launch_infer<float>(a, st); }
 
+// dx of a local site from a g that is already in memory (the one a reduce kernel wrote, or dy itself where g = dy):
+// k_bn_bwd_elemt reads it as kGradMasked, with this call's norm_fct = (float)(1.0 / m).
+static cudaError_t launch_elemt_of(const BwdArgs& a, const bf16* g, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  const void* ptrs[3] = {a.x, a.dx, g};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const BwdElemtKernel ke = bwd_elemt_kernel(vec, kGradMasked, false, false);
+  if (!ke) return kNoKernel;
+  ke<<<grid, block, 0, st>>>(g, nullptr, nullptr, nullptr, static_cast<const bf16*>(a.x), static_cast<bf16*>(a.dx), a.save_mean,
+                             a.save_invstd, a.weight, s.sums, s.sums + a.c, nullptr, (float)(1.0 / a.m), nullptr, nullptr, nullptr,
+                             nullptr, nullptr, nullptr, a.m, a.c);
+  return cudaGetLastError();
+}
+
 // ---- batch norm followed by ReLU6, SiLU or Hardswish ----
 // The statistics are the local site's (k_bn_stats); the transform, like k_bn_transform, then writes act(t).
 cudaError_t forward_act(const FwdArgs& a, int act, cudaStream_t st) {
@@ -475,14 +520,7 @@ cudaError_t backward_act(const BwdArgs& a, const float* bias, int act, cudaStrea
                              a.grad_weight, a.grad_bias, s.staging, s.semaphores, g, a.m, a.c);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  const void* ptrs[3] = {a.x, a.dx, g};
-  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
-  ew_config(a.m, a.c, vec, &block, &grid);
-  const BwdElemtKernel ke = bwd_elemt_kernel(vec, kGradMasked, false, false);
-  if (!ke) return kNoKernel;
-  ke<<<grid, block, 0, st>>>(g, nullptr, nullptr, nullptr, x, static_cast<bf16*>(a.dx), a.save_mean, a.save_invstd, a.weight, s.sums,
-                             s.sums + a.c, nullptr, (float)(1.0 / a.m), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.m, a.c);
-  return cudaGetLastError();
+  return launch_elemt_of(a, g, st);
 }
 
 template <typename P>
@@ -503,6 +541,59 @@ static cudaError_t launch_infer_act(const InferArgs& a, int act, cudaStream_t st
 cudaError_t infer_act(const InferArgs& a, int act, cudaStream_t st) {
   return a.param_bf16 ? launch_infer_act<bf16>(a, act, st) : launch_infer_act<float>(a, act, st);
 }
+
+// ---- batch norm followed by a residual add, with or without stochastic depth ----
+// The statistics are the local site's (k_bn_stats).  Without an identity the transform is k_bn_transform<V, kTailNone>.
+cudaError_t forward_res(const FwdArgs& a, const void* noise, int rows_per_sample, cudaStream_t st) {
+  if (!a.identity) return forward(a, st);
+  const cudaError_t e = launch_stats(a, nullptr, st);
+  if (e != cudaSuccess) return e;
+  const void* ptrs[3] = {a.x, a.y, a.identity};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const ResTransformKernel k = res_transform_kernel(vec, noise != nullptr);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.identity), static_cast<const bf16*>(noise),
+                            static_cast<bf16*>(a.y), a.save_mean, a.save_invstd, a.weight, a.bias, rows_per_sample, a.m, a.c);
+  return cudaGetLastError();
+}
+
+// Without noise g = dy: k_bn_bwd_reduce<kGradDy, false> sums dy, and the elementwise kernel reads dy as its g.  With
+// noise the reduce derives g = bf16(dy * noise[n]) and writes it to a.dy_masked for the elementwise kernel.
+cudaError_t backward_res(const BwdArgs& a, const void* noise, int rows_per_sample, cudaStream_t st) {
+  if (!noise) {
+    const cudaError_t e = launch_bwd_reduce(a, st);
+    return e == cudaSuccess ? launch_elemt_of(a, static_cast<const bf16*>(a.dy), st) : e;
+  }
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const ResBwdReduceKernel kr = res_bwd_reduce_kernel();
+  bf16* g = static_cast<bf16*>(a.dy_masked);
+  kr<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(noise), a.save_mean,
+                             a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, g, rows_per_sample,
+                             a.m, a.c);
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? launch_elemt_of(a, g, st) : e;
+}
+
+template <typename P>
+static cudaError_t launch_infer_res(const InferArgs& a, cudaStream_t st) {
+  const void* ptrs[3] = {a.x, a.y, a.identity ? a.identity : a.x};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const ResInferKernel<P> k = res_infer_kernel<P>(vec, a.identity != nullptr);
+  if (!k) return kNoKernel;
+  const InferParams& b = a.bn;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.identity), static_cast<bf16*>(a.y),
+                            static_cast<const P*>(b.running_mean), static_cast<const P*>(b.running_var), static_cast<const P*>(b.weight),
+                            static_cast<const P*>(b.bias), b.eps, a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_res(const InferArgs& a, cudaStream_t st) { return a.param_bf16 ? launch_infer_res<bf16>(a, st) : launch_infer_res<float>(a, st); }
 
 // ---- sync batch norm ----
 // The sync scratch is the local one followed, from a 16-byte boundary, by W + 1 rows of [mean | invstd | count]:

@@ -114,5 +114,14 @@ cudaError_t forward_act(const FwdArgs& a, int act, cudaStream_t s);
 cudaError_t backward_act(const BwdArgs& a, const float* bias, int act, cudaStream_t s);
 cudaError_t infer_act(const InferArgs& a, int act, cudaStream_t s);
 
+// Batch norm followed by a residual add, with or without stochastic depth (norm_res.cuh).  A local training site: the
+// forward reads FwdArgs without mask or stem (relu false), an optional identity and, with it, optional bf16 noise of
+// one value per rows_per_sample rows (2 kernels); the backward reads BwdArgs.dy / x / dx / weight, the statistics,
+// sums and scratch, and with noise writes g = bf16(dy * noise) to BwdArgs.dy_masked (2 kernels).  The eval site reads
+// InferArgs without downsample or stem (1 kernel).
+cudaError_t forward_res(const FwdArgs& a, const void* noise, int rows_per_sample, cudaStream_t s);
+cudaError_t backward_res(const BwdArgs& a, const void* noise, int rows_per_sample, cudaStream_t s);
+cudaError_t infer_res(const InferArgs& a, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

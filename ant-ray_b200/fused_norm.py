@@ -1,5 +1,5 @@
 """Fused batch norm for the training step and eval forward of ResNets and of torchvision's Conv2dNormActivation blocks
-(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh).
+(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
 by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
@@ -33,6 +33,13 @@ activation run as one site per direction (`bn_act`, norm_act.cuh): the forward w
 bits, and the backward recomputes bn(x) from x instead of saving it.  `bn_act` runs nn.ReLU on the ReLU sites above.  The
 conditions are those above, with no hook on the batch norm or the activation; in eval without autograd recording the
 site is one launch.  A sync site with one of those activations runs the sync batch norm alone, then the activation.
+
+Inverted-residual blocks: `fuse_model` also swaps torchvision's MobileNetV2 / V3 `InvertedResidual` and
+EfficientNet's `MBConv` for subclasses whose projection batch norm (the 1x1 convolution's, without activation) runs
+with what follows it as one site per direction (`bn_res`, norm_res.cuh): nothing, the residual add, or EfficientNet's
+stochastic depth ("row" mode, its noise built by torchvision's own torch calls) and the add.  The conditions are those
+above, with no hook on the block's Sequential, the projection, its batch norm or the stochastic depth; in eval without
+autograd recording the site is one launch.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -345,6 +352,64 @@ class _FusedBatchNormAct(torch.autograd.Function):
         return dx, grad_weight, grad_bias, None, None
 
 
+class _FusedBatchNormRes(torch.autograd.Function):
+    """bn(x), bn(x) + identity or, with `noise`, bf16(bn(x) * noise) + identity in training mode: the projection batch
+    norm of an inverted-residual block, and the stochastic depth (`noise`, torchvision's [N, 1, 1, 1] bf16 "row" noise)
+    and residual add after it.  Only the sum is written.  The identity's gradient is dy itself; with noise the backward
+    writes stochastic depth's g = bf16(dy * noise) for the batch norm's elementwise backward.
+
+    A gradient that arrives in another layout than channels-last makes eager torch's mul write g in that layout and its
+    batch-norm backward run its NCHW kernels; there the backward runs those torch ops, as _FusedBatchNormAct does."""
+
+    @staticmethod
+    def forward(ctx, x, identity, weight, bias, bn, noise):
+        lib = _native_lib()
+        c = x.shape[1]
+        m = x.numel() // c
+        y = torch.empty_like(x)
+        nbt = bn.num_batches_tracked
+        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_forward_res(x.data_ptr(), identity.data_ptr() if identity is not None else None,
+                                         noise.data_ptr() if noise is not None else None, x.shape[2] * x.shape[3], y.data_ptr(),
+                                         weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                         nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, m, c, bn.momentum, bn.eps,
+                                         _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        ctx.residual, ctx.eps = identity is not None, bn.eps
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, weight, stats, noise)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None, None, None, None
+        x, weight, stats, noise = ctx.saved_tensors
+        c = x.shape[1]
+        m = x.numel() // c
+        d_identity = dy if ctx.residual else None
+        if not dy.is_contiguous(memory_format=torch.channels_last):
+            g = dy * noise if noise is not None else dy
+            # the running statistics are not read in training mode
+            dx, grad_weight, grad_bias = torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, stats[:c], stats[c:], True,
+                                                                                   ctx.eps, [True, True, True])
+            return dx, d_identity, grad_weight, grad_bias, None, None
+        lib = _native_lib()
+        dx = torch.empty_like(x)
+        g = torch.empty_like(x) if noise is not None else None
+        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
+        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        mean = stats.data_ptr()
+        stream = _raw_stream(x.device.index)
+        N.check(lib.b200c_bn_backward_res(dy.data_ptr(), noise.data_ptr() if noise is not None else None, x.shape[2] * x.shape[3],
+                                          x.data_ptr(), g.data_ptr() if g is not None else None, dx.data_ptr(), weight.data_ptr(), mean,
+                                          mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c,
+                                          _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        return dx, d_identity, grad_weight, grad_bias, None, None
+
+
 def _activation(t):
     # With one channel, NCHW strides also pass the channels-last check, but torch runs its NCHW statistics kernel
     # unless stride(1) == 1 (batch_norm_choose_impl), so the channel stride must be 1 as well.
@@ -491,6 +556,34 @@ def bn_act(bn, act, x):
     if _sync_comm(bn, x) is None and _local_ok(bn, x):
         return _FusedBatchNormAct.apply(x, bn.weight, bn.bias, bn, code)
     return act(bn(x))
+
+
+def _noise_ok(noise, x):
+    """Whether `noise` is stochastic depth's "row" noise for `x` as the kernels read it: bf16 [N, 1, 1, 1] on x's device."""
+    return (noise.dtype == torch.bfloat16 and noise.device == x.device and noise.shape == (x.shape[0], 1, 1, 1)
+            and noise.is_contiguous() and not noise.requires_grad)
+
+
+def bn_res(bn, x, identity=None, noise=None):
+    """`bn(x)`, `bn(x) + identity`, or with `noise` (torchvision's stochastic depth noise in "row" mode, [N, 1, 1, 1])
+    `bn(x) * noise + identity`, with eager torch's bits, fused when the site allows it: an eval site (no noise) in one
+    launch, else a local training site, with the conditions of bn_relu's and no hook on `bn`.  Noise needs an identity.
+    Anything else runs the modules' ops."""
+    operands = () if identity is None else (identity,)
+    site = (not _hooked(bn) and not _global_hooks() and (noise is None or (identity is not None and _noise_ok(noise, x)))
+            and all(_activation(t) and t.shape == x.shape and t.device == x.device for t in operands))
+    if site and noise is None and _infer_bn_ok(bn, x, *operands):
+        y = torch.empty_like(x)
+        c = x.shape[1]
+        N.check(_native_lib().b200c_bn_infer_res(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
+                                                 *_infer_params(bn), bn.eps, x.numel() // c, c, _raw_stream(x.device.index)))
+        return y
+    if site and _sync_comm(bn, x) is None and _local_ok(bn, x):
+        return _FusedBatchNormRes.apply(x, identity, bn.weight, bn.bias, bn, noise)
+    out = bn(x)
+    if noise is not None:
+        out = out * noise
+    return out if identity is None else out + identity
 
 
 def _pool_fusable(pool):
@@ -702,12 +795,96 @@ else:
                 return super().forward(x)
             return bn_act(bn, act, conv(x))
 
+
+def _row_noise(sd, t):
+    """torchvision's stochastic_depth(t, sd.p, "row", sd.training) noise, built by the same torch calls in the same
+    order (so the RNG stream and the bits are torch's), or None where it returns t unchanged (eval, p == 0)."""
+    if not sd.training or sd.p == 0.0:
+        return None
+    survival_rate = 1.0 - sd.p
+    noise = torch.empty([t.shape[0]] + [1] * (t.ndim - 1), dtype=t.dtype, device=t.device)
+    noise = noise.bernoulli_(survival_rate)
+    if survival_rate > 0.0:
+        noise.div_(survival_rate)
+    return noise
+
+
+def _res_forward(block, seq, nested, x, identity, sd=None):
+    """The inverted-residual block's forward with its projection batch norm as one bn_res site: every module of `seq`
+    before the projection, then the projection's convolution as a module, then bn_res with `identity` (None without a
+    residual connection) and stochastic depth `sd`'s noise.  The projection is `seq`'s last two modules, or with
+    `nested` the two of its last module, a Conv2dNormActivation without activation.
+
+    None where the block must run its parent's forward: eval with gradients recorded, a projection other than exactly
+    nn.Conv2d then nn.BatchNorm2d (a SyncBatchNorm stays with FusedSyncBatchNorm), stochastic depth other than
+    torchvision's in "row" mode with 0 <= p <= 1, or a hook that calling the modules one by one would skip (on `seq`,
+    the projection's Conv2dNormActivation, the batch norm, `sd`, or a global one)."""
+    if (not block.training and torch.is_grad_enabled()) or type(seq) is not nn.Sequential or len(seq) < 2:
+        return None
+    if nested:
+        last = seq[-1]
+        if type(last) is not Conv2dNormActivation or len(last) != 2 or _hooked(last):
+            return None
+        head, conv, bn = list(seq)[:-1], last[0], last[1]
+    else:
+        head, conv, bn = list(seq)[:-2], seq[-2], seq[-1]
+    if type(conv) is not nn.Conv2d or type(bn) is not nn.BatchNorm2d or _hooked(seq) or _hooked(bn) or _global_hooks():
+        return None
+    if sd is not None and (type(sd) is not StochasticDepth or sd.mode != "row" or not 0.0 <= sd.p <= 1.0 or _hooked(sd)):
+        return None
+    out = x
+    for mod in head:
+        out = mod(out)
+    out = conv(out)
+    noise = _row_noise(sd, out) if sd is not None and identity is not None else None
+    return bn_res(bn, out, identity, noise)
+
+
+try:
+    from torchvision.models import efficientnet, mobilenetv2, mobilenetv3
+    from torchvision.ops import StochasticDepth
+except ImportError:  # without torchvision there is nothing to rewrite
+    _RES_SWAP = {}
+else:
+
+    # The projection of these blocks ends in an nn.Conv2d and a batch norm without activation: MobileNetV2's last two
+    # modules of `conv`, MobileNetV3's and EfficientNet's last Conv2dNormActivation of `block` (activation_layer None).
+
+    class FusedInvertedResidualV2(mobilenetv2.InvertedResidual):
+        """MobileNetV2's block, `x + conv(x)` or `conv(x)`, whose projection batch norm and residual add are one bn_res site."""
+
+        def forward(self, x):
+            out = _res_forward(self, self.conv, False, x, x if self.use_res_connect else None)
+            return super().forward(x) if out is None else out
+
+    class FusedInvertedResidualV3(mobilenetv3.InvertedResidual):
+        """MobileNetV3's block, `block(x)` then `+= x`, whose projection batch norm and residual add are one bn_res site."""
+
+        def forward(self, input):
+            out = _res_forward(self, self.block, True, input, input if self.use_res_connect else None)
+            return super().forward(input) if out is None else out
+
+    class FusedMBConv(efficientnet.MBConv):
+        """EfficientNet's block, `stochastic_depth(block(x))` then `+= x`, whose projection batch norm, stochastic depth
+        and residual add are one bn_res site."""
+
+        def forward(self, input):
+            out = _res_forward(self, self.block, True, input, input if self.use_res_connect else None,
+                               self.stochastic_depth)
+            return super().forward(input) if out is None else out
+
+    _RES_SWAP = {mobilenetv2.InvertedResidual: FusedInvertedResidualV2, mobilenetv3.InvertedResidual: FusedInvertedResidualV3,
+                 efficientnet.MBConv: FusedMBConv}
+
+
 def fuse_model(model):
     """Rewrite `model` in place: `fuse_resnet`, and every module whose class is exactly torchvision's
     Conv2dNormActivation and whose last module is an nn.ReLU6, SiLU or Hardswish (MobileNetV2 / V3, EfficientNet)
-    becomes a FusedConv2dNormActivation.  Parameters, buffers, state_dict keys, hooks and the object itself are
-    unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in training and in eval
-    (see `fuse_resnet` for inference).
+    becomes a FusedConv2dNormActivation.  Every module whose class is exactly torchvision's MobileNetV2 or MobileNetV3
+    InvertedResidual or EfficientNet's MBConv gets the fused subclass, whose projection batch norm (with the stochastic
+    depth and residual add after it) runs as one bn_res site.  Parameters, buffers, state_dict keys, hooks and the
+    object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
+    training and in eval (see `fuse_resnet` for inference).
 
     Blocks ending in nn.ReLU (MobileNetV3, RegNet) keep torchvision's forward: bn_act would run them on bn_relu's sites,
     but a regnet_y_400mf training step with them fused took about 11 ms more host time than the untouched model (DESIGN.md
@@ -717,6 +894,10 @@ def fuse_model(model):
         for mod in model.modules():
             if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
                 mod.__class__ = FusedConv2dNormActivation
+    for mod in model.modules():
+        cls = _RES_SWAP.get(type(mod))
+        if cls is not None:
+            mod.__class__ = cls
     return model
 
 

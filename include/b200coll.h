@@ -406,6 +406,31 @@ int b200c_bn_backward_act(const void* dy, const void* x, void* g, void* dx, cons
 int b200c_bn_infer_act(const void* x, void* y, const void* weight, const void* bias, const void* running_mean, const void* running_var,
                        int param_bf16, float eps, int act, int m, int channels, b200c_stream_t stream);
 
+/* ---- fused batch norm followed by a residual add, with or without stochastic depth (inverted-residual blocks) ----
+ * y = bn(x), y = bn(x) + identity or y = stochastic_depth(bn(x)) + identity over channels-last bf16 activations,
+ * bit-identical to eager torch: the batch norm's output t is rounded to bf16; stochastic depth multiplies it by
+ * noise[n] (bf16, one value per sample n = row / rows_per_sample, as torchvision's "row" mode builds it) and rounds to
+ * bf16; the add sums in fp32 and rounds to bf16.  `identity` may be null (no add); `noise` may be null (no stochastic
+ * depth) and needs an identity and a rows_per_sample >= 1 that divides m.  Channels 1..131072, m >= 1 rows, fewer than
+ * 2^31 elements; every argument is checked before the first launch.
+ *
+ * b200c_bn_forward_res: the training forward of b200c_bn_forward (statistics, running statistics,
+ * num_batches_tracked, scratch of b200c_bn_scratch_bytes(channels)) without ReLU.  2 kernels.
+ * b200c_bn_backward_res: from dy (the gradient of y), x, weight and the saved statistics, writes dx, grad_weight and
+ * grad_bias.  The identity's gradient is dy itself.  With noise, g = bf16(dy * noise[n]) (stochastic depth's backward)
+ * is written to `g` (m rows, required then, null otherwise), which the batch norm's elementwise backward reads.
+ * 2 kernels.
+ * b200c_bn_infer_res: the eval site, y = bf16(bn(x)) or bf16(bf16(bn(x)) + identity) (stochastic depth is the
+ * identity in eval), with weight, bias and running statistics of fp32, or of bf16 with param_bf16.  1 kernel. */
+int b200c_bn_forward_res(const void* x, const void* identity, const void* noise, int rows_per_sample, void* y, const float* weight,
+                         const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                         float* save_invstd, int m, int channels, float momentum, float eps, void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_res(const void* dy, const void* noise, int rows_per_sample, const void* x, void* g, void* dx, const float* weight,
+                          const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m, int channels,
+                          void* scratch, b200c_stream_t stream);
+int b200c_bn_infer_res(const void* x, const void* identity, void* y, const void* weight, const void* bias, const void* running_mean,
+                       const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
+
 /* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
  * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
  * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)

@@ -1,19 +1,22 @@
 #!/usr/bin/env python
 """Training step and eval forward of torchvision CNNs whose batch norms sit in Conv2dNormActivation blocks
 (mobilenet_v2, mobilenet_v3_large, efficientnet_b0, regnet_y_400mf), with and without `fused_norm.fuse_model`.
+The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model) and "act_only" (fuse_model without the
+inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused).
 
 Batch `--batch` (256) at 224 x 224, bf16 autocast with fp32 parameters, channels-last, SGD with momentum.  Per model,
-alternating the two builds ("fused", "unfused") in one process, `--runs` times each, the order swapped every run:
+alternating the builds in one process, `--runs` times each, the order reversed every run (ABBA):
   train_images_per_sec   `--iters` training steps between device events, after `--warmup` steps
   eval_images_per_sec    `--iters` forwards under inference_mode, the same way
-Both builds start from the same weights and train on the same batches, reseeded per step, so after the timed runs
-their parameters and eval logits must have identical bits ("identical").  Then the host's time per training step
+All builds start from the same weights and train on the same batches, reseeded per step, so after the timed runs
+their parameters and eval logits must have identical bits ("identical", each build against the first).  Then the host's time per training step
 (forward and backward, no optimizer step): the wall time per step at batch `--host-batch` (4), where the GPU work is
 too small to set the pace.  Then, in a separate profiled run per build, the kernel time per step by family.
 
 Writes OUT/cnn_step.json; prints the summary.  The card's name and power limit are read in the same run.
 
-  python tools/cnn_step.py --out DIR [--models a,b] [--batch 256] [--runs 4] [--iters 10] [--warmup 3] [--host-batch 4]
+  python tools/cnn_step.py --out DIR [--models a,b] [--builds fused,unfused] [--batch 256] [--runs 4] [--iters 10]
+                           [--warmup 3] [--host-batch 4]
 """
 import argparse
 import copy
@@ -34,9 +37,11 @@ MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "regnet_y_400
 # first match wins
 FAMILIES = [
     ("bn_stats", r"k_bn_stats|batch_norm_collect_statistics"),
-    ("bn_transform_act", r"k_act_transform|k_act_infer|k_bn_transform|k_infer_transform|batch_norm_transform_input"),
-    ("bn_bwd_reduce", r"k_act_bwd_reduce|k_bn_bwd_reduce|batch_norm_backward_reduce"),
+    ("bn_transform_act", r"k_act_transform|k_act_infer|k_res_transform|k_res_infer|k_bn_transform|k_infer_transform"
+                         r"|batch_norm_transform_input"),
+    ("bn_bwd_reduce", r"k_act_bwd_reduce|k_res_bwd_reduce|k_bn_bwd_reduce|batch_norm_backward_reduce"),
     ("bn_bwd_elemt", r"k_act_bwd_elemt|k_bn_bwd_elemt|batch_norm_backward_elemt"),
+    ("torch_add_mul", r"CUDAFunctor_add|MulFunctor|bernoulli"),
     ("torch_act", r"silu|hardswish|hardsigmoid|clamp|hardtanh|threshold|relu"),
     ("conv", r"conv|cudnn|xmma|gemm|nvjet|cutlass|fprop|dgrad|wgrad|implicit_|nhwc|nchw|sm90_"),
 ]
@@ -53,6 +58,7 @@ def main():
     p = argparse.ArgumentParser()
     p.add_argument("--out", required=True)
     p.add_argument("--models", default=",".join(MODELS))
+    p.add_argument("--builds", default="fused,unfused")
     p.add_argument("--batch", type=int, default=256)
     p.add_argument("--runs", type=int, default=4)
     p.add_argument("--iters", type=int, default=10)
@@ -80,7 +86,18 @@ def main():
     for arch in args.models.split(","):
         torch.manual_seed(0)
         base = getattr(torchvision.models, arch)(weights=None).to(device).to(memory_format=torch.channels_last)
-        models = {"fused": fused_norm.fuse_model(copy.deepcopy(base)), "unfused": base}
+        builds = args.builds.split(",")
+        models = {}
+        for b in builds:
+            m = copy.deepcopy(base)
+            if b in ("fused", "act_only"):
+                fused_norm.fuse_model(m)
+            if b == "act_only":   # the projection sites' blocks back to torchvision's classes
+                parents = {cls: parent for parent, cls in fused_norm._RES_SWAP.items()}
+                for mod in m.modules():
+                    if type(mod) in parents:
+                        mod.__class__ = parents[type(mod)]
+            models[b] = m
         opts = {b: torch.optim.SGD(m.parameters(), lr=0.01, momentum=0.9) for b, m in models.items()}
         steps = {b: 0 for b in models}
 
@@ -111,18 +128,19 @@ def main():
 
         res = {b: {"train_images_per_sec": [], "eval_images_per_sec": []} for b in models}
         for r in range(args.runs):
-            for b in (["fused", "unfused"] if r % 2 == 0 else ["unfused", "fused"]):   # alternating builds, ABBA
+            for b in (builds if r % 2 == 0 else builds[::-1]):   # alternating builds, ABBA
                 models[b].train()
                 res[b]["train_images_per_sec"].append(timed(b, train_step))
                 models[b].eval()
                 res[b]["eval_images_per_sec"].append(timed(b, forward))
         ints = {2: torch.int16, 4: torch.int32}
         same = lambda a, c: a.dtype == c.dtype and bool(torch.equal(a.view(ints[a.element_size()]), c.view(ints[c.element_size()])))  # noqa: E731
-        entry = {"builds": res, "act_sites": len([m for m in models["fused"].modules() if type(m) is fused_norm.FusedConv2dNormActivation and len(m) == 3]),
-                 "identical": {"parameters": all(same(a, c) for a, c in zip(models["fused"].parameters(), models["unfused"].parameters())),
-                               "buffers": all(same(a, c) for a, c in zip(models["fused"].buffers(), models["unfused"].buffers())
-                                              if a.is_floating_point()),
-                               "eval_logits": same(forward("fused"), forward("unfused"))}}
+        first = models[builds[0]]
+        entry = {"builds": res, "act_sites": len([m for m in first.modules() if type(m) is fused_norm.FusedConv2dNormActivation and len(m) == 3]),
+                 "res_sites": len([m for m in first.modules() if type(m) in fused_norm._RES_SWAP.values()]),
+                 "identical": {b: {"parameters": all(same(a, c) for a, c in zip(models[b].parameters(), first.parameters())),
+                                   "buffers": all(same(a, c) for a, c in zip(models[b].buffers(), first.buffers()) if a.is_floating_point()),
+                                   "eval_logits": same(forward(b), forward(builds[0]))} for b in builds[1:]}}
         # host time: at batch `--host-batch` the GPU work is small, so a step's wall time is what the host needs to issue it
         xs, ys = x[:args.host_batch].clone(), y[:args.host_batch].clone()
 
@@ -135,7 +153,7 @@ def main():
 
         host = {b: [] for b in models}
         for r in range(args.runs):
-            for b in (["fused", "unfused"] if r % 2 == 0 else ["unfused", "fused"]):
+            for b in (builds if r % 2 == 0 else builds[::-1]):
                 models[b].train()
                 for _ in range(args.warmup):
                     host_step(b)

@@ -47,6 +47,44 @@ static bool vec_ok(int stride, const void* const* ptrs, int n) {
   return true;
 }
 
+// The vector paths' rings (norm_kernels.cuh) live in dynamic shared memory and, with each kernel's static shared
+// memory, stay within the 48 KB a block may use without an opt-in attribute, so no launch depends on one being set.
+constexpr size_t kBlockSmem = 48 * 1024;
+constexpr size_t kStatsStaticSmem = 3 * kMaxBlock * 4 + 16;   // bn_stats_body's tree and last-block flag
+constexpr size_t kBwdStaticSmem = 2 * kMaxBlock * 4 + 16;     // k_bn_bwd_reduce's tree and last-block flag
+
+// The statistics ring: kStatsStages iterations of kParallelLoads rows of kStatsVec channels per hardware thread.
+static size_t stats_ring_bytes(dim3 block) {
+  return (size_t)kStatsStages * kParallelLoads * block.x * block.y * sizeof(BVec<kStatsVec>);
+}
+static_assert(kStatsStaticSmem + (size_t)kStatsStages * kParallelLoads * (kMaxBlock / kStatsVec) * sizeof(BVec<kStatsVec>) <= kBlockSmem,
+              "the statistics ring fits every block");
+
+// The backward reduce runs kBwdVec channels per hardware thread with a ring when the rows allow it (C % 8 == 0 and
+// every operand it copies or writes on the 16-byte grid, as vec_ok decides for the elementwise kernels); otherwise
+// one channel per thread with the register walk.  The logical block is reduce_config's.
+static_assert(kBwdStaticSmem + (size_t)kBwdStagesWide * 5 * kParallelLoads * (kMaxBlock / kBwdVec) * sizeof(BVec<kBwdVec>) <= kBlockSmem &&
+                  kBwdStaticSmem + (size_t)kBwdStages * 2 * kParallelLoads * (kMaxBlock / kBwdVec) * sizeof(BVec<kBwdVec>) <= kBlockSmem,
+              "the backward ring fits every block: 2 stages of up to 5 operands, 3 of 2");
+struct BwdReduceLaunch {
+  dim3 block, grid;
+  int vec;
+  size_t smem;
+};
+static BwdReduceLaunch bwd_reduce_launch(int m, int c, GradSrc src, bool dy2, bool dual, const void* const* ptrs, int n) {
+  BwdReduceLaunch l;
+  reduce_config(m, c, &l.block, &l.grid);
+  l.vec = 1;
+  l.smem = 0;
+  if (src == kGradPool || !vec_ok(c, ptrs, n)) return l;
+  const int ops = bwd_ring_operands(src == kGradY, dy2, dual);
+  const size_t ring = (size_t)bwd_ring_stages(ops) * ops * kParallelLoads * (l.block.x / kBwdVec) * l.block.y * sizeof(BVec<kBwdVec>);
+  l.block.x /= kBwdVec;
+  l.vec = kBwdVec;
+  l.smem = ring;
+  return l;
+}
+
 // Elementwise kernels: `rows` rows per block, and enough blocks for a few waves on the GPU (each thread then
 // strides over the rows).
 static void ew_config(int reduction, int stride, int vec, dim3* block, dim3* grid) {
@@ -105,7 +143,7 @@ using TransformKernel = void (*)(const bf16*, const bf16*, bf16*, uint8_t*, cons
 using PoolFwdKernel = void (*)(const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*, PoolDims, int, int);
 using BwdReduceKernel = void (*)(const bf16*, const bf16*, const bf16*, const bf16*, const uint8_t*, bf16*, const float*, const float*,
                                  float*, float*, float*, float*, volatile float*, int*, PoolDims, const bf16*, const float*, const float*,
-                                 float*, float*, float*, int, int);
+                                 float*, float*, float*, int, int, int);
 using BwdElemtKernel = void (*)(const bf16*, const bf16*, const bf16*, const uint8_t*, const bf16*, bf16*, const float*, const float*,
                                 const float*, const float*, const float*, const float*, float, const bf16*, bf16*, const float*,
                                 const float*, const float*, const float*, int, int);
@@ -277,17 +315,18 @@ static cudaError_t launch_stats(const FwdArgs& a, float* sync_row, cudaStream_t 
   reduce_config(a.m, a.c, &block, &grid);
   const int vec = vec_ok(a.c, &a.x, 1) ? kStatsVec : 1;
   block.x /= vec;
+  const size_t smem = vec == kStatsVec ? stats_ring_bytes(block) : 0;
   const bf16* x = static_cast<const bf16*>(a.x);
   if (sync_row) {
     const SyncStatsKernel k = sync_stats_kernel(vec);
     if (!k) return kNoKernel;
-    k<<<grid, block, 0, st>>>(x, sync_row, a.eps, s.staging, s.semaphores, a.m, a.c);
+    k<<<grid, block, smem, st>>>(x, sync_row, a.eps, s.staging, s.semaphores, a.m, a.c);
   } else {
     const StatsKernel k = stats_kernel(vec);
     if (!k) return kNoKernel;
     StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
                (float)((double)a.m / (double)(a.m - 1)), a.eps};
-    k<<<grid, block, 0, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
+    k<<<grid, block, smem, st>>>(x, o, s.staging, s.semaphores, a.m, a.c);
   }
   return cudaGetLastError();
 }
@@ -339,16 +378,16 @@ static GradSrc grad_src(const BwdArgs& a, bool reduced) {
 
 static cudaError_t launch_bwd_reduce(const BwdArgs& a, cudaStream_t st) {
   Scratch s = carve(a.scratch, a.c);
-  dim3 block, grid;
-  reduce_config(a.m, a.c, &block, &grid);
   const GradSrc src = grad_src(a, false);
+  const void* ptrs[5] = {a.x, a.dy, a.dy2 ? a.dy2 : a.dy, src == kGradY ? a.y : a.dy, a.dy_masked ? a.dy_masked : a.dy};
+  const BwdReduceLaunch l = bwd_reduce_launch(a.m, a.c, src, a.dy2 != nullptr, false, ptrs, 5);
   const BwdReduceKernel k = bwd_reduce_kernel(src, false);
   if (!k) return kNoKernel;
   const void* mask = src == kGradPool ? a.argmax : a.mask;
-  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
+  k<<<l.grid, l.block, l.smem, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
                             static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(mask), static_cast<bf16*>(a.dy_masked),
                             a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores,
-                            pool_dims(a.pool_h, a.pool_w), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.m, a.c);
+                            pool_dims(a.pool_h, a.pool_w), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.m, a.c, l.vec);
   return cudaGetLastError();
 }
 
@@ -394,13 +433,14 @@ cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
   const int svec = vec_ok(a.c, xs, 2) ? kStatsVec : 1;
   block.x /= svec;
   grid.z = 2;
+  const size_t smem = svec == kStatsVec ? stats_ring_bytes(block) : 0;
   const StatsDualKernel ks = stats_dual_kernel(svec);
   if (!ks) return kNoKernel;
   StatsOut oa{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
               (float)((double)a.m / (double)(a.m - 1)), a.eps};
   StatsOut ob{b.save_mean, b.save_invstd, b.running_mean, b.running_var, b.num_batches_tracked, b.momentum,
               (float)((double)b.m / (double)(b.m - 1)), b.eps};
-  ks<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(b.x), oa, ob, s.staging,
+  ks<<<grid, block, smem, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(b.x), oa, ob, s.staging,
                              dual_staging(a.scratch, a.c), s.semaphores, a.m, a.c);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
@@ -421,18 +461,19 @@ cudaError_t backward_dual(const BwdArgs& a, const BwdArgs& b, cudaStream_t st) {
   Scratch s = carve(a.scratch, a.c);
   float* sum2 = dual_sum_xmu2(a.scratch, a.c);
   const GradSrc src = a.mask ? kGradBits : kGradY;
-  dim3 block, grid;
-  reduce_config(a.m, a.c, &block, &grid);
+  const void* rptrs[5] = {a.x, a.dy, a.dy2 ? a.dy2 : a.dy, src == kGradY ? a.y : a.dy, b.x};
+  const BwdReduceLaunch l = bwd_reduce_launch(a.m, a.c, src, a.dy2 != nullptr, true, rptrs, 5);
   const BwdReduceKernel kr = bwd_reduce_kernel(src, true);
   if (!kr) return kNoKernel;
-  kr<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
+  kr<<<l.grid, l.block, l.smem, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), static_cast<const bf16*>(a.dy2),
                              static_cast<const bf16*>(a.y), static_cast<const uint8_t*>(a.mask), nullptr, a.save_mean, a.save_invstd,
                              s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, pool_dims(0, 0),
-                             static_cast<const bf16*>(b.x), b.save_mean, b.save_invstd, sum2, b.grad_weight, b.grad_bias, a.m, a.c);
+                             static_cast<const bf16*>(b.x), b.save_mean, b.save_invstd, sum2, b.grad_weight, b.grad_bias, a.m, a.c, l.vec);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const void* ptrs[7] = {a.x, a.dx, a.dy, a.dy2 ? a.dy2 : a.dy, b.x, b.dx, a.y};
   const int vec = vec_ok(a.c, ptrs, src == kGradY ? 7 : 6) ? kEwVec : 1;
+  dim3 block, grid;
   ew_config(a.m, a.c, vec, &block, &grid);
   const BwdElemtKernel ke = bwd_elemt_kernel(vec, src, false, true);
   if (!ke) return kNoKernel;

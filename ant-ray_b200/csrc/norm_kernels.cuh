@@ -6,14 +6,16 @@
 // and its contributors; the kernels originate in NVIDIA Apex).  They keep torch's launch shape, per-thread
 // sequence of rows, block tree and grid merge, and torch's expressions, so that every per-channel sum is rounded
 // exactly as torch rounds it.  That is what makes the outputs bit-identical to eager torch (torch 2.x runs bf16
-// batch norm on these native kernels, not on cuDNN).  Within those constraints the reducing kernels issue all loads
-// of an iteration before using any, and the statistics kernel carries 4 channels per thread.  The elementwise
+// batch norm on these native kernels, not on cuDNN).  Within those constraints the reducing kernels carry 4 channels
+// per thread where C % 8 == 0 and keep several iterations of rows in flight through per-thread cp.async rings.  The elementwise
 // kernels (transform, backward elementwise) have no cross-element rounding, so they are restructured freely: 16-byte
 // loads of 8 channels per thread.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace b200c {
 namespace bn {
@@ -26,8 +28,21 @@ constexpr int kElemsPerThread = 16;
 constexpr int kTileW = 32;
 constexpr int kMaxHBlock = 128;
 // statistics kernel: channels per hardware thread on its vector path (8-byte loads).  Measured on H100 against 1, 2
-// and 8 (DESIGN.md section 7); the backward reduce is fastest at one channel per thread, so it has no vector path.
+// and 8 (DESIGN.md section 7).
 constexpr int kStatsVec = 4;
+// backward reduce: channels per hardware thread on its vector path (8-byte copies)
+constexpr int kBwdVec = 4;
+// The vector paths' ring depth, in iterations of kParallelLoads rows, measured on H100 against 6 and 8 for the
+// statistics and 4 for the backward (DESIGN.md section 7).  A backward ring of 3 or more operands keeps 2 stages: at
+// 3 stages a tail's ring (dy, dy2, x) took 36 KB per block and ran slower than torch's register walk.  Every ring
+// and its kernel's static shared memory stay within the 48 KB a block gets without an opt-in, so every launch is
+// valid whether or not the context has set any function attribute.
+constexpr int kStatsStages = 4;
+constexpr unsigned kBwdStages = 3;       // a backward ring of dy and x
+constexpr unsigned kBwdStagesWide = 2;   // one of 3 or more operands (a tail's dy2, y, a downsample branch's x2)
+__host__ __device__ constexpr unsigned bwd_ring_stages(int ops) { return ops >= 3 ? kBwdStagesWide : kBwdStages; }
+// operands of the backward reduce's ring: dy, x, and dy2, y, x2 where the site has them
+__host__ __device__ constexpr int bwd_ring_operands(bool y, bool dy2, bool dual) { return 2 + dy2 + y + dual; }
 // elementwise kernels
 constexpr int kEwThreads = 256;
 constexpr int kEwVec = 8;
@@ -38,6 +53,24 @@ template <int V>
 struct alignas(2 * V) BVec {
   bf16 v[V];
 };
+
+// ---- the vector paths' row rings ----
+// A thread copies its own rows with cp.async into its own slots of a ring in dynamic shared memory, one commit
+// group per iteration of kParallelLoads rows, and reads back only what it copied itself: cp.async.wait_group alone
+// makes a slot visible to its thread, so the row walk has no barrier.  Slots are laid out [stage][operand][row j]
+// [thread] in words of one thread's V channels, so that consecutive threads touch consecutive words.
+__device__ __forceinline__ unsigned char* ring_smem() {
+  extern __shared__ __align__(16) unsigned char bn_ring[];
+  return bn_ring;
+}
+template <int BYTES>
+__device__ __forceinline__ void cp_async(void* smem, const void* gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem), "n"(BYTES)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 
 // ---- reduction helpers (torch's, per channel) ----
 // The statistics kernel runs V adjacent torch threads in one hardware thread: hardware thread (tx, ty) of a block
@@ -91,22 +124,39 @@ __device__ __forceinline__ void welford_merge_block_vertical(int (&count)[V], fl
   }
 }
 
-__device__ __forceinline__ void merge_block_vertical_backward(float& sum_dy, float& sum_dy_xmu, float* shmem_sum_dy,
+// torch's backward tree over threadIdx.y, with shared memory indexed by torch's thread as above
+template <int V>
+__device__ __forceinline__ void merge_block_vertical_backward(float (&sum_dy)[V], float (&sum_dy_xmu)[V], float* shmem_sum_dy,
                                                               float* shmem_sum_dy_xmu) {
-  auto address_base = threadIdx.x + threadIdx.y * blockDim.x;
+  const int block_x = blockDim.x * V;
+  auto address_base = threadIdx.x * V + threadIdx.y * block_x;
 #pragma unroll
   for (int offset = blockDim.y / 2; offset > 0; offset >>= 1) {
     if (threadIdx.y < offset * 2) {
-      shmem_sum_dy[address_base] = sum_dy;
-      shmem_sum_dy_xmu[address_base] = sum_dy_xmu;
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        shmem_sum_dy[address_base + k] = sum_dy[k];
+        shmem_sum_dy_xmu[address_base + k] = sum_dy_xmu[k];
+      }
     }
     __syncthreads();
     if (threadIdx.y < offset && threadIdx.y + offset < blockDim.y) {
-      auto address = address_base + offset * blockDim.x;
-      sum_dy += shmem_sum_dy[address];
-      sum_dy_xmu += shmem_sum_dy_xmu[address];
+      auto address = address_base + offset * block_x;
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        sum_dy[k] += shmem_sum_dy[address + k];
+        sum_dy_xmu[k] += shmem_sum_dy_xmu[address + k];
+      }
     }
   }
+}
+
+__device__ __forceinline__ void merge_block_vertical_backward(float& sum_dy, float& sum_dy_xmu, float* shmem_sum_dy,
+                                                              float* shmem_sum_dy_xmu) {
+  float a[1] = {sum_dy}, b[1] = {sum_dy_xmu};
+  merge_block_vertical_backward<1>(a, b, shmem_sum_dy, shmem_sum_dy_xmu);
+  sum_dy = a[0];
+  sum_dy_xmu = b[0];
 }
 
 struct StatsOut {
@@ -136,9 +186,10 @@ __device__ __forceinline__ void finish_stats(const StatsOut& o, int c, float mea
 // leaves its semaphore at zero for the next call.
 //
 // Each of torch's threads walks rows m_offset + r * inner_loop_stride into PARALLEL_LOADS accumulators, one
-// iteration of PARALLEL_LOADS rows at a time.  Here all rows of an iteration are loaded (V channels in one load)
-// before the first update, so that they are in flight together; torch's kernel waits for each row's value before it
-// loads the next.  The V channels of a thread share each row's validity, hence count[j] and its reciprocal.
+// iteration of PARALLEL_LOADS rows at a time.  With V = 1 all rows of an iteration are loaded before the first
+// update, so that they are in flight together; torch's kernel waits for each row's value before it loads the next.
+// With V = kStatsVec the rows come through the ring (V channels in one 8-byte copy), kStatsStages - 1 iterations
+// ahead of the updates.  The V channels of a thread share each row's validity, hence count[j] and its reciprocal.
 template <int V, typename Finish>
 __device__ __forceinline__ void bn_stats_body(const bf16* __restrict__ input, volatile float* staging_data, int* semaphores,
                                               const int reduction_size, const int stride, Finish finish) {
@@ -162,39 +213,68 @@ __device__ __forceinline__ void bn_stats_body(const bf16* __restrict__ input, vo
   int loop_count = 1 + (reduction_size - 1) / (inner_loop_stride * PARALLEL_LOADS);
   const bool c_valid = c_offset < stride;
 
-  for (int i = 0; i < loop_count; i++) {
-    // all rows of the iteration are loaded before any update uses one
-    BVec<V> xv[PARALLEL_LOADS];
+  // torch's update of accumulator j with the next row of the walk, read from *xv when the row exists
+  auto update = [&](int j, const BVec<V>* xv) {
+    float x_math[V];
+    float x_count_inv;
+    float is_valid;
+    if (c_valid && m_offset < reduction_size) {
+      const BVec<V> x = *xv;
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      const int m = m_offset + j * inner_loop_stride;
-      if (c_valid && m < reduction_size) xv[j] = *reinterpret_cast<const BVec<V>*>(input + ((size_t)m * stride + c_offset));
+      for (int k = 0; k < V; k++) x_math[k] = __bfloat162float(x.v[k]);
+      count[j]++;
+      x_count_inv = float(1) / count[j];
+      is_valid = float(1);
+    } else {
+#pragma unroll
+      for (int k = 0; k < V; k++) x_math[k] = float(0);
+      x_count_inv = float(0);
+      is_valid = float(0);
     }
+    m_offset += inner_loop_stride;
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      float x_math[V];
-      float x_count_inv;
-      float is_valid;
-      if (c_valid && m_offset < reduction_size) {
+    for (int k = 0; k < V; k++) {
+      float delta0 = x_math[k] - x_mean[j][k];
+      x_mean[j][k] = __fmaf_rn(delta0, x_count_inv, x_mean[j][k]);   // x_mean += delta0 * x_count_inv
+      float delta1 = x_math[k] - x_mean[j][k];
+      m_2_n[j][k] = __fmaf_rn(__fmul_rn(delta0, delta1), is_valid, m_2_n[j][k]);   // m_2_n += delta0 * delta1 * is_valid
+    }
+  };
+
+  if constexpr (V == 1) {
+    for (int i = 0; i < loop_count; i++) {
+      // all rows of the iteration are loaded before any update uses one
+      BVec<V> xv[PARALLEL_LOADS];
 #pragma unroll
-        for (int k = 0; k < V; k++) x_math[k] = __bfloat162float(xv[j].v[k]);
-        count[j]++;
-        x_count_inv = float(1) / count[j];
-        is_valid = float(1);
-      } else {
-#pragma unroll
-        for (int k = 0; k < V; k++) x_math[k] = float(0);
-        x_count_inv = float(0);
-        is_valid = float(0);
+      for (int j = 0; j < PARALLEL_LOADS; j++) {
+        const int m = m_offset + j * inner_loop_stride;
+        if (c_valid && m < reduction_size) xv[j] = *reinterpret_cast<const BVec<V>*>(input + ((size_t)m * stride + c_offset));
       }
-      m_offset += inner_loop_stride;
 #pragma unroll
-      for (int k = 0; k < V; k++) {
-        float delta0 = x_math[k] - x_mean[j][k];
-        x_mean[j][k] = __fmaf_rn(delta0, x_count_inv, x_mean[j][k]);   // x_mean += delta0 * x_count_inv
-        float delta1 = x_math[k] - x_mean[j][k];
-        m_2_n[j][k] = __fmaf_rn(__fmul_rn(delta0, delta1), is_valid, m_2_n[j][k]);   // m_2_n += delta0 * delta1 * is_valid
-      }
+      for (int j = 0; j < PARALLEL_LOADS; j++) update(j, &xv[j]);
+    }
+  } else {
+    // the ring: iterations i + 1 .. i + kStatsStages - 1 are in flight while iteration i is consumed
+    constexpr unsigned D = kStatsStages;
+    const int threads = blockDim.x * blockDim.y;
+    BVec<V>* ring = reinterpret_cast<BVec<V>*>(ring_smem()) + threadIdx.y * blockDim.x + threadIdx.x;
+    const int first_row = m_offset;
+    auto issue = [&](unsigned it) {
+      BVec<V>* slot = ring + (it % D) * PARALLEL_LOADS * threads;
+      int m = first_row + (int)it * PARALLEL_LOADS * inner_loop_stride;
+#pragma unroll
+      for (int j = 0; j < PARALLEL_LOADS; j++, m += inner_loop_stride)
+        if (c_valid && m < reduction_size) cp_async<sizeof(BVec<V>)>(slot + j * threads, input + ((size_t)m * stride + c_offset));
+      cp_async_commit();
+    };
+#pragma unroll
+    for (unsigned it = 0; it < D - 1; it++) issue(it);
+    for (unsigned i = 0; i < (unsigned)loop_count; i++) {
+      issue(i + D - 1);
+      cp_async_wait<D - 1>();
+      const BVec<V>* slot = ring + (i % D) * PARALLEL_LOADS * threads;
+#pragma unroll
+      for (int j = 0; j < PARALLEL_LOADS; j++) update(j, slot + j * threads);
     }
   }
   float mean_th[V], m2_th[V];
@@ -549,14 +629,18 @@ constexpr int kGradSrcs = 5;
 // `output`.  With `grad_output2` set, dy is the bf16 sum of the two gradients, as autograd rounds it when a tensor
 // has two consumers; without it dy is taken as it is, so a -0.0 gradient stays -0.0.  With `masked` set (the block
 // tail, where g is also the identity branch's gradient, and the stem) g is written there as well.  kGradPool reads
-// the pooled gradient from `grad_output` and the argmax bytes from `mask`, over the input geometry `pool`.  As in
-// k_bn_stats, all rows of an iteration are loaded before the first sum uses one.
+// the pooled gradient from `grad_output` and the argmax bytes from `mask`, over the input geometry `pool`.
+//
+// With `vec` = kBwdVec (the launcher divides block.x by it) a hardware thread carries kBwdVec adjacent torch
+// threads, as in k_bn_stats, and reads dy, x, dy2, y and x2 through the ring, bwd_ring_stages(operands) - 1 iterations
+// ahead of the sums; g is written kBwdVec channels at a time.  With `vec` = 1 (C % 8 != 0, an operand off the
+// 16-byte grid, the stem's kGradPool) each thread loads all rows of an iteration before the first sum uses one.
 //
 // DUAL (a tail whose identity is a downsample branch's batch norm, fed the same g): `input2` is that batch norm's
 // input, and the same walk also sums g * (x2 - mean2).  Each of the three sums is accumulated, merged over the block
 // and over the grid exactly as a k_bn_bwd_reduce launch for its own batch norm would, so Σg is both dbias values.
 template <GradSrc G, bool DUAL>
-__global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
+__global__ void __launch_bounds__(kMaxBlock) k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __restrict__ grad_output,
                                 const bf16* __restrict__ grad_output2, const bf16* __restrict__ output,
                                 const uint8_t* __restrict__ mask, bf16* __restrict__ masked, const float* __restrict__ mean,
                                 const float* __restrict__ inv_std, float* __restrict__ sum_dy_o, float* __restrict__ sum_dy_xmu_o,
@@ -564,144 +648,245 @@ __global__ void k_bn_bwd_reduce(const bf16* __restrict__ input, const bf16* __re
                                 int* semaphores, const PoolDims pool, const bf16* __restrict__ input2,
                                 const float* __restrict__ mean2, const float* __restrict__ inv_std2, float* __restrict__ sum_dy_xmu2_o,
                                 float* __restrict__ grad_weight2, float* __restrict__ grad_bias2, const int reduction_size,
-                                const int stride) {
+                                const int stride, const int vec) {
   static_assert(G != kGradMasked, "the reduce kernel computes g");
   constexpr bool BITS = G == kGradBits;
   constexpr bool POOL = G == kGradPool;
   constexpr int PARALLEL_LOADS = kParallelLoads;
-  float sum_dy[PARALLEL_LOADS];
-  float sum_dy_xmu[PARALLEL_LOADS];
-  float sum_dy_xmu2[PARALLEL_LOADS];
-#pragma unroll
-  for (int i = 0; i < PARALLEL_LOADS; i++) {
-    sum_dy[i] = float(0);
-    sum_dy_xmu[i] = float(0);
-    sum_dy_xmu2[i] = float(0);
-  }
-  int inner_loop_stride = blockDim.y * gridDim.y;
-  int m_offset = blockIdx.y * blockDim.y + threadIdx.y;
-  int c_offset = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c_offset >= stride || m_offset >= reduction_size) return;
+  __shared__ float shmem_sum_dy[kMaxBlock];
+  __shared__ float shmem_sum_dy_xmu[kMaxBlock];
+  __shared__ bool is_last_block_done;
 
-  int loop_count = 1 + (reduction_size - 1) / (inner_loop_stride * PARALLEL_LOADS);
-  int address_base = m_offset * stride + c_offset;
-  int address_increment = inner_loop_stride * stride;
-  auto r_mean = mean[c_offset];
-  auto factor = inv_std[c_offset];
-  const float r_mean2 = DUAL ? mean2[c_offset] : 0.f;
-
-  for (int i = 0; i < loop_count; i++) {
-    bf16 dy_v[PARALLEL_LOADS], dy2_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS], x2_v[PARALLEL_LOADS];
-    uint8_t mask_v[PARALLEL_LOADS];
+  // V channels (torch threads) per hardware thread: 1, the register walk, or kBwdVec, the ring
+  auto body = [&](auto vec_c) {
+    constexpr int V = decltype(vec_c)::value;
+    float sum_dy[PARALLEL_LOADS][V];
+    float sum_dy_xmu[PARALLEL_LOADS][V];
+    float sum_dy_xmu2[PARALLEL_LOADS][V];
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      if (m_offset + j * inner_loop_stride < reduction_size) {
-        const int a = address_base + j * address_increment;
-        if (POOL) dy_v[j] = pool_grad(grad_output, mask, pool, m_offset + j * inner_loop_stride, c_offset, stride);
-        else dy_v[j] = grad_output[a];
-        if (grad_output2) dy2_v[j] = grad_output2[a];
-        if (BITS) mask_v[j] = mask[a >> 3];
-        else if (G == kGradY) y_v[j] = output[a];
-        x_v[j] = input[a];
-        if (DUAL) x2_v[j] = input2[a];
+    for (int i = 0; i < PARALLEL_LOADS; i++) {
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        sum_dy[i][k] = float(0);
+        sum_dy_xmu[i][k] = float(0);
+        sum_dy_xmu2[i][k] = float(0);
       }
     }
-    float x_input[PARALLEL_LOADS];
-    float x_input2[PARALLEL_LOADS];
-    float x_grad_output[PARALLEL_LOADS];
+    int inner_loop_stride = blockDim.y * gridDim.y;
+    int m_offset = blockIdx.y * blockDim.y + threadIdx.y;
+    int c_offset = (blockIdx.x * blockDim.x + threadIdx.x) * V;
+    if (c_offset >= stride || m_offset >= reduction_size) return;
+
+    int loop_count = 1 + (reduction_size - 1) / (inner_loop_stride * PARALLEL_LOADS);
+    int address_base = m_offset * stride + c_offset;
+    int address_increment = inner_loop_stride * stride;
+    float r_mean[V], factor[V], r_mean2[V];
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      if (c_offset < stride && m_offset < reduction_size) {
-        const bf16 dy = !POOL && grad_output2 ? add_grads(dy_v[j], dy2_v[j]) : dy_v[j];
-        const bf16 g = BITS ? relu_grad_bit(dy, (mask_v[j] >> (address_base & 7)) & 1u) : G == kGradY ? relu_grad(dy, y_v[j]) : dy;
-        if (masked) masked[address_base] = g;
-        x_input[j] = __bfloat162float(x_v[j]);
-        x_input2[j] = DUAL ? __bfloat162float(x2_v[j]) : 0.f;
-        x_grad_output[j] = __bfloat162float(g);
+    for (int k = 0; k < V; k++) {
+      r_mean[k] = mean[c_offset + k];
+      factor[k] = inv_std[c_offset + k];
+      r_mean2[k] = DUAL ? mean2[c_offset + k] : 0.f;
+    }
+
+    // the next row of the walk into accumulators j: g from dy (, dy2) and y or the mask byte, written to `masked`
+    // where that is set, then torch's sums; the operands are read only when the row exists
+    auto consume = [&](int j, const BVec<V>* dy_p, const BVec<V>* dy2_p, const BVec<V>* y_p, uint8_t mask_byte, const BVec<V>* x_p,
+                       const BVec<V>* x2_p) {
+      float x_input[V], x_input2[V], x_grad_output[V];
+      if (m_offset < reduction_size) {
+        const unsigned bits = BITS ? mask_byte >> (address_base & 7) : 0u;
+        BVec<V> gv;
+#pragma unroll
+        for (int k = 0; k < V; k++) {
+          const bf16 dy = !POOL && grad_output2 ? add_grads(dy_p->v[k], dy2_p->v[k]) : dy_p->v[k];
+          gv.v[k] = BITS ? relu_grad_bit(dy, (bits >> k) & 1u) : G == kGradY ? relu_grad(dy, y_p->v[k]) : dy;
+          x_input[k] = __bfloat162float(x_p->v[k]);
+          x_input2[k] = DUAL ? __bfloat162float(x2_p->v[k]) : 0.f;
+          x_grad_output[k] = __bfloat162float(gv.v[k]);
+        }
+        if (masked) *reinterpret_cast<BVec<V>*>(masked + address_base) = gv;
       } else {
-        x_input[j] = float(0);
-        x_input2[j] = float(0);
-        x_grad_output[j] = float(0);
+#pragma unroll
+        for (int k = 0; k < V; k++) {
+          x_input[k] = float(0);
+          x_input2[k] = float(0);
+          x_grad_output[k] = float(0);
+        }
       }
       m_offset += inner_loop_stride;
       address_base += address_increment;
-    }
 #pragma unroll
-    for (int j = 0; j < PARALLEL_LOADS; j++) {
-      sum_dy[j] += x_grad_output[j];
-      sum_dy_xmu[j] = __fmaf_rn(x_grad_output[j], x_input[j] - r_mean, sum_dy_xmu[j]);   // += g * (x - mean)
-      if (DUAL) sum_dy_xmu2[j] = __fmaf_rn(x_grad_output[j], x_input2[j] - r_mean2, sum_dy_xmu2[j]);
-    }
-  }
-#pragma unroll
-  for (int j = 1; j < PARALLEL_LOADS; j++) {
-    sum_dy[0] += sum_dy[j];
-    sum_dy_xmu[0] += sum_dy_xmu[j];
-    if (DUAL) sum_dy_xmu2[0] += sum_dy_xmu2[j];
-  }
-  auto sum_dy_th = sum_dy[0];
-  auto sum_dy_xmu_th = sum_dy_xmu[0];
-  float sum_dy_xmu2_th = sum_dy_xmu2[0];
-
-  __shared__ float shmem_sum_dy[kMaxBlock];
-  __shared__ float shmem_sum_dy_xmu[kMaxBlock];
-  // the third sum takes the same tree after the first two (each value's tree is independent of the others)
-  auto merge = [&]() {
-    merge_block_vertical_backward(sum_dy_th, sum_dy_xmu_th, shmem_sum_dy, shmem_sum_dy_xmu);
-    if (DUAL) {
-      __syncthreads();
-      float unused = 0.f;
-      merge_block_vertical_backward(sum_dy_xmu2_th, unused, shmem_sum_dy, shmem_sum_dy_xmu);
-    }
-  };
-  merge();
-
-  auto write_sums = [&]() {
-    grad_bias[c_offset] = sum_dy_th;
-    grad_weight[c_offset] = sum_dy_xmu_th * factor;
-    sum_dy_o[c_offset] = sum_dy_th;
-    sum_dy_xmu_o[c_offset] = sum_dy_xmu_th;
-    if (DUAL) {
-      grad_bias2[c_offset] = sum_dy_th;
-      grad_weight2[c_offset] = sum_dy_xmu2_th * inv_std2[c_offset];
-      sum_dy_xmu2_o[c_offset] = sum_dy_xmu2_th;
-    }
-  };
-  if (gridDim.y > 1) {
-    volatile float* staging_sum_dy = staging_data;
-    volatile float* staging_sum_dy_xmu = &staging_data[stride * gridDim.y];
-    volatile float* staging_sum_dy_xmu2 = &staging_data[2 * stride * gridDim.y];
-    address_base = c_offset + blockIdx.y * stride;
-    if (threadIdx.y == 0 && c_offset < stride) {
-      staging_sum_dy[address_base] = sum_dy_th;
-      staging_sum_dy_xmu[address_base] = sum_dy_xmu_th;
-      if (DUAL) staging_sum_dy_xmu2[address_base] = sum_dy_xmu2_th;
-    }
-    __threadfence();
-    __syncthreads();
-    __shared__ bool is_last_block_done;
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-      int old = atomicAdd(&semaphores[blockIdx.x], 1);
-      is_last_block_done = (old == (gridDim.y - 1));
-      if (is_last_block_done) semaphores[blockIdx.x] = 0;
-    }
-    __syncthreads();
-    if (is_last_block_done) {
-      sum_dy_th = float(0.0);
-      sum_dy_xmu_th = float(0.0);
-      sum_dy_xmu2_th = float(0.0);
-      for (int y = threadIdx.y; y < gridDim.y; y += blockDim.y) {
-        address_base = c_offset + y * stride;
-        sum_dy_th += (c_offset < stride ? staging_sum_dy[address_base] : float(0.0));
-        sum_dy_xmu_th += (c_offset < stride ? staging_sum_dy_xmu[address_base] : float(0.0));
-        if (DUAL) sum_dy_xmu2_th += (c_offset < stride ? staging_sum_dy_xmu2[address_base] : float(0.0));
+      for (int k = 0; k < V; k++) {
+        sum_dy[j][k] += x_grad_output[k];
+        sum_dy_xmu[j][k] = __fmaf_rn(x_grad_output[k], x_input[k] - r_mean[k], sum_dy_xmu[j][k]);   // += g * (x - mean)
+        if (DUAL) sum_dy_xmu2[j][k] = __fmaf_rn(x_grad_output[k], x_input2[k] - r_mean2[k], sum_dy_xmu2[j][k]);
       }
-      merge();
-      if (threadIdx.y == 0 && c_offset < stride) write_sums();
+    };
+
+    if constexpr (V == 1) {
+      for (int i = 0; i < loop_count; i++) {
+        // all rows of the iteration are loaded before any sum uses one
+        BVec<V> dy_v[PARALLEL_LOADS], dy2_v[PARALLEL_LOADS], y_v[PARALLEL_LOADS], x_v[PARALLEL_LOADS], x2_v[PARALLEL_LOADS];
+        uint8_t mask_v[PARALLEL_LOADS];
+#pragma unroll
+        for (int j = 0; j < PARALLEL_LOADS; j++) {
+          if (m_offset + j * inner_loop_stride < reduction_size) {
+            const int a = address_base + j * address_increment;
+            if (POOL) dy_v[j].v[0] = pool_grad(grad_output, mask, pool, m_offset + j * inner_loop_stride, c_offset, stride);
+            else dy_v[j].v[0] = grad_output[a];
+            if (grad_output2) dy2_v[j].v[0] = grad_output2[a];
+            if (BITS) mask_v[j] = mask[a >> 3];
+            else if (G == kGradY) y_v[j].v[0] = output[a];
+            x_v[j].v[0] = input[a];
+            if (DUAL) x2_v[j].v[0] = input2[a];
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < PARALLEL_LOADS; j++) consume(j, &dy_v[j], &dy2_v[j], &y_v[j], mask_v[j], &x_v[j], &x2_v[j]);
+      }
+    } else {
+      const int ops = bwd_ring_operands(G == kGradY, grad_output2 != nullptr, DUAL);
+      // the ring: iterations i + 1 .. i + D - 1 are in flight while iteration i is consumed
+      auto ring_walk = [&](auto stages_c) {
+        constexpr unsigned D = decltype(stages_c)::value;
+        const int threads = blockDim.x * blockDim.y;
+        const int op_dy2 = 2, op_y = op_dy2 + (grad_output2 != nullptr), op_x2 = op_y + (G == kGradY);   // dy is 0, x is 1
+        BVec<V>* ring = reinterpret_cast<BVec<V>*>(ring_smem()) + threadIdx.y * blockDim.x + threadIdx.x;
+        auto stage = [&](unsigned it) { return ring + (it % D) * ops * PARALLEL_LOADS * threads; };
+        const int first_row = m_offset;
+        const int iteration_rows = PARALLEL_LOADS * inner_loop_stride;
+        auto issue = [&](unsigned it) {
+          BVec<V>* slot = stage(it);
+          int m = first_row + (int)it * iteration_rows;
+#pragma unroll
+          for (int j = 0; j < PARALLEL_LOADS; j++, m += inner_loop_stride, slot += threads) {
+            if (m < reduction_size) {
+              const size_t a = (size_t)m * stride + c_offset;
+              cp_async<sizeof(BVec<V>)>(slot, grad_output + a);
+              cp_async<sizeof(BVec<V>)>(slot + PARALLEL_LOADS * threads, input + a);
+              if (grad_output2) cp_async<sizeof(BVec<V>)>(slot + op_dy2 * PARALLEL_LOADS * threads, grad_output2 + a);
+              if (G == kGradY) cp_async<sizeof(BVec<V>)>(slot + op_y * PARALLEL_LOADS * threads, output + a);
+              if (DUAL) cp_async<sizeof(BVec<V>)>(slot + op_x2 * PARALLEL_LOADS * threads, input2 + a);
+            }
+          }
+          cp_async_commit();
+        };
+        // the mask (1/16 of the traffic; one byte holds a thread's V bits) is a plain load, one iteration ahead
+        uint8_t mask_next[PARALLEL_LOADS];
+        auto load_mask = [&](unsigned it) {
+          int m = first_row + (int)it * iteration_rows;
+#pragma unroll
+          for (int j = 0; j < PARALLEL_LOADS; j++, m += inner_loop_stride)
+            if (m < reduction_size) mask_next[j] = mask[((size_t)m * stride + c_offset) >> 3];
+        };
+        if (BITS) load_mask(0);
+#pragma unroll
+        for (unsigned it = 0; it < D - 1; it++) issue(it);
+        for (unsigned i = 0; i < (unsigned)loop_count; i++) {
+          issue(i + D - 1);
+          uint8_t mask_v[PARALLEL_LOADS];
+#pragma unroll
+          for (int j = 0; j < PARALLEL_LOADS; j++) mask_v[j] = mask_next[j];
+          if (BITS) load_mask(i + 1);
+          cp_async_wait<D - 1>();
+          const BVec<V>* slot = stage(i);
+#pragma unroll
+          for (int j = 0; j < PARALLEL_LOADS; j++, slot += threads)
+            consume(j, slot, slot + op_dy2 * PARALLEL_LOADS * threads, slot + op_y * PARALLEL_LOADS * threads, mask_v[j],
+                    slot + PARALLEL_LOADS * threads, slot + op_x2 * PARALLEL_LOADS * threads);
+        }
+      };
+      if (DUAL || bwd_ring_stages(ops) == kBwdStagesWide) ring_walk(std::integral_constant<unsigned, kBwdStagesWide>{});
+      else ring_walk(std::integral_constant<unsigned, kBwdStages>{});
     }
-  } else {
-    if (blockIdx.y == 0 && threadIdx.y == 0 && c_offset < stride) write_sums();
-  }
+
+    float sum_dy_th[V], sum_dy_xmu_th[V], sum_dy_xmu2_th[V];
+#pragma unroll
+    for (int k = 0; k < V; k++) {
+#pragma unroll
+      for (int j = 1; j < PARALLEL_LOADS; j++) {
+        sum_dy[0][k] += sum_dy[j][k];
+        sum_dy_xmu[0][k] += sum_dy_xmu[j][k];
+        if (DUAL) sum_dy_xmu2[0][k] += sum_dy_xmu2[j][k];
+      }
+      sum_dy_th[k] = sum_dy[0][k];
+      sum_dy_xmu_th[k] = sum_dy_xmu[0][k];
+      sum_dy_xmu2_th[k] = sum_dy_xmu2[0][k];
+    }
+
+    // the third sum takes the same tree after the first two (each value's tree is independent of the others)
+    auto merge = [&]() {
+      merge_block_vertical_backward<V>(sum_dy_th, sum_dy_xmu_th, shmem_sum_dy, shmem_sum_dy_xmu);
+      if (DUAL) {
+        __syncthreads();
+        float unused[V] = {};
+        merge_block_vertical_backward<V>(sum_dy_xmu2_th, unused, shmem_sum_dy, shmem_sum_dy_xmu);
+      }
+    };
+    merge();
+
+    auto write_sums = [&]() {
+#pragma unroll
+      for (int k = 0; k < V; k++) {
+        const int c = c_offset + k;
+        grad_bias[c] = sum_dy_th[k];
+        grad_weight[c] = sum_dy_xmu_th[k] * factor[k];
+        sum_dy_o[c] = sum_dy_th[k];
+        sum_dy_xmu_o[c] = sum_dy_xmu_th[k];
+        if (DUAL) {
+          grad_bias2[c] = sum_dy_th[k];
+          grad_weight2[c] = sum_dy_xmu2_th[k] * inv_std2[c];
+          sum_dy_xmu2_o[c] = sum_dy_xmu2_th[k];
+        }
+      }
+    };
+    if (gridDim.y > 1) {
+      volatile float* staging_sum_dy = staging_data;
+      volatile float* staging_sum_dy_xmu = &staging_data[stride * gridDim.y];
+      volatile float* staging_sum_dy_xmu2 = &staging_data[2 * stride * gridDim.y];
+      address_base = c_offset + blockIdx.y * stride;
+      if (threadIdx.y == 0 && c_offset < stride) {
+#pragma unroll
+        for (int k = 0; k < V; k++) {
+          staging_sum_dy[address_base + k] = sum_dy_th[k];
+          staging_sum_dy_xmu[address_base + k] = sum_dy_xmu_th[k];
+          if (DUAL) staging_sum_dy_xmu2[address_base + k] = sum_dy_xmu2_th[k];
+        }
+      }
+      __threadfence();
+      __syncthreads();
+      if (threadIdx.x == 0 && threadIdx.y == 0) {
+        int old = atomicAdd(&semaphores[blockIdx.x], 1);
+        is_last_block_done = (old == (gridDim.y - 1));
+        if (is_last_block_done) semaphores[blockIdx.x] = 0;
+      }
+      __syncthreads();
+      if (is_last_block_done) {
+#pragma unroll
+        for (int k = 0; k < V; k++) {
+          sum_dy_th[k] = float(0.0);
+          sum_dy_xmu_th[k] = float(0.0);
+          sum_dy_xmu2_th[k] = float(0.0);
+        }
+        for (int y = threadIdx.y; y < gridDim.y; y += blockDim.y) {
+          address_base = c_offset + y * stride;
+#pragma unroll
+          for (int k = 0; k < V; k++) {
+            sum_dy_th[k] += (c_offset < stride ? staging_sum_dy[address_base + k] : float(0.0));
+            sum_dy_xmu_th[k] += (c_offset < stride ? staging_sum_dy_xmu[address_base + k] : float(0.0));
+            if (DUAL) sum_dy_xmu2_th[k] += (c_offset < stride ? staging_sum_dy_xmu2[address_base + k] : float(0.0));
+          }
+        }
+        merge();
+        if (threadIdx.y == 0 && c_offset < stride) write_sums();
+      }
+    } else {
+      if (blockIdx.y == 0 && threadIdx.y == 0 && c_offset < stride) write_sums();
+    }
+  };
+  if constexpr (POOL) body(std::integral_constant<int, 1>{});
+  else if (vec == kBwdVec) body(std::integral_constant<int, kBwdVec>{});
+  else body(std::integral_constant<int, 1>{});
 }
 
 // dx (torch: batch_norm_backward_elemt_channels_last_kernel_impl) with g from G (kGradMasked: `grad_output` is the

@@ -303,16 +303,21 @@ def site_inputs(m, c, seed):
     return x, dy, bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var
 
 
-def torch_site(x, dy, w, b, rm, rv, eps=1e-5, momentum=0.1):
+def torch_site(x, dy, w, b, rm, rv, eps=1e-5, momentum=0.1, dy2=None, relu=True):
+    """torch's functional chain for one site of m rows: native_batch_norm, relu (unless `relu` is False), then
+    threshold_backward of the output gradient, bf16(dy + dy2) where the output has two consumers, and
+    native_batch_norm_backward.  "g" is the batch norm's output gradient."""
     m, c = x.shape
     x4, dy4 = x.view(m, c, 1, 1), dy.view(m, c, 1, 1)   # NCHW strides with stride(1) == 1: torch's channels-last kernels
+    if dy2 is not None:
+        dy4 = dy4 + dy2.view(m, c, 1, 1)
     rm, rv = rm.clone(), rv.clone()
     out, mean, invstd = torch.native_batch_norm(x4, w, b, rm, rv, True, momentum, eps)
-    y = torch.relu(out)
-    grad = torch.ops.aten.threshold_backward(dy4, y, 0)
+    y = torch.relu(out) if relu else out
+    grad = torch.ops.aten.threshold_backward(dy4, y, 0) if relu else dy4
     dx, dw, db = torch.ops.aten.native_batch_norm_backward(grad, x4, w, rm, rv, mean, invstd, True, eps, [True, True, True])
     return {"y": y.view(m, c), "mean": mean, "invstd": invstd, "running_mean": rm, "running_var": rv, "dx": dx.view(m, c),
-            "dweight": dw, "dbias": db}
+            "dweight": dw, "dbias": db, "g": grad.view(m, c)}
 
 
 def native_site(x, dy, w, b, rm, rv, scratch, stream, eps=1e-5, momentum=0.1):
@@ -367,7 +372,7 @@ def check_native_site(m, c, seed):
     launch()
     torch.cuda.synchronize()
     check_scratch(buf, need)
-    for k in want:
+    for k in got:
         assert same_bits(got[k], want[k]), k
     return x, got
 

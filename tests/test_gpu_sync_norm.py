@@ -11,8 +11,10 @@ Sites: ReLU (stem / conv1 / conv2 positions), tails with one and with two output
 module's own forward, e.g. a downsample branch).  Shapes: every batch-norm shape of ResNet-50 with a global batch
 split unevenly over the ranks, including an empty and a single-row rank; one shape per launch regime of the reducing
 kernels on rank 0 with one image on every other rank (gpu_common.BN_REGIME_SHAPES); C = 100 (scalar kernels, no
-mask); an operand off the 16-byte grid; the value edges of test_gpu_fused_norm; through the C-ABI, a ReLU site that
-reads y instead of a mask at C % 8 == 0, and the sync scratch's guard bytes."""
+mask); an operand off the 16-byte grid, on every rank or on one rank only; ranks whose row walks through the
+statistics' and backward reduce's rings have different lengths (test_bn_ring_cpu.sync_splits); the value edges of
+test_gpu_fused_norm; through the C-ABI, a ReLU site that reads y instead of a mask at C % 8 == 0, with one output
+gradient or two, and the sync scratch's guard bytes."""
 import copy
 
 import pytest
@@ -22,6 +24,7 @@ import torch.nn as nn
 from ant_ray_b200 import _native as N
 from ant_ray_b200 import fused_norm
 from gpu_common import BN_MAX_CHANNELS, BN_REGIME_SHAPES, assert_same_values
+from test_bn_ring_cpu import SYNC_RING_C, sync_splits
 from test_gpu_fused_norm import RESNET50_BN_SHAPES, edge_bn_setup, edge_site_inputs, misaligned
 
 pytestmark = pytest.mark.gpu
@@ -136,15 +139,18 @@ def reference(bn, xs, ids, dys, dy2s, kind):
     return out
 
 
-def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=()):
+def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=(), misalign_ranks=None):
+    """`misalign` names the operands moved off the 16-byte grid, on the ranks in `misalign_ranks` (every rank when
+    None)."""
     W = world.world_size
     bns = [fused_norm.sync_batch_norm(copy.deepcopy(bn), world.comms[r]) for r in range(W)]
     relu = nn.ReLU(inplace=True)
     results = [None] * W
     # inputs that require grad are leaves made on the current stream before the ranks' streams start
     # (an empty input keeps its own strides: see test_empty_rank_input_from_a_convolution)
-    xs = [(misaligned(x) if "x" in misalign and x.numel() else x.clone() if x.numel() else x.detach()).requires_grad_()
-          for x in xs]
+    off = lambda r: misalign_ranks is None or r in misalign_ranks  # noqa: E731
+    xs = [(misaligned(x) if "x" in misalign and x.numel() and off(r) else x.clone() if x.numel() else x.detach()).requires_grad_()
+          for r, x in enumerate(xs)]
     ids = [(i.clone() if i is not None else None) for i in ids]
     for i in ids:
         if i is not None:
@@ -208,7 +214,7 @@ def collective_launches(world, c):
 
 
 def check_sites(world, n, c, h, w, kind, seed, inputs=None, bn_setup=None, misalign=(), sizes=None, collectives=None,
-                **bn_args):
+                misalign_ranks=None, **bn_args):
     W = world.world_size
     sizes = sizes or split_rows(n, W, seed)
     assert sum(sizes) == n
@@ -228,7 +234,7 @@ def check_sites(world, n, c, h, w, kind, seed, inputs=None, bn_setup=None, misal
     if bn_setup is not None:
         bn_setup(bn)
     want = reference(bn, xs, ids, dys, dy2s, kind)
-    got, launched = run_native(world, bn, xs, ids, dys, dy2s, kind, misalign)
+    got, launched = run_native(world, bn, xs, ids, dys, dy2s, kind, misalign, misalign_ranks)
     compare(got, want, sizes)
     # per rank: 2 collectives (one launch each, unless `collectives` counts their pieces), the merge, and 4 local
     # kernels when it has rows
@@ -324,6 +330,19 @@ def test_misaligned_input_takes_the_scalar_kernels(world, kind):
     check_sites(world, 3 * world.world_size, 64, 7, 7, kind, seed=5, misalign=("x",))
 
 
+@pytest.mark.parametrize("kind", ["relu", "tail2", "plain"])
+def test_ranks_walk_the_rings_for_different_lengths(world, kind):
+    # H = W = 1: each rank's rows are its images.  Every split runs once with every rank on its ring and once with one
+    # rank's x off the 16-byte grid, so that rank takes the register walks while its peers take the rings.
+    W = world.world_size
+    for i, sizes in enumerate(sync_splits(W)):
+        check_sites(world, sum(sizes), SYNC_RING_C, 1, 1, kind, seed=31 * i + W, sizes=sizes)
+        rank = max(range(W), key=lambda r: (sizes[r], -r)) if i % 2 else (i // 2) % W
+        if sizes[rank]:
+            check_sites(world, sum(sizes), SYNC_RING_C, 1, 1, kind, seed=31 * i + W, sizes=sizes, misalign=("x",),
+                        misalign_ranks=(rank,))
+
+
 @pytest.mark.parametrize("kind", ["tail", "plain"])
 @pytest.mark.parametrize("grad_edges", [False, True], ids=["input_edges", "gradient_edges"])
 def test_value_edges(world, grad_edges, kind):
@@ -388,18 +407,26 @@ def test_relu_site_reading_y_through_the_c_abi(world, c):
     check_relu_site_reading_y(world, c)
 
 
-def check_relu_site_reading_y(world, c):
+@pytest.mark.parametrize("c", [64, 2048])
+def test_relu_site_reading_y_with_two_gradients_through_the_c_abi(world, c):
+    # the backward reduce's ring of dy, x, y and dy2: 4 operands, 2 stages
+    check_relu_site_reading_y(world, c, two_grads=True)
+
+
+def check_relu_site_reading_y(world, c, two_grads=False):
     """b200c_bn_sync_forward with relu = 1 and no mask, then b200c_bn_sync_backward from y: the vector elementwise
     backward that reads y and the device's 1 / rows of all ranks (the fused module passes a mask at C % 8 == 0).  The
-    ranks hold different batch sizes, so a rank's own 1 / rows would differ from the global one."""
+    ranks hold different batch sizes, so a rank's own 1 / rows would differ from the global one.  With `two_grads`
+    the output has a second gradient dy2, summed to bf16(dy + dy2) as autograd sums it."""
     W, h, w = world.world_size, 5, 5
     sizes = [2 + r for r in range(W)]
     lib = N.load()
     g = torch.Generator(device="cuda").manual_seed(c + W)
     xs = [cl((torch.randn(m, c, h, w, device="cuda", generator=g) * 2 + 0.5).to(torch.bfloat16)) for m in sizes]
     dys = [cl(torch.randn(m, c, h, w, device="cuda", generator=g).to(torch.bfloat16)) for m in sizes]
+    dy2s = [cl(torch.randn(m, c, h, w, device="cuda", generator=g).to(torch.bfloat16)) if two_grads else None for m in sizes]
     bn = make_sync_bn(c, c + W)
-    want = reference(bn, xs, [None] * W, dys, [None] * W, "relu")
+    want = reference(bn, xs, [None] * W, [d + d2 for d, d2 in zip(dys, dy2s)] if two_grads else dys, [None] * W, "relu")
     need = int(lib.b200c_bn_sync_scratch_bytes(c, W))
     w_, b_ = bn.weight.detach(), bn.bias.detach()
     st = [dict(rm=bn.running_mean.clone(), rv=bn.running_var.clone(), nbt=bn.num_batches_tracked.clone(), y=torch.empty_like(x),
@@ -412,9 +439,9 @@ def check_relu_site_reading_y(world, c):
         N.check(lib.b200c_bn_sync_forward(comm._h(), xs[r].data_ptr(), None, s["y"].data_ptr(), None, 1, w_.data_ptr(),
                                           b_.data_ptr(), s["rm"].data_ptr(), s["rv"].data_ptr(), s["nbt"].data_ptr(), p, p + 4 * c,
                                           p + 8 * c, m, c, 0.1, 1e-5, s["scratch"].data_ptr(), stream))
-        N.check(lib.b200c_bn_sync_backward(comm._h(), dys[r].data_ptr(), None, s["y"].data_ptr(), None, 1, xs[r].data_ptr(), None,
-                                           s["dx"].data_ptr(), w_.data_ptr(), p, p + 4 * c, p + 8 * c, s["dw"].data_ptr(),
-                                           s["db"].data_ptr(), m, c, s["scratch"].data_ptr(), stream))
+        N.check(lib.b200c_bn_sync_backward(comm._h(), dys[r].data_ptr(), dy2s[r].data_ptr() if two_grads else None, s["y"].data_ptr(),
+                                           None, 1, xs[r].data_ptr(), None, s["dx"].data_ptr(), w_.data_ptr(), p, p + 4 * c, p + 8 * c,
+                                           s["dw"].data_ptr(), s["db"].data_ptr(), m, c, s["scratch"].data_ptr(), stream))
 
     world.run(step)
     torch.cuda.synchronize()

@@ -136,13 +136,17 @@ def test_outputs_at_the_corners_and_past_exp_overflow(act):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("c", [64, 100])
+@pytest.mark.parametrize("c", [1, 64, 100])
 @pytest.mark.parametrize("act", list(ACTS))
 def test_nchw_gradient_keeps_eager_torch_s_backward(act, c):
     # an NCHW dy (the gradient a model's average pool hands its last block): eager torch's activation backward writes g
-    # in NCHW and its batch-norm backward takes its NCHW kernels, so the site's backward runs those torch ops
+    # in NCHW and its batch-norm backward takes its NCHW kernels, so the site's backward runs those torch ops.  With one
+    # channel NCHW strides (stride(1) == H * W) also pass the channels-last check, so the site runs its native backward,
+    # and eager torch's kernels on that gradient must round alike.
     x, dy = gauss_inputs(8, c, 7, 7, c)
-    check_site(act, x, dy.contiguous(), launches=2, seed=c)
+    dy = torch.empty(dy.shape, dtype=dy.dtype, device=dy.device).copy_(dy)   # default strides, even where C == 1
+    assert dy.stride(1) == 7 * 7 and dy.is_contiguous(memory_format=CL) == (c == 1)
+    check_site(act, x, dy, launches=4 if c == 1 else 2, seed=c)
 
 
 @pytest.mark.gpu

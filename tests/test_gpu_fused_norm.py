@@ -80,16 +80,21 @@ def test_fused_site_is_bit_identical_to_eager_torch(n, c, h, w, residual):
 def test_one_scratch_serves_every_channel_count():
     # A narrow site whose grid merge spans many rows stages its partial sums in the scratch buffer that the
     # semaphores of a later wide site share (one buffer per stream); every site must still merge correctly.  Local,
-    # dual and stem sites interleave on the stream: the buffer grows at the first dual site, which needs more than
-    # the sites before it; a wide dual site (plane 1 on semaphores 512 .. 1023) is followed by narrow local sites,
-    # and a dual site's plane 1 counts on semaphores a wider local site used before it.
+    # dual, stem, activation and residual sites interleave on the stream: the buffer grows at the first dual site,
+    # which needs more than the sites before it; a narrow merged activation site follows a wide local site; a wide dual
+    # site (plane 1 on semaphores 512 .. 1023) and a wide stochastic-depth site, whose backward reduce keeps its own copy
+    # of the grid merge, are followed by narrow local sites; and a dual site's plane 1 counts on semaphores a wider
+    # local site used before it.  After every site the semaphores are all back at zero.
+    import test_gpu_fused_act as act
+    import test_gpu_fused_res as res
     from test_gpu_fused_dual import check_dual, inputs as dual_inputs
     from test_gpu_fused_stem import check_stem, gauss_inputs
 
     fused_norm._scratch.clear()
     sites = [("local", (256, 16, 56, 56)), ("stem", (8, 16, 56, 56)), ("dual", (32, 512, 28, 28)), ("local", (256, 2048, 7, 7)),
-             ("local", (256, 32, 56, 56)), ("dual", (2, 16384, 32, 32)), ("local", (256, 16, 56, 56)), ("local", (3, 100, 9, 9)),
-             ("local", (256, 2048, 7, 7)), ("dual", (32, 1024, 14, 14)), ("stem", (3, 100, 9, 9)), ("local", (256, 32, 56, 56))]
+             ("silu", (256, 16, 56, 56)), ("local", (256, 32, 56, 56)), ("dual", (2, 16384, 32, 32)), ("drop", (2, 16384, 32, 32)),
+             ("local", (256, 16, 56, 56)), ("local", (3, 100, 9, 9)), ("add", (32, 24, 56, 56)), ("local", (256, 2048, 7, 7)),
+             ("dual", (32, 1024, 14, 14)), ("hardswish", (64, 100, 28, 28)), ("stem", (3, 100, 9, 9)), ("local", (256, 32, 56, 56))]
     sizes = []
     for kind, (n, c, h, w) in sites:
         if kind == "local":
@@ -98,10 +103,17 @@ def test_one_scratch_serves_every_channel_count():
         elif kind == "dual":
             x3, x_ds, dy1, dy2 = dual_inputs(n, c, h, w, c + n)
             check_dual(x3, x_ds, dy1, dy2, "pair", make_bn(c, 1), make_bn(c, 2))
-        else:
+        elif kind == "stem":
             check_stem(*gauss_inputs(n, c, h, w, c + n), make_bn(c, 3))
+        elif kind in act.ACTS:
+            act.check_gauss_site(kind, n, c, h, w)
+        else:
+            res.check_gauss_site(kind, n, c, h, w)
+        torch.cuda.synchronize()
         assert len(fused_norm._scratch) == 1
-        sizes.append(next(iter(fused_norm._scratch.values()))[0])
+        size, _, buf = next(iter(fused_norm._scratch.values()))
+        assert (buf[:SEMAPHORE_BYTES] == 0).all(), f"a {kind} site at {(n, c, h, w)} left a semaphore set"
+        sizes.append(size)
     assert sizes[2] > sizes[1] == sizes[0], sizes
 
 

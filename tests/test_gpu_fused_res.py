@@ -173,13 +173,16 @@ def test_hyperparameters(kind, momentum, eps):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("c", [64, 100])
+@pytest.mark.parametrize("c", [1, 64, 100])
 @pytest.mark.parametrize("kind", KINDS)
 def test_nchw_gradient_keeps_eager_torch_s_backward(kind, c):
     # an NCHW dy: eager torch's mul writes g in NCHW and its batch-norm backward takes its NCHW kernels, so the site's
-    # backward runs those torch ops
+    # backward runs those torch ops.  With one channel NCHW strides (stride(1) == H * W) also pass the channels-last
+    # check, so the site runs its native backward, and eager torch's kernels on that gradient must round alike.
     x, identity, dy = gauss_inputs(8, c, 7, 7, c)
-    check_site(kind, x, identity, dy.contiguous(), launches=2, seed=c)
+    dy = torch.empty(dy.shape, dtype=dy.dtype, device=dy.device).copy_(dy)   # default strides, even where C == 1
+    assert dy.stride(1) == 7 * 7 and dy.is_contiguous(memory_format=CL) == (c == 1)
+    check_site(kind, x, identity, dy, launches=4 if c == 1 else 2, seed=c)
 
 
 # ---- eval sites -------------------------------------------------------------------------------------------------

@@ -17,6 +17,7 @@
 #include "byte_kernels.cuh"
 #include "launch_typed.cuh"
 #include "norm_launch.h"
+#include "se_launch.h"
 
 using namespace b200c;
 
@@ -1746,6 +1747,75 @@ extern "C" int b200c_bn_infer_res(const void* x, const void* identity, void* y, 
   if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer res: null buffer");
   RT(bn::infer_res({x, identity, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0},
                    (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// squeeze-and-excitation (se_kernels.cuh, launched by inst_se.cu): one kernel per call
+// ------------------------------------------------------------------------------------------------
+// The shape checks of every call.  With one channel and more than one row the reduced dimension is the fastest one,
+// where torch's reduction takes another path (vectorize along input), so the reducing kernels reject it.
+static int check_se(const char* site, int n, int c, int hw, bool reduce) {
+  if (n < 1 || c < 1 || hw < 1 || (int64_t)n * c * hw > INT32_MAX)
+    return fail(B200C_EINVAL, "%s: bad shape n=%d c=%d hw=%d", site, n, c, hw);
+  if (reduce && c == 1 && hw > 1) return fail(B200C_EINVAL, "%s: one channel with hw=%d reduces along the fastest dimension", site, hw);
+  return B200C_OK;
+}
+
+extern "C" size_t b200c_se_scratch_bytes(int n, int c, int hw) {
+  if (n < 1 || c < 1 || hw < 1 || (int64_t)n * c * hw > INT32_MAX) return 0;
+  cudaError_t e;
+  size_t bytes = se::scratch_bytes(n, c, hw, &e);
+  if (e != cudaSuccess) fail(B200C_ECUDA, "se scratch: %s", cudaGetErrorString(e));
+  return bytes;
+}
+
+static int check_se_scratch(const char* site, int n, int c, int hw, const void* scratch, size_t scratch_bytes) {
+  if (!scratch) return fail(B200C_EINVAL, "%s: null scratch", site);
+  const size_t need = b200c_se_scratch_bytes(n, c, hw);
+  if (!need) return B200C_ECUDA;
+  if (scratch_bytes < need) return fail(B200C_EINVAL, "%s: scratch of %zu bytes, needs %zu", site, scratch_bytes, need);
+  return B200C_OK;
+}
+
+extern "C" int b200c_se_pool(const void* x, void* pooled, int n, int channels, int hw, void* scratch, size_t scratch_bytes,
+                             b200c_stream_t stream) {
+  int rc = check_se("se pool", n, channels, hw, true);
+  if (!rc && (!x || !pooled)) rc = fail(B200C_EINVAL, "se pool: null buffer");
+  if (!rc) rc = check_se_scratch("se pool", n, channels, hw, scratch, scratch_bytes);
+  if (rc) return rc;
+  RT(se::pool(x, pooled, n, channels, hw, scratch, (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+extern "C" int b200c_se_scale(const void* x, const void* s, void* y, int n, int channels, int hw, b200c_stream_t stream) {
+  int rc = check_se("se scale", n, channels, hw, false);
+  if (rc) return rc;
+  if (!x || !s || !y) return fail(B200C_EINVAL, "se scale: null buffer");
+  RT(se::scale(x, s, y, n, channels, hw, (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+extern "C" int b200c_se_backward_reduce(const void* dy, const void* x, void* ds, int n, int channels, int hw, void* scratch,
+                                        size_t scratch_bytes, b200c_stream_t stream) {
+  int rc = check_se("se backward reduce", n, channels, hw, true);
+  if (!rc && (!dy || !x || !ds)) rc = fail(B200C_EINVAL, "se backward reduce: null buffer");
+  if (!rc) rc = check_se_scratch("se backward reduce", n, channels, hw, scratch, scratch_bytes);
+  if (rc) return rc;
+  RT(se::backward_reduce(dy, x, ds, n, channels, hw, scratch, (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+extern "C" int b200c_se_backward_elemt(const void* dy, const void* s, const void* gp, void* dx, int n, int channels, int hw,
+                                       b200c_stream_t stream) {
+  int rc = check_se("se backward elemt", n, channels, hw, false);
+  if (rc) return rc;
+  if (!dy || !s || !gp || !dx) return fail(B200C_EINVAL, "se backward elemt: null buffer");
+  RT(se::backward_elemt(dy, s, gp, dx, n, channels, hw, (cudaStream_t)stream));
   g_launches.fetch_add(1);
   return B200C_OK;
 }

@@ -1,5 +1,6 @@
 """Fused batch norm for the training step and eval forward of ResNets and of torchvision's Conv2dNormActivation blocks
-(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh).
+(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh), and the squeeze-and-excitation of
+EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
 by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
@@ -41,6 +42,18 @@ stochastic depth ("row" mode, its noise built by torchvision's own torch calls) 
 above, with no hook on the block's Sequential, the projection, its batch norm or the stochastic depth; in eval without
 autograd recording the site is one launch.
 
+Squeeze-and-excitation: inside those swapped MBConv and MobileNetV3 blocks, `fuse_model` also swaps torchvision's
+`SqueezeExcitation` for `FusedSqueezeExcitation`, whose average pool and scale `s * x` run on native kernels (the
+squeeze path, fc1, activation, fc2 and scale activation, still runs as modules on torch): in training, a pool and a
+scale forward, and backward one reduce (s's gradient, the sum over H, W of dy * x) and one elementwise kernel that
+writes x's whole gradient (dy * s plus the mean's gp / HW) once; without autograd recording, the two forward launches.
+The two sums keep the launch shape and order of torch's reduce kernel, so outputs and gradients are eager torch's bits.
+A site runs there when x is a non-empty bf16 channels-last CUDA tensor with a channel stride of 1, fewer than 2^30
+elements and not one channel over several rows, the module's avgpool is exactly an nn.AdaptiveAvgPool2d(1) without
+hooks, and no global module hook is registered; otherwise the parent's forward runs.  A squeeze path that returns
+anything but a bf16 [N, C, 1, 1] on x's device gets torch's `s * x`, and a gradient that arrives in another layout
+than channels-last torch's backward ops.
+
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
 more than one rank (a "sync site"), its statistics are gathered and its gradient sums reduced over that
@@ -66,6 +79,9 @@ _lib = None
 # are ordered.
 _scratch = {}
 _scratch_need = {}   # (channels, world or None) -> the library's scratch bytes; 0: more channels than the kernels take
+# the squeeze-excitation sites' scratch, as _scratch (its semaphores sit at the start as well, so it is a buffer of its own)
+_se_scratch = {}
+_se_need = {}        # (device index, n, c, hw) -> b200c_se_scratch_bytes
 _NATIVE = torch._C._BatchNormBackend.Native
 # the current stream's handle without building a torch.cuda.Stream object: each step makes 98 fused calls
 _raw_stream = torch._C._cuda_getCurrentRawStream
@@ -93,12 +109,12 @@ def _scratch_bytes(channels, world=None):
     return need
 
 
-def _scratch_ptr(device, stream, need):
+def _scratch_ptr(device, stream, need, table=_scratch):
     key = (device.index, stream)
-    entry = _scratch.get(key)
+    entry = table.get(key)
     if entry is None or entry[0] < need:
         buf = torch.zeros(need, dtype=torch.uint8, device=device)
-        entry = _scratch[key] = (need, buf.data_ptr(), buf)
+        entry = table[key] = (need, buf.data_ptr(), buf)
     return entry[1]
 
 
@@ -877,16 +893,192 @@ else:
                  efficientnet.MBConv: FusedMBConv}
 
 
+# Torch sums a tensor of fewer elements than this (2^31 bytes of bf16) in one launch of its reduce kernel, whose order
+# the squeeze-excitation kernels restate; a larger one it splits into 32-bit-indexed pieces.
+_SE_MAX_NUMEL = 2 ** 30
+
+
+class _SELink:
+    """What a squeeze-excitation site's scale backward hands its pool backward, which runs after the squeeze path's
+    backward: s, and dy (channels-last, for the elementwise kernel) or, for a gradient in another layout, eager
+    torch's dy * s.  It holds them only from the one backward to the other, and never s's graph: both Functions' ctx
+    keep the link, and s's grad_fn leads back to the pool's node through the squeeze path, so a graph-carrying tensor
+    on the link would close a cycle through C++ autograd edges that Python's collector cannot free."""
+
+    __slots__ = ("s", "dy", "xgrad")
+
+    def __init__(self):
+        self.s = self.dy = self.xgrad = None
+
+
+def _se_scratch_bytes(x, n, c, hw):
+    """The scratch a squeeze-excitation site of x's shape needs on x's device; 0 where the library takes no such site."""
+    key = (x.device.index, n, c, hw)
+    need = _se_need.get(key)
+    if need is None:
+        need = _se_need[key] = int(_native_lib().b200c_se_scratch_bytes(n, c, hw))
+    return need
+
+
+def _se_scratch_ptr(x, n, c, hw, stream):
+    """The scratch pointer and its size in bytes for a squeeze-excitation site of x's shape on `stream`."""
+    ptr = _scratch_ptr(x.device, stream, _se_scratch_bytes(x, n, c, hw), _se_scratch)
+    return ptr, _se_scratch[(x.device.index, stream)][0]
+
+
+def _se_like(t):
+    """A tensor like `t` (channels-last [N, C, H, W]) with the strides torch's elementwise ops give s * t or t * s:
+    channels-last, except over one row per sample, where every operand is also contiguous and so is the output."""
+    n, c, h, w = t.shape
+    return torch.empty_like(t) if h * w > 1 else torch.empty((n, c, 1, 1), dtype=t.dtype, device=t.device)
+
+
+class _SqueezePool(torch.autograd.Function):
+    """pooled = x.mean((-1, -2), keepdim=True), with the strides adaptive_avg_pool2d gives it.  The backward writes x's
+    whole gradient in one kernel: the mean's (gp / HW) plus the scale's (dy * s, which `link` carries)."""
+
+    @staticmethod
+    def forward(ctx, x, link):
+        n, c, h, w = x.shape
+        pooled = torch.empty((n, c, 1, 1), dtype=x.dtype, device=x.device)
+        # adaptive_avg_pool2d restrides the mean of a channels-last input, which it decides from x's strides
+        if h * w > 1 or torch._prims_common.suggest_memory_format(x) == torch.channels_last:
+            pooled = pooled.as_strided((n, c, 1, 1), (c, 1, c, c))
+        stream = _raw_stream(x.device.index)
+        scratch, size = _se_scratch_ptr(x, n, c, h * w, stream)
+        N.check(_native_lib().b200c_se_pool(x.data_ptr(), pooled.data_ptr(), n, c, h * w, scratch, size, stream))
+        ctx.shape, ctx.link = x.shape, link
+        ctx.set_materialize_grads(False)
+        return pooled
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gp):
+        link, shape = ctx.link, ctx.shape
+        dy, s, xgrad = link.dy, link.s, link.xgrad
+        link.dy = link.s = link.xgrad = None
+        n, c, h, w = shape
+        if gp is None or dy is None:
+            # eager torch's ops: the scale's gradient (if any) plus the mean's backward, added in place as autograd adds
+            if dy is not None:
+                xgrad = dy * s
+            if gp is None:
+                return xgrad, None
+            mean_grad = gp.expand(shape) / (h * w)
+            return (mean_grad if xgrad is None else xgrad.add_(mean_grad)), None
+        gp = gp.reshape(n, c).contiguous()
+        s2 = s.reshape(n, c).contiguous()
+        dx = _se_like(dy)
+        N.check(_native_lib().b200c_se_backward_elemt(dy.data_ptr(), s2.data_ptr(), gp.data_ptr(), dx.data_ptr(), n, c, h * w,
+                                                      _raw_stream(dy.device.index)))
+        return dx, None
+
+
+class _SqueezeScale(torch.autograd.Function):
+    """y = s * x for s of [N, C, 1, 1].  The backward writes s's gradient (the sum over H, W of dy * x, in torch's
+    order) and hands dy to the pool's backward through `link`, which writes x's gradient; where s needs no gradient
+    (the pool's backward may then never run) x's gradient is eager torch's dy * s here.
+
+    A gradient that arrives in another layout than channels-last makes eager torch's product and sum run in that layout,
+    whose reduction order differs; there the backward runs those torch ops."""
+
+    @staticmethod
+    def forward(ctx, s, x, link):
+        n, c, h, w = x.shape
+        y = _se_like(x)
+        s2 = s.reshape(n, c).contiguous()
+        N.check(_native_lib().b200c_se_scale(x.data_ptr(), s2.data_ptr(), y.data_ptr(), n, c, h * w, _raw_stream(x.device.index)))
+        ctx.link = link
+        ctx.save_for_backward(s, x)
+        ctx.set_materialize_grads(False)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None
+        s, x = ctx.saved_tensors
+        need_s, need_x = ctx.needs_input_grad[:2]
+        link = ctx.link
+        ds = dx = None
+        if not _activation(dy):
+            if need_s:
+                ds = (dy * x).sum_to_size(s.shape)
+            if need_x:
+                if need_s:
+                    link.xgrad = (dy * s).detach()
+                else:
+                    dx = dy * s
+            return ds, dx, None
+        n, c, h, w = x.shape
+        if need_s:
+            # sum_to's keepdim sum writes a contiguous [N, C, 1, 1]; over one row it returns the product itself, which is
+            # contiguous too (_se_like)
+            ds = torch.empty((n, c, 1, 1), dtype=dy.dtype, device=dy.device)
+            stream = _raw_stream(x.device.index)
+            scratch, size = _se_scratch_ptr(x, n, c, h * w, stream)
+            N.check(_native_lib().b200c_se_backward_reduce(dy.data_ptr(), x.data_ptr(), ds.data_ptr(), n, c, h * w, scratch, size,
+                                                           stream))
+        if need_x:
+            if need_s:
+                link.dy, link.s = dy.detach(), s.detach()
+            else:
+                dx = dy * s
+        return ds, dx, None
+
+
+def _se_ok(se, x):
+    """Whether squeeze-excitation module `se` can run its pool and scale on the kernels for input x: the conditions of
+    the module docstring."""
+    if not _activation(x) or x.numel() == 0 or x.numel() >= _SE_MAX_NUMEL:
+        return False
+    n, c, h, w = x.shape
+    if c == 1 and h * w > 1:   # torch reduces one channel along its fastest dimension, in another order
+        return False
+    pool = se.avgpool
+    if type(pool) is not nn.AdaptiveAvgPool2d or pool.output_size not in (1, (1, 1)) or _hooked(pool) or _global_hooks():
+        return False
+    return _se_scratch_bytes(x, n, c, h * w) > 0
+
+
+try:
+    from torchvision.ops.misc import SqueezeExcitation
+except ImportError:  # without torchvision there is nothing to rewrite
+    SqueezeExcitation = None
+else:
+
+    class FusedSqueezeExcitation(SqueezeExcitation):
+        """torchvision's SqueezeExcitation whose average pool and scale run on the squeeze-excitation kernels: the pool,
+        then fc1, activation, fc2 and scale_activation called as modules, then the scale.  Both writes and both
+        gradients of x (the scale's and the mean's) have eager torch's bits; the backward reads x and dy twice and
+        writes dx once.  Runs the parent's forward where the kernels do not apply (the module docstring), and torch's
+        `s * x` where the squeeze path returns anything but a bf16 [N, C, 1, 1] on x's device."""
+
+        def forward(self, input):
+            if not _se_ok(self, input):
+                return super().forward(input)
+            link = _SELink()
+            s = self.scale_activation(self.fc2(self.activation(self.fc1(_SqueezePool.apply(input, link)))))
+            n, c = input.shape[:2]
+            if not (isinstance(s, torch.Tensor) and s.dtype == torch.bfloat16 and s.device == input.device
+                    and s.shape == (n, c, 1, 1)):
+                return s * input
+            return _SqueezeScale.apply(s, input, link)
+
+
 def fuse_model(model):
     """Rewrite `model` in place: `fuse_resnet`, and every module whose class is exactly torchvision's
     Conv2dNormActivation and whose last module is an nn.ReLU6, SiLU or Hardswish (MobileNetV2 / V3, EfficientNet)
     becomes a FusedConv2dNormActivation.  Every module whose class is exactly torchvision's MobileNetV2 or MobileNetV3
     InvertedResidual or EfficientNet's MBConv gets the fused subclass, whose projection batch norm (with the stochastic
-    depth and residual add after it) runs as one bn_res site.  Parameters, buffers, state_dict keys, hooks and the
+    depth and residual add after it) runs as one bn_res site, and every SqueezeExcitation (exactly that class) inside such
+an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Parameters, buffers, state_dict keys, hooks and the
     object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
     training and in eval (see `fuse_resnet` for inference).
 
-    Blocks ending in nn.ReLU (MobileNetV3, RegNet) keep torchvision's forward: bn_act would run them on bn_relu's sites,
+    RegNet's squeeze-excitation and SqueezeExcitation modules outside those blocks keep torchvision's class.  Blocks
+    ending in nn.ReLU (MobileNetV3, RegNet) keep torchvision's forward: bn_act would run them on bn_relu's sites,
     but a regnet_y_400mf training step with them fused took about 11 ms more host time than the untouched model (DESIGN.md
     section 10), more than the kernel time they save."""
     fuse_resnet(model)
@@ -898,6 +1090,12 @@ def fuse_model(model):
         cls = _RES_SWAP.get(type(mod))
         if cls is not None:
             mod.__class__ = cls
+    if SqueezeExcitation is not None and _RES_SWAP:
+        for mod in model.modules():
+            if type(mod) in (FusedMBConv, FusedInvertedResidualV3):
+                for sub in mod.modules():
+                    if type(sub) is SqueezeExcitation:
+                        sub.__class__ = FusedSqueezeExcitation
     return model
 
 

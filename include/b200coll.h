@@ -431,6 +431,34 @@ int b200c_bn_backward_res(const void* dy, const void* noise, int rows_per_sample
 int b200c_bn_infer_res(const void* x, const void* identity, void* y, const void* weight, const void* bias, const void* running_mean,
                        const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
 
+/* ---- squeeze-and-excitation (torchvision's SqueezeExcitation without its squeeze path) ----
+ * Over channels-last bf16 activations x, y, dy, dx of n samples, hw = H * W rows per sample and `channels` channels
+ * ([n][hw][channels]), and bf16 per-sample vectors pooled, s, ds, gp of [n][channels]; bit-identical to eager torch:
+ *
+ * b200c_se_pool: pooled = x.mean((-1, -2)) = bf16(sum_hw float(x) * factor), factor = float(n * c) / (n * c * hw), summed
+ * in the order of torch's reduce kernel for that tensor: its launch follows from the shape, x's address and the
+ * current device's multiProcessorCount and maxThreadsPerMultiProcessor.  1 kernel.
+ * b200c_se_scale: y = bf16(float(s[n, c]) * float(x)).  1 kernel.
+ * b200c_se_backward_reduce: ds = bf16(sum_hw float(bf16(float(dy) * float(x)))), summed as torch sums a freshly allocated
+ * product tensor of x's shape (the gradient of s in y = s * x); with hw == 1 torch reduces nothing and ds is that
+ * product itself, -0.0 included.  1 kernel.
+ * b200c_se_backward_elemt: dx = bf16(float(bf16(float(dy) * float(s))) + float(bf16(float(gp) * (1 / float(hw))))), the
+ * gradient of x from y = s * x plus the mean's, gp being pooled's gradient.  1 kernel.
+ *
+ * n, channels, hw >= 1 with n * channels * hw < 2^31; the reducing calls also reject channels == 1 with hw > 1 (torch
+ * reduces that along the fastest dimension, another order).  Torch sums in one launch, the order restated here, up to
+ * 2^30 elements.  The reducing calls take `scratch` of at least b200c_se_scratch_bytes(n, channels, hw) bytes
+ * (`scratch_bytes` its size), zero-filled before its first use; every call leaves its semaphores at zero, so one buffer
+ * of the largest size serves every site on one stream.  b200c_se_scratch_bytes returns 0 for a bad shape.  Every
+ * argument is checked before the launch. */
+size_t b200c_se_scratch_bytes(int n, int channels, int hw);
+int b200c_se_pool(const void* x, void* pooled, int n, int channels, int hw, void* scratch, size_t scratch_bytes, b200c_stream_t stream);
+int b200c_se_scale(const void* x, const void* s, void* y, int n, int channels, int hw, b200c_stream_t stream);
+int b200c_se_backward_reduce(const void* dy, const void* x, void* ds, int n, int channels, int hw, void* scratch, size_t scratch_bytes,
+                             b200c_stream_t stream);
+int b200c_se_backward_elemt(const void* dy, const void* s, const void* gp, void* dx, int n, int channels, int hw,
+                            b200c_stream_t stream);
+
 /* Sync batch norm: torch.nn.SyncBatchNorm's training-mode forward and backward over the ranks of `comm`, with the
  * same fusions as the calls above, bit-identical to torch's sync functions (batch_norm_stats,
  * batch_norm_gather_stats_with_counts, batch_norm_elemt, batch_norm_backward_reduce, batch_norm_backward_elemt)

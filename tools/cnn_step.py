@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Training step and eval forward of torchvision CNNs whose batch norms sit in Conv2dNormActivation blocks
-(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, regnet_y_400mf), with and without `fused_norm.fuse_model`.
-The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model) and "act_only" (fuse_model without the
-inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused).
+(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf), with and without
+`fused_norm.fuse_model`.  The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model), "act_only"
+(fuse_model without the inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused) and
+"no_se" (fuse_model with the squeeze-excitation modules back on torchvision's class).
 
 Batch `--batch` (256) at 224 x 224, bf16 autocast with fp32 parameters, channels-last, SGD with momentum.  Per model,
 alternating the builds in one process, `--runs` times each, the order reversed every run (ABBA):
@@ -33,7 +34,7 @@ for _p in (ROOT, os.path.join(ROOT, "tools")):
 
 from step_profile import gpu_identity  # noqa: E402
 
-MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "regnet_y_400mf"]
+MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "efficientnet_v2_s", "regnet_y_400mf"]
 # first match wins
 FAMILIES = [
     ("bn_stats", r"k_bn_stats|batch_norm_collect_statistics"),
@@ -41,6 +42,8 @@ FAMILIES = [
                          r"|batch_norm_transform_input"),
     ("bn_bwd_reduce", r"k_act_bwd_reduce|k_res_bwd_reduce|k_bn_bwd_reduce|batch_norm_backward_reduce"),
     ("bn_bwd_elemt", r"k_act_bwd_elemt|k_bn_bwd_elemt|batch_norm_backward_elemt"),
+    ("se", r"b200c::se::k_se"),
+    ("torch_reduce", r"at::native::reduce_kernel"),   # torch's mean and sum (the squeeze-excitation's among them)
     ("torch_add_mul", r"CUDAFunctor_add|MulFunctor|bernoulli"),
     ("torch_act", r"silu|hardswish|hardsigmoid|clamp|hardtanh|threshold|relu"),
     ("conv", r"conv|cudnn|xmma|gemm|nvjet|cutlass|fprop|dgrad|wgrad|implicit_|nhwc|nchw|sm90_"),
@@ -90,8 +93,12 @@ def main():
         models = {}
         for b in builds:
             m = copy.deepcopy(base)
-            if b in ("fused", "act_only"):
+            if b in ("fused", "act_only", "no_se"):
                 fused_norm.fuse_model(m)
+            if b == "no_se":   # the squeeze-excitation sites back to torchvision's class
+                for mod in m.modules():
+                    if type(mod) is fused_norm.FusedSqueezeExcitation:
+                        mod.__class__ = fused_norm.SqueezeExcitation
             if b == "act_only":   # the projection sites' blocks back to torchvision's classes
                 parents = {cls: parent for parent, cls in fused_norm._RES_SWAP.items()}
                 for mod in m.modules():
@@ -138,6 +145,7 @@ def main():
         first = models[builds[0]]
         entry = {"builds": res, "act_sites": len([m for m in first.modules() if type(m) is fused_norm.FusedConv2dNormActivation and len(m) == 3]),
                  "res_sites": len([m for m in first.modules() if type(m) in fused_norm._RES_SWAP.values()]),
+                 "se_sites": len([m for m in first.modules() if type(m) is fused_norm.FusedSqueezeExcitation]),
                  "identical": {b: {"parameters": all(same(a, c) for a, c in zip(models[b].parameters(), first.parameters())),
                                    "buffers": all(same(a, c) for a, c in zip(models[b].buffers(), first.buffers()) if a.is_floating_point()),
                                    "eval_logits": same(forward(b), forward(builds[0]))} for b in builds[1:]}}

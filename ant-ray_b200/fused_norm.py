@@ -13,9 +13,18 @@ outputs, gradients and running statistics are bit-identical to eager torch.
 
 A site runs fused when it is in training mode, its input is a bf16 channels-last CUDA tensor with more than one
 value per channel, a channel stride of 1 and at most 131072 channels, its batch norm is
-a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum, and
-torch would run it on its native kernels (`torch._C._select_batch_norm_backend`).  Otherwise the block runs the
-parent class's ops, so the choice never changes a result.
+a plain `BatchNorm2d` with fp32 affine weight and bias, tracked running statistics and a numeric momentum,
+torch would run it on its native kernels (`torch._C._select_batch_norm_backend`), and the hook rule holds.
+Otherwise the block runs the parent class's ops, so the choice never changes a result.
+
+The hook rule, the same at every site of every kind below, training and eval, local and sync: the kernels replace
+the calls of the batch norm and of other modules (the ReLU or activation, the stem's max-pool, a downsample branch's
+Sequential and batch norm, an inverted-residual block's projection and stochastic depth, the squeeze-excitation's
+average pool), so a site runs on them only where none of those modules has a forward, forward-pre, backward or
+backward-pre hook and no global module hook is registered.  Otherwise the modules are called and every hook runs as
+in eager torch.  `_site` decides every batch-norm site: the hook rule, the other operands, then an eval site, a sync
+site or a local site.  The stem's max-pool and a downsample branch are checked for their own hooks with their shape
+and structure (`_pool_fusable`, `_downsample_bn`), before the site asks `_site`.
 
 Eval mode: where no gradient is recorded (`torch.no_grad()`, `torch.inference_mode()`, or nothing the site reads
 requires grad), the same four kinds of site run as one native launch each on the eval kernels, which read the
@@ -24,22 +33,22 @@ of eager torch's eval batch norm and the ReLU, add and max-pool after it.  A sit
 a `BatchNorm2d`, or a SyncBatchNorm (which torch does not synchronise in eval), in eval mode with running
 statistics and a positive eps; its weight, bias and running statistics are contiguous on the input's device and
 all fp32 or all bf16 (a model cast to bf16); the input is a non-empty bf16 channels-last CUDA tensor with a channel
-stride of 1 and fewer than 2^31 elements; torch would run it on its native kernels; and no hook of the batch norm,
-the ReLU or the global registry would be skipped.  Otherwise the site runs torch's ops.  With gradients recorded,
+stride of 1 and fewer than 2^31 elements; torch would run it on its native kernels; and the hook rule holds.
+Otherwise the site runs torch's ops.  With gradients recorded,
 eval runs the parent classes' forward.
 
 Conv2dNormActivation: `fuse_model` also swaps every torchvision `Conv2dNormActivation` that ends in an nn.ReLU6,
 nn.SiLU or nn.Hardswish (MobileNetV2 / V3, EfficientNet) for `FusedConv2dNormActivation`, whose batch norm and
 activation run as one site per direction (`bn_act`, norm_act.cuh): the forward writes act(bn(x)) with eager torch's
 bits, and the backward recomputes bn(x) from x instead of saving it.  `bn_act` runs nn.ReLU on the ReLU sites above.  The
-conditions are those above, with no hook on the batch norm or the activation; in eval without autograd recording the
-site is one launch.  A sync site with one of those activations runs the sync batch norm alone, then the activation.
+conditions are those above, the hook rule covering the activation; in eval without autograd recording the site is
+one launch.  A sync site with one of those activations runs the sync batch norm alone, then the activation.
 
 Inverted-residual blocks: `fuse_model` also swaps torchvision's MobileNetV2 / V3 `InvertedResidual` and
 EfficientNet's `MBConv` for subclasses whose projection batch norm (the 1x1 convolution's, without activation) runs
 with what follows it as one site per direction (`bn_res`, norm_res.cuh): nothing, the residual add, or EfficientNet's
 stochastic depth ("row" mode, its noise built by torchvision's own torch calls) and the add.  The conditions are those
-above, with no hook on the block's Sequential, the projection, its batch norm or the stochastic depth; in eval without
+above, the hook rule covering the block's Sequential, the projection and the stochastic depth; in eval without
 autograd recording the site is one launch.
 
 Squeeze-and-excitation: inside those swapped MBConv and MobileNetV3 blocks, `fuse_model` also swaps torchvision's
@@ -49,8 +58,8 @@ scale forward, and backward one reduce (s's gradient, the sum over H, W of dy * 
 writes x's whole gradient (dy * s plus the mean's gp / HW) once; without autograd recording, the two forward launches.
 The two sums keep the launch shape and order of torch's reduce kernel, so outputs and gradients are eager torch's bits.
 A site runs there when x is a non-empty bf16 channels-last CUDA tensor with a channel stride of 1, fewer than 2^30
-elements and not one channel over several rows, the module's avgpool is exactly an nn.AdaptiveAvgPool2d(1) without
-hooks, and no global module hook is registered; otherwise the parent's forward runs.  A squeeze path that returns
+elements and not one channel over several rows, the module's avgpool is exactly an nn.AdaptiveAvgPool2d(1), and the
+hook rule holds for it; otherwise the parent's forward runs.  A squeeze path that returns
 anything but a bf16 [N, C, 1, 1] on x's device gets torch's `s * x`, and a gradient that arrives in another layout
 than channels-last torch's backward ops.
 
@@ -60,7 +69,8 @@ more than one rank (a "sync site"), its statistics are gathered and its gradient
 communicator instead of torch's NCCL process group, with one native call per direction that also fuses the ReLU and
 the residual add at ResNet positions; the results have the bits of torch's SyncBatchNorm function (ranks folded in
 rank order).  Whether a site syncs depends only on the module and the input's layout, never on the rank's batch
-size, so every rank joins the same collectives: a rank with an empty batch still contributes its zero row.  A
+size, so every rank joins the same collectives: a rank with an empty batch still contributes its zero row.  Where
+the hook rule fails, the block calls the FusedSyncBatchNorm, whose own forward is the sync site without ReLU.  A
 SyncBatchNorm that torch would not synchronise (no process group, or one rank) runs the local fused site above,
 which is what torch's F.batch_norm computes.
 """
@@ -118,6 +128,52 @@ def _scratch_ptr(device, stream, need, table=_scratch):
     return entry[1]
 
 
+def _stream_scratch(x, comm=None, dual=False):
+    """The stream a training site's calls run on and its scratch there: the current stream and a local site's scratch
+    for x's channels (with `dual` a dual tail's), or with `comm` the communicator's stream and a sync site's scratch."""
+    if comm is not None:
+        stream = comm.stream().cuda_stream
+        return stream, _scratch_ptr(x.device, stream, _scratch_bytes(x.shape[1], comm.world_size))
+    stream = _raw_stream(x.device.index)
+    return stream, _scratch_ptr(x.device, stream, _scratch_bytes(x.shape[1], "dual" if dual else None))
+
+
+def _forward_args(x, bn, weight, bias, comm=None, dual=False):
+    """What every training site's forward call takes for its batch norm `bn`: the stats tensor it writes, [save_mean (C)
+    | save_invstd (C)] (followed at a sync site by norm_fct, the backward's 1 / rows of all ranks, whose statistics are
+    the global ones), the seven pointers weight, bias, running_mean, running_var, num_batches_tracked or None,
+    save_mean and save_invstd, and _stream_scratch's stream and scratch."""
+    c = x.shape[1]
+    stats = torch.empty(2 * c + (comm is not None), dtype=torch.float32, device=x.device)
+    mean = stats.data_ptr()
+    nbt = bn.num_batches_tracked
+    params = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+              nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c)
+    return (stats, params, *_stream_scratch(x, comm, dual))
+
+
+def _backward_args(x, comm=None, dual=False):
+    """What every training site's backward call writes for its batch norm of input x, dx, grad_weight and grad_bias,
+    and _stream_scratch's stream and scratch."""
+    c = x.shape[1]
+    return (torch.empty_like(x), torch.empty(c, dtype=torch.float32, device=x.device),
+            torch.empty(c, dtype=torch.float32, device=x.device), *_stream_scratch(x, comm, dual))
+
+
+def _torch_backward(g, x, weight, stats, eps):
+    """Eager torch's batch-norm backward (dx, grad_weight, grad_bias) of a training site for g, the gradient of its
+    output: the sites whose gradient arrives in another layout than channels-last run it, as eager torch then runs its
+    NCHW kernels, whose sums round differently.  The running statistics are not read in training mode."""
+    c = x.shape[1]
+    return torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, stats[:c], stats[c:], True, eps, [True, True, True])
+
+
+def _pooled_like(x):
+    """An empty channels-last output of the stem's nn.MaxPool2d(3, 2, 1) over x."""
+    n, c, h, w = x.shape
+    return torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+
+
 class _FusedBatchNorm(torch.autograd.Function):
     """relu(bn(x)) or, with `identity`, relu(bn(x) + identity) in training mode.
 
@@ -135,7 +191,6 @@ class _FusedBatchNorm(torch.autograd.Function):
         c = x.shape[1]
         m = x.numel() // c
         y = torch.empty_like(x)
-        nbt = bn.num_batches_tracked
         id_ptr = identity.data_ptr() if identity is not None else None
         ctx.residual = identity is not None
         ctx.comm, ctx.relu = comm, relu
@@ -145,24 +200,15 @@ class _FusedBatchNorm(torch.autograd.Function):
         masked = relu and c % 8 == 0
         relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if masked else y if relu else None
         mask_ptr = relu_src.data_ptr() if masked else None
-        # stats = [save_mean (c) | save_invstd (c)], followed at a sync site by norm_fct: there the statistics are the
-        # global ones and norm_fct is the backward's 1 / rows of all ranks
-        stats = torch.empty(2 * c + (comm is not None), dtype=torch.float32, device=x.device)
-        mean = stats.data_ptr()
-        params = (weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                  nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c)
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias, comm)
         if comm is not None:
-            stream = comm.stream().cuda_stream
-            scratch = _scratch_ptr(x.device, stream, _scratch_bytes(c, comm.world_size))
             N.check(lib.b200c_bn_sync_forward(comm._h(), x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, int(relu), *params,
-                                              mean + 8 * c, m, c, bn.momentum, bn.eps, scratch, stream))
+                                              stats.data_ptr() + 8 * c, m, c, bn.momentum, bn.eps, scratch, stream))
+        elif masked:
+            N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, *params, m, c, bn.momentum, bn.eps,
+                                              scratch, stream))
         else:
-            stream = _raw_stream(x.device.index)
-            site = (m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream)
-            if masked:
-                N.check(lib.b200c_bn_forward_mask(x.data_ptr(), id_ptr, y.data_ptr(), mask_ptr, *params, *site))
-            else:
-                N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *params, *site))
+            N.check(lib.b200c_bn_forward(x.data_ptr(), id_ptr, y.data_ptr(), *params, m, c, bn.momentum, bn.eps, scratch, stream))
         ctx.save_for_backward(x, relu_src, weight, stats)
         return (y, y.view_as(y)) if pair else y
 
@@ -180,10 +226,8 @@ class _FusedBatchNorm(torch.autograd.Function):
         lib = _native_lib()
         c = x.shape[1]
         m = x.numel() // c
-        dx = torch.empty_like(x)
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(x, comm)
         d_identity = torch.empty_like(x) if ctx.residual else None
-        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
-        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
         mean = stats.data_ptr()
         did_ptr = d_identity.data_ptr() if d_identity is not None else None
         # the forward's relu_src: the mask, y, or nothing
@@ -191,8 +235,6 @@ class _FusedBatchNorm(torch.autograd.Function):
         y = relu_src.data_ptr() if relu_src is not None and mask is None else None
         dy2 = grads[1].data_ptr() if len(grads) == 2 else None
         if comm is not None:
-            stream = comm.stream().cuda_stream
-            scratch = _scratch_ptr(x.device, stream, _scratch_bytes(c, comm.world_size))
             N.check(lib.b200c_bn_sync_backward(comm._h(), grads[0].data_ptr(), dy2, y, mask, int(ctx.relu), x.data_ptr(),
                                                did_ptr, dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, mean + 8 * c,
                                                grad_weight.data_ptr(), grad_bias.data_ptr(), m, c, scratch, stream))
@@ -200,9 +242,8 @@ class _FusedBatchNorm(torch.autograd.Function):
                 # as torch's SyncBatchNorm: no gradient for an empty input, nor for weight and bias from this rank
                 return None, d_identity, None, None, None, None, None, None
             return dx, d_identity, grad_weight, grad_bias, None, None, None, None
-        stream = _raw_stream(x.device.index)
         site = (x.data_ptr(), did_ptr, dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
-                grad_bias.data_ptr(), m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream)
+                grad_bias.data_ptr(), m, c, scratch, stream)
         if mask is not None:
             N.check(lib.b200c_bn_backward_mask(grads[0].data_ptr(), dy2, mask, *site))
         else:
@@ -218,26 +259,18 @@ class _FusedBatchNormDual(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, x_ds, weight, bias, weight_ds, bias_ds, bn, bn_ds, pair):
-        lib = _native_lib()
         c = x.shape[1]
         m = x.numel() // c
         y = torch.empty_like(x)
         ctx.set_materialize_grads(False)
         masked = c % 8 == 0
         relu_src = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device) if masked else y
-        # [save_mean | save_invstd] of bn, then of bn_ds
-        stats = torch.empty(4 * c, dtype=torch.float32, device=x.device)
-        mean = stats.data_ptr()
-        nbt, nbt_ds = bn.num_batches_tracked, bn_ds.num_batches_tracked
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_forward_dual(
-            x.data_ptr(), x_ds.data_ptr(), y.data_ptr(), relu_src.data_ptr() if masked else None,
-            weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-            nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, bn.momentum, bn.eps,
-            weight_ds.data_ptr(), bias_ds.data_ptr(), bn_ds.running_mean.data_ptr(), bn_ds.running_var.data_ptr(),
-            nbt_ds.data_ptr() if nbt_ds is not None else None, mean + 8 * c, mean + 12 * c, bn_ds.momentum, bn_ds.eps,
-            m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c, "dual")), stream))
-        ctx.save_for_backward(x, x_ds, relu_src, weight, weight_ds, stats)
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias, dual=True)
+        stats_ds, params_ds, _, _ = _forward_args(x_ds, bn_ds, weight_ds, bias_ds, dual=True)
+        N.check(_native_lib().b200c_bn_forward_dual(x.data_ptr(), x_ds.data_ptr(), y.data_ptr(), relu_src.data_ptr() if masked else None,
+                                                    *params, bn.momentum, bn.eps, *params_ds, bn_ds.momentum, bn_ds.eps, m, c,
+                                                    scratch, stream))
+        ctx.save_for_backward(x, x_ds, relu_src, weight, weight_ds, stats, stats_ds)
         return (y, y.view_as(y)) if pair else y
 
     @staticmethod
@@ -246,21 +279,17 @@ class _FusedBatchNormDual(torch.autograd.Function):
         grads = [g.contiguous(memory_format=torch.channels_last) for g in grads if g is not None]
         if not grads:
             return (None,) * 9
-        x, x_ds, relu_src, weight, weight_ds, stats = ctx.saved_tensors
-        lib = _native_lib()
+        x, x_ds, relu_src, weight, weight_ds, stats, stats_ds = ctx.saved_tensors
         c = x.shape[1]
-        m = x.numel() // c
-        dx, dx_ds = torch.empty_like(x), torch.empty_like(x_ds)
-        dw, db, dw_ds, db_ds = (torch.empty(c, dtype=torch.float32, device=x.device) for _ in range(4))
-        mean = stats.data_ptr()
+        dx, dw, db, stream, scratch = _backward_args(x, dual=True)
+        dx_ds, dw_ds, db_ds, _, _ = _backward_args(x_ds, dual=True)
+        mean, mean_ds = stats.data_ptr(), stats_ds.data_ptr()
         masked = relu_src.dtype == torch.uint8
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_backward_dual(
+        N.check(_native_lib().b200c_bn_backward_dual(
             grads[0].data_ptr(), grads[1].data_ptr() if len(grads) == 2 else None, None if masked else relu_src.data_ptr(),
             relu_src.data_ptr() if masked else None, x.data_ptr(), x_ds.data_ptr(), dx.data_ptr(), dx_ds.data_ptr(),
-            weight.data_ptr(), mean, mean + 4 * c, dw.data_ptr(), db.data_ptr(), weight_ds.data_ptr(), mean + 8 * c,
-            mean + 12 * c, dw_ds.data_ptr(), db_ds.data_ptr(), m, c, _scratch_ptr(x.device, stream, _scratch_bytes(c, "dual")),
-            stream))
+            weight.data_ptr(), mean, mean + 4 * c, dw.data_ptr(), db.data_ptr(), weight_ds.data_ptr(), mean_ds, mean_ds + 4 * c,
+            dw_ds.data_ptr(), db_ds.data_ptr(), x.numel() // c, c, scratch, stream))
         return dx, dx_ds, dw, db, dw_ds, db_ds, None, None, None
 
 
@@ -271,19 +300,12 @@ class _FusedBatchNormPool(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, bn):
-        lib = _native_lib()
         n, c, h, w = x.shape
-        y = torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device,
-                        memory_format=torch.channels_last)
+        y = _pooled_like(x)
         argmax = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)
-        nbt = bn.num_batches_tracked
-        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
-        mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_forward_pool(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), weight.data_ptr(), bias.data_ptr(),
-                                          bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                                          nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, n, h, w, c,
-                                          bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias)
+        N.check(_native_lib().b200c_bn_forward_pool(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), *params, n, h, w, c,
+                                                    bn.momentum, bn.eps, scratch, stream))
         ctx.save_for_backward(x, argmax, weight, stats)
         return y
 
@@ -294,17 +316,13 @@ class _FusedBatchNormPool(torch.autograd.Function):
             return None, None, None, None
         dy = dy.contiguous(memory_format=torch.channels_last)
         x, argmax, weight, stats = ctx.saved_tensors
-        lib = _native_lib()
         n, c, h, w = x.shape
         g = torch.empty_like(x)
-        dx = torch.empty_like(x)
-        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
-        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(x)
         mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_backward_pool(dy.data_ptr(), argmax.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(),
-                                           weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(),
-                                           n, h, w, c, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        N.check(_native_lib().b200c_bn_backward_pool(dy.data_ptr(), argmax.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(),
+                                                     weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
+                                                     grad_bias.data_ptr(), n, h, w, c, scratch, stream))
         return dx, grad_weight, grad_bias, None
 
 
@@ -325,17 +343,11 @@ class _FusedBatchNormAct(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, bn, code):
-        lib = _native_lib()
         c = x.shape[1]
-        m = x.numel() // c
         y = torch.empty_like(x)
-        nbt = bn.num_batches_tracked
-        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
-        mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_forward_act(x.data_ptr(), y.data_ptr(), weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(),
-                                         bn.running_var.data_ptr(), nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c,
-                                         code, m, c, bn.momentum, bn.eps, _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias)
+        N.check(_native_lib().b200c_bn_forward_act(x.data_ptr(), y.data_ptr(), *params, code, x.numel() // c, c, bn.momentum, bn.eps,
+                                                   scratch, stream))
         ctx.code, ctx.eps = code, bn.eps
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(x, weight, bias, stats)
@@ -348,23 +360,15 @@ class _FusedBatchNormAct(torch.autograd.Function):
             return None, None, None, None, None
         x, weight, bias, stats = ctx.saved_tensors
         c = x.shape[1]
-        m = x.numel() // c
         if not dy.is_contiguous(memory_format=torch.channels_last):
-            mean, invstd = stats[:c], stats[c:]
-            t = torch.batch_norm_elemt(x, weight, bias, mean, invstd, ctx.eps)
-            g = _ACT_BACKWARD[ctx.code](dy, t)
-            # the running statistics are not read in training mode
-            return (*torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, mean, invstd, True, ctx.eps,
-                                                               [True, True, True]), None, None)
-        lib = _native_lib()
-        g, dx = torch.empty_like(x), torch.empty_like(x)
-        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
-        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+            t = torch.batch_norm_elemt(x, weight, bias, stats[:c], stats[c:], ctx.eps)
+            return (*_torch_backward(_ACT_BACKWARD[ctx.code](dy, t), x, weight, stats, ctx.eps), None, None)
+        g = torch.empty_like(x)
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(x)
         mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_backward_act(dy.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(), weight.data_ptr(), bias.data_ptr(), mean,
-                                          mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), ctx.code, m, c,
-                                          _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        N.check(_native_lib().b200c_bn_backward_act(dy.data_ptr(), x.data_ptr(), g.data_ptr(), dx.data_ptr(), weight.data_ptr(),
+                                                    bias.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(),
+                                                    ctx.code, x.numel() // c, c, scratch, stream))
         return dx, grad_weight, grad_bias, None, None
 
 
@@ -379,19 +383,12 @@ class _FusedBatchNormRes(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, identity, weight, bias, bn, noise):
-        lib = _native_lib()
         c = x.shape[1]
-        m = x.numel() // c
         y = torch.empty_like(x)
-        nbt = bn.num_batches_tracked
-        stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
-        mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_forward_res(x.data_ptr(), identity.data_ptr() if identity is not None else None,
-                                         noise.data_ptr() if noise is not None else None, x.shape[2] * x.shape[3], y.data_ptr(),
-                                         weight.data_ptr(), bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                                         nbt.data_ptr() if nbt is not None else None, mean, mean + 4 * c, m, c, bn.momentum, bn.eps,
-                                         _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias)
+        N.check(_native_lib().b200c_bn_forward_res(x.data_ptr(), identity.data_ptr() if identity is not None else None,
+                                                   noise.data_ptr() if noise is not None else None, x.shape[2] * x.shape[3],
+                                                   y.data_ptr(), *params, x.numel() // c, c, bn.momentum, bn.eps, scratch, stream))
         ctx.residual, ctx.eps = identity is not None, bn.eps
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(x, weight, stats, noise)
@@ -404,25 +401,17 @@ class _FusedBatchNormRes(torch.autograd.Function):
             return None, None, None, None, None, None
         x, weight, stats, noise = ctx.saved_tensors
         c = x.shape[1]
-        m = x.numel() // c
         d_identity = dy if ctx.residual else None
         if not dy.is_contiguous(memory_format=torch.channels_last):
-            g = dy * noise if noise is not None else dy
-            # the running statistics are not read in training mode
-            dx, grad_weight, grad_bias = torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, stats[:c], stats[c:], True,
-                                                                                   ctx.eps, [True, True, True])
+            dx, grad_weight, grad_bias = _torch_backward(dy * noise if noise is not None else dy, x, weight, stats, ctx.eps)
             return dx, d_identity, grad_weight, grad_bias, None, None
-        lib = _native_lib()
-        dx = torch.empty_like(x)
         g = torch.empty_like(x) if noise is not None else None
-        grad_weight = torch.empty(c, dtype=torch.float32, device=x.device)
-        grad_bias = torch.empty(c, dtype=torch.float32, device=x.device)
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(x)
         mean = stats.data_ptr()
-        stream = _raw_stream(x.device.index)
-        N.check(lib.b200c_bn_backward_res(dy.data_ptr(), noise.data_ptr() if noise is not None else None, x.shape[2] * x.shape[3],
-                                          x.data_ptr(), g.data_ptr() if g is not None else None, dx.data_ptr(), weight.data_ptr(), mean,
-                                          mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), m, c,
-                                          _scratch_ptr(x.device, stream, _scratch_bytes(c)), stream))
+        N.check(_native_lib().b200c_bn_backward_res(dy.data_ptr(), noise.data_ptr() if noise is not None else None,
+                                                    x.shape[2] * x.shape[3], x.data_ptr(), g.data_ptr() if g is not None else None,
+                                                    dx.data_ptr(), weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
+                                                    grad_bias.data_ptr(), x.numel() // c, c, scratch, stream))
         return dx, d_identity, grad_weight, grad_bias, None, None
 
 
@@ -449,18 +438,8 @@ def _module_ok(bn):
                for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
 
 
-def _relu_fusable(bn, relu):
-    return type(relu) is nn.ReLU and not bn._forward_hooks and not bn._forward_pre_hooks
-
-
-def _fusable(bn, relu, x):
-    """Whether this site can run fused as a local site: the conditions of the module docstring.  A site that cannot
-    falls back to the parent class's ops."""
-    return _relu_fusable(bn, relu) and _local_ok(bn, x)
-
-
 def _local_ok(bn, x):
-    """_fusable's conditions on the batch norm and its input."""
+    """_site's conditions of a local training site on the batch norm and its input."""
     local = type(bn) is nn.BatchNorm2d or (isinstance(bn, nn.SyncBatchNorm) and not _torch_syncs(bn))
     if not local or not _module_ok(bn):
         return False
@@ -475,19 +454,8 @@ def _local_ok(bn, x):
 _PARAM_DTYPES = ({torch.float32}, {torch.bfloat16})
 
 
-def _infer_ok(bn, relu, x, *operands):
-    """Whether this site can run as an eval site (the module docstring's conditions): `operands` are the other tensors
-    the kernel reads (the identity), which must not require grad either."""
-    return type(relu) is nn.ReLU and not _skips_hooks(bn, relu) and _infer_bn_ok(bn, x, *operands)
-
-
-def _skips_hooks(bn, act):
-    """Whether calling a kernel instead of `bn` and `act` would skip a hook: theirs or the global registry's."""
-    return _hooked(bn) or _hooked(act) or _global_hooks()
-
-
 def _infer_bn_ok(bn, x, *operands):
-    """_infer_ok's conditions on the batch norm and its input."""
+    """_site's conditions of an eval site on the batch norm and its input: `operands` must not require grad either."""
     # eps <= 0 stays on torch, whose F.batch_norm raises for it
     if bn.training or not (type(bn) is nn.BatchNorm2d or isinstance(bn, nn.SyncBatchNorm)) or not bn.eps > 0:
         return False
@@ -507,13 +475,11 @@ def _infer_params(bn):
             int(bn.weight.dtype == torch.bfloat16))
 
 
-def _infer(bn, x, identity=None):
-    """relu(bn(x)) or relu(bn(x) + identity) of an eval site, in one native launch."""
-    y = torch.empty_like(x)
-    c = x.shape[1]
-    N.check(_native_lib().b200c_bn_infer(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
-                                         *_infer_params(bn), bn.eps, x.numel() // c, c,
-                                         _raw_stream(x.device.index)))
+def _infer(bn, x, launch, pooled=False):
+    """The output y of an eval site's one native launch: like x, or with `pooled` the stem's pooled output.
+    `launch(y, params, stream)` makes the C-ABI call from y's pointer, _infer_params(bn) and the current stream."""
+    y = _pooled_like(x) if pooled else torch.empty_like(x)
+    N.check(launch(y.data_ptr(), _infer_params(bn), _raw_stream(x.device.index)))
     return y
 
 
@@ -537,15 +503,54 @@ def _sync_comm(bn, x):
     return comm
 
 
+def _hooked(mod):
+    return bool(mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks)
+
+
+def _global_hooks():
+    from torch.nn.modules import module
+
+    return bool(module._global_forward_hooks or module._global_forward_pre_hooks or module._global_backward_hooks
+                or module._global_backward_pre_hooks)
+
+
+def _skips_hooks(*mods):
+    """Whether calling kernels in place of the modules `mods` would skip a hook: one of theirs or a global one."""
+    return any(map(_hooked, mods)) or _global_hooks()
+
+
+# how a batch-norm site runs (_site), besides the communicator of a sync site and None for the modules' own ops
+_EVAL, _LOCAL = "eval", "local"
+
+
+def _site(bn, x, mods=(), operands=(), sync=True):
+    """How the site of batch norm `bn` on input x runs, by the module docstring's conditions: _EVAL (one launch on the
+    eval kernels), _LOCAL (a local training site), the communicator of a sync site, or None: the modules run.  `mods`
+    are the other modules whose calls the kernels replace, `operands` the other tensors they read (the identity).
+    Where the entry point has no sync form (`sync` False), a sync batch norm gets None and runs its own module forward,
+    FusedSyncBatchNorm's sync site."""
+    if _skips_hooks(bn, *mods):
+        return None
+    for t in operands:
+        # _rows: an eval or local site has rows, and so then has an operand of x's shape, where _rows is _activation
+        if t.shape != x.shape or t.device != x.device or not _rows(t):
+            return None
+    if _infer_bn_ok(bn, x, *operands):
+        return _EVAL
+    comm = _sync_comm(bn, x)
+    if comm is not None:
+        return comm if sync else None
+    return _LOCAL if _local_ok(bn, x) else None
+
+
 def bn_relu(bn, relu, x):
     """relu(bn(x)), fused when the site allows it."""
-    if _infer_ok(bn, relu, x):
-        return _infer(bn, x)
-    comm = _sync_comm(bn, x)
-    if comm is not None and _relu_fusable(bn, relu):
-        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, comm, True)
-    if comm is None and _fusable(bn, relu, x):
-        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False)
+    site = _site(bn, x, (relu,)) if type(relu) is nn.ReLU else None
+    if site is _EVAL:
+        c = x.shape[1]
+        return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer(x.data_ptr(), None, y, *p, bn.eps, x.numel() // c, c, s))
+    if site is not None:
+        return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, None if site is _LOCAL else site, True)
     return relu(bn(x))
 
 
@@ -556,20 +561,16 @@ _ACT_CODES = {nn.ReLU6: N.ACT_RELU6, nn.SiLU: N.ACT_SILU, nn.Hardswish: N.ACT_HA
 def bn_act(bn, act, x):
     """act(bn(x)) for `act` an nn.ReLU, nn.ReLU6, nn.SiLU or nn.Hardswish (exactly those classes), fused when the site
     allows it: ReLU through bn_relu (its sync sites included); for the others an eval site, else a local training
-    site, with the conditions of bn_relu's and no hook on `act`.  A sync site with another activation runs the
-    batch norm's own forward (FusedSyncBatchNorm's sync site) and then `act`; anything else runs `act(bn(x))`."""
+    site.  A sync site with another activation runs the batch norm's own forward (FusedSyncBatchNorm's sync site) and
+    then `act`; anything else runs `act(bn(x))`."""
     if type(act) is nn.ReLU:
         return bn_relu(bn, act, x)
     code = _ACT_CODES.get(type(act))
-    if code is None or _skips_hooks(bn, act):
-        return act(bn(x))
-    if _infer_bn_ok(bn, x):
-        y = torch.empty_like(x)
+    site = _site(bn, x, (act,), sync=False) if code is not None else None
+    if site is _EVAL:
         c = x.shape[1]
-        N.check(_native_lib().b200c_bn_infer_act(x.data_ptr(), y.data_ptr(), *_infer_params(bn), bn.eps, code, x.numel() // c, c,
-                                                 _raw_stream(x.device.index)))
-        return y
-    if _sync_comm(bn, x) is None and _local_ok(bn, x):
+        return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_act(x.data_ptr(), y, *p, bn.eps, code, x.numel() // c, c, s))
+    if site is _LOCAL:
         return _FusedBatchNormAct.apply(x, bn.weight, bn.bias, bn, code)
     return act(bn(x))
 
@@ -583,18 +584,15 @@ def _noise_ok(noise, x):
 def bn_res(bn, x, identity=None, noise=None):
     """`bn(x)`, `bn(x) + identity`, or with `noise` (torchvision's stochastic depth noise in "row" mode, [N, 1, 1, 1])
     `bn(x) * noise + identity`, with eager torch's bits, fused when the site allows it: an eval site (no noise) in one
-    launch, else a local training site, with the conditions of bn_relu's and no hook on `bn`.  Noise needs an identity.
-    Anything else runs the modules' ops."""
-    operands = () if identity is None else (identity,)
-    site = (not _hooked(bn) and not _global_hooks() and (noise is None or (identity is not None and _noise_ok(noise, x)))
-            and all(_activation(t) and t.shape == x.shape and t.device == x.device for t in operands))
-    if site and noise is None and _infer_bn_ok(bn, x, *operands):
-        y = torch.empty_like(x)
+    launch, else a local training site.  Noise needs an identity.  Anything else runs the modules' ops."""
+    site = None
+    if noise is None or (identity is not None and _noise_ok(noise, x)):
+        site = _site(bn, x, operands=() if identity is None else (identity,), sync=False)
+    if site is _EVAL and noise is None:
         c = x.shape[1]
-        N.check(_native_lib().b200c_bn_infer_res(x.data_ptr(), identity.data_ptr() if identity is not None else None, y.data_ptr(),
-                                                 *_infer_params(bn), bn.eps, x.numel() // c, c, _raw_stream(x.device.index)))
-        return y
-    if site and _sync_comm(bn, x) is None and _local_ok(bn, x):
+        id_ptr = identity.data_ptr() if identity is not None else None
+        return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_res(x.data_ptr(), id_ptr, y, *p, bn.eps, x.numel() // c, c, s))
+    if site is _LOCAL:
         return _FusedBatchNormRes.apply(x, identity, bn.weight, bn.bias, bn, noise)
     out = bn(x)
     if noise is not None:
@@ -603,25 +601,22 @@ def bn_res(bn, x, identity=None, noise=None):
 
 
 def _pool_fusable(pool):
-    """Whether `pool` is exactly nn.MaxPool2d(3, 2, 1) (dilation 1, floor mode, no indices) and calling the kernel
-    instead of the module skips no hook."""
+    """Whether the stem kernel can replace `pool`'s call: `pool` is exactly nn.MaxPool2d(3, 2, 1) (dilation 1, floor
+    mode, no indices) without a hook of its own (the site's `_site` checks the global ones)."""
     two = lambda v, k: v in (k, (k, k))  # noqa: E731
     return (type(pool) is nn.MaxPool2d and two(pool.kernel_size, 3) and two(pool.stride, 2) and two(pool.padding, 1)
-            and two(pool.dilation, 1) and not pool.ceil_mode and not pool.return_indices and not _hooked(pool)
-            and not _global_hooks())
+            and two(pool.dilation, 1) and not pool.ceil_mode and not pool.return_indices and not _hooked(pool))
 
 
 def bn_relu_maxpool(bn, relu, pool, x):
-    """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) and the batch norm can run as a local
-    fused site; otherwise bn_relu and the module call."""
-    if _pool_fusable(pool) and _infer_ok(bn, relu, x):
+    """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) and the batch norm can run as an
+    eval or a local training site; otherwise bn_relu and the module call."""
+    site = _site(bn, x, (relu,), sync=False) if type(relu) is nn.ReLU and _pool_fusable(pool) else None
+    if site is _EVAL:
         n, c, h, w = x.shape
-        y = torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device,
-                        memory_format=torch.channels_last)
-        N.check(_native_lib().b200c_bn_infer_pool(x.data_ptr(), y.data_ptr(), *_infer_params(bn), bn.eps, n, h, w, c,
-                                                  _raw_stream(x.device.index)))
-        return y
-    if _pool_fusable(pool) and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
+        return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_pool(x.data_ptr(), y, *p, bn.eps, n, h, w, c, s),
+                      pooled=True)
+    if site is _LOCAL:
         return _FusedBatchNormPool.apply(x, bn.weight, bn.bias, bn)
     return pool(bn_relu(bn, relu, x))
 
@@ -629,15 +624,14 @@ def bn_relu_maxpool(bn, relu, pool, x):
 def bn_add_relu(bn, relu, x, identity, pair=False):
     """`out = bn(x); out += identity; relu(out)`, fused when the site allows it.  With `pair`, returns `(out,
     out_id)`: the same values, whose gradients a fused site receives apart and sums in its backward kernel."""
-    if _infer_ok(bn, relu, x, identity) and _activation(identity) and identity.shape == x.shape and identity.device == x.device:
-        out = _infer(bn, x, identity)
+    site = _site(bn, x, (relu,), (identity,)) if type(relu) is nn.ReLU else None
+    if site is _EVAL:
+        c = x.shape[1]
+        out = _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer(x.data_ptr(), identity.data_ptr(), y, *p, bn.eps,
+                                                                          x.numel() // c, c, s))
         return (out, out) if pair else out
-    comm = _sync_comm(bn, x)
-    if comm is not None:
-        if _relu_fusable(bn, relu) and _rows(identity) and identity.shape == x.shape:
-            return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair, comm, True)
-    elif _fusable(bn, relu, x) and _activation(identity) and identity.shape == x.shape:
-        return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair)
+    if site is not None:
+        return _FusedBatchNorm.apply(x, identity, bn.weight, bn.bias, bn, pair, None if site is _LOCAL else site, True)
     out = bn(x)
     out += identity
     out = relu(out)
@@ -646,10 +640,9 @@ def bn_add_relu(bn, relu, x, identity, pair=False):
 
 def _downsample_bn(ds):
     """The batch norm of a downsample branch that a dual tail can run: `ds` exactly nn.Sequential(nn.Conv2d, batch
-    norm), where calling the convolution and the kernel instead of the two modules skips no hook; else None."""
-    if type(ds) is not nn.Sequential or len(ds) != 2 or type(ds[0]) is not nn.Conv2d or _global_hooks():
-        return None
-    if _hooked(ds) or _hooked(ds[1]):
+    norm), neither the Sequential nor the batch norm with a hook of its own (the site's `_site` checks the global
+    ones); else None."""
+    if type(ds) is not nn.Sequential or len(ds) != 2 or type(ds[0]) is not nn.Conv2d or _hooked(ds) or _hooked(ds[1]):
         return None
     return ds[1]
 
@@ -660,35 +653,21 @@ def bn_add_relu_downsample(bn, relu, x, downsample, x_id, pair=False):
     one native call per direction (in eval, one launch) and the branch's output is never written; otherwise
     bn_add_relu."""
     bn_ds = _downsample_bn(downsample)
-    if bn_ds is not None and bn_ds is not bn and _infer_ok(bn, relu, x):
-        x_ds = downsample[0](x_id)
-        if x_ds.shape == x.shape and _infer_ok(bn_ds, relu, x_ds) and bn_ds.weight.dtype == bn.weight.dtype:
-            y = torch.empty_like(x)
-            c = x.shape[1]
-            ptrs, ptrs_ds = _infer_params(bn)[:4], _infer_params(bn_ds)[:4]
-            N.check(_native_lib().b200c_bn_infer_dual(x.data_ptr(), x_ds.data_ptr(), y.data_ptr(), *ptrs, bn.eps, *ptrs_ds, bn_ds.eps,
-                                                      int(bn.weight.dtype == torch.bfloat16), x.numel() // c, c,
-                                                      _raw_stream(x.device.index)))
-            return (y, y) if pair else y
-        return bn_add_relu(bn, relu, x, bn_ds(x_ds), pair)
-    if bn_ds is not None and bn_ds is not bn and _sync_comm(bn, x) is None and _fusable(bn, relu, x):
-        x_ds = downsample[0](x_id)
-        if (x_ds.shape == x.shape and _sync_comm(bn_ds, x_ds) is None and _fusable(bn_ds, relu, x_ds)
-                and _scratch_bytes(x.shape[1], "dual")):
-            return _FusedBatchNormDual.apply(x, x_ds, bn.weight, bn.bias, bn_ds.weight, bn_ds.bias, bn, bn_ds, pair)
-        return bn_add_relu(bn, relu, x, bn_ds(x_ds), pair)
-    return bn_add_relu(bn, relu, x, downsample(x_id), pair)
-
-
-def _hooked(mod):
-    return bool(mod._forward_hooks or mod._forward_pre_hooks or mod._backward_hooks or mod._backward_pre_hooks)
-
-
-def _global_hooks():
-    from torch.nn.modules import module
-
-    return bool(module._global_forward_hooks or module._global_forward_pre_hooks or module._global_backward_hooks
-                or module._global_backward_pre_hooks)
+    site = None
+    if bn_ds is not None and bn_ds is not bn and type(relu) is nn.ReLU:
+        site = _site(bn, x, (relu,), sync=False)
+    if site is None:
+        return bn_add_relu(bn, relu, x, downsample(x_id), pair)
+    x_ds = downsample[0](x_id)
+    site_ds = _site(bn_ds, x_ds, sync=False) if x_ds.shape == x.shape else None
+    if site is _EVAL and site_ds is _EVAL and bn_ds.weight.dtype == bn.weight.dtype:
+        c = x.shape[1]
+        out = _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_dual(
+            x.data_ptr(), x_ds.data_ptr(), y, *p[:4], bn.eps, *_infer_params(bn_ds)[:4], bn_ds.eps, p[4], x.numel() // c, c, s))
+        return (out, out) if pair else out
+    if site is _LOCAL and site_ds is _LOCAL and _scratch_bytes(x.shape[1], "dual"):
+        return _FusedBatchNormDual.apply(x, x_ds, bn.weight, bn.bias, bn_ds.weight, bn_ds.bias, bn, bn_ds, pair)
+    return bn_add_relu(bn, relu, x, bn_ds(x_ds), pair)
 
 
 try:
@@ -763,6 +742,8 @@ class FusedSyncBatchNorm(nn.SyncBatchNorm):
     b200_comm = None
 
     def forward(self, x):
+        # _site's sync step alone: the module call has run this module's hooks and replaces no other module, and this
+        # is where every other site with a sync batch norm that runs its modules joins the collectives
         comm = _sync_comm(self, x)
         if comm is None:
             return super().forward(x)
@@ -839,14 +820,18 @@ def _res_forward(block, seq, nested, x, identity, sd=None):
         return None
     if nested:
         last = seq[-1]
-        if type(last) is not Conv2dNormActivation or len(last) != 2 or _hooked(last):
+        if type(last) is not Conv2dNormActivation or len(last) != 2:
             return None
-        head, conv, bn = list(seq)[:-1], last[0], last[1]
+        head, conv, bn, mods = list(seq)[:-1], last[0], last[1], [seq, last]
     else:
-        head, conv, bn = list(seq)[:-2], seq[-2], seq[-1]
-    if type(conv) is not nn.Conv2d or type(bn) is not nn.BatchNorm2d or _hooked(seq) or _hooked(bn) or _global_hooks():
+        head, conv, bn, mods = list(seq)[:-2], seq[-2], seq[-1], [seq]
+    if type(conv) is not nn.Conv2d or type(bn) is not nn.BatchNorm2d:
         return None
-    if sd is not None and (type(sd) is not StochasticDepth or sd.mode != "row" or not 0.0 <= sd.p <= 1.0 or _hooked(sd)):
+    if sd is not None:
+        if type(sd) is not StochasticDepth or sd.mode != "row" or not 0.0 <= sd.p <= 1.0:
+            return None
+        mods.append(sd)
+    if _skips_hooks(bn, *mods):
         return None
     out = x
     for mod in head:
@@ -1037,7 +1022,7 @@ def _se_ok(se, x):
     if c == 1 and h * w > 1:   # torch reduces one channel along its fastest dimension, in another order
         return False
     pool = se.avgpool
-    if type(pool) is not nn.AdaptiveAvgPool2d or pool.output_size not in (1, (1, 1)) or _hooked(pool) or _global_hooks():
+    if type(pool) is not nn.AdaptiveAvgPool2d or pool.output_size not in (1, (1, 1)) or _skips_hooks(pool):
         return False
     return _se_scratch_bytes(x, n, c, h * w) > 0
 

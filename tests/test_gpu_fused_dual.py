@@ -215,7 +215,7 @@ def test_above_the_dual_limit_the_downsample_batch_norm_runs_on_torch():
 
 
 # ---- whole blocks: the dual tail and its fallbacks -----------------------------------------------------------
-@pytest.mark.parametrize("case", ["nonstandard_downsample", "hooked_downsample_bn", "hooked_downsample"])
+@pytest.mark.parametrize("case", ["nonstandard_downsample", "hooked_downsample_bn", "hooked_downsample", "hooked_relu"])
 def test_other_downsamples_fall_back_with_the_same_bits(case):
     pytest.importorskip("torchvision")
     import test_gpu_fused_resnet as R
@@ -223,18 +223,32 @@ def test_other_downsamples_fall_back_with_the_same_bits(case):
 
     base = R.make_model("resnet50").cuda().to(memory_format=CL)
     ds = base.layer2[0].downsample
+    seen = []
     if case == "nonstandard_downsample":
         base.layer2[0].downsample = nn.Sequential(ds[0], ds[1], nn.Identity())
     elif case == "hooked_downsample_bn":
         ds[1].register_forward_hook(lambda mod, args, out: None)
-    else:
+    elif case == "hooked_downsample":
         ds.register_forward_pre_hook(lambda mod, args: None)
+    else:
+        # the block's ReLU module, called after each of its three batch norms; the copies below share the hook
+        base.layer2[0].relu.register_forward_hook(lambda mod, args, out: seen.append(mod))
     data = R.batches()
     ref = copy.deepcopy(base)
     want = R.train_steps(ref, data)
     fused = train.prepare_model(copy.deepcopy(base), parallel_strategy=None)
-    assert fused_norm._downsample_bn(fused.layer2[0].downsample) is None
-    assert fused_norm._downsample_bn(fused.layer3[0].downsample) is not None
-    # the fallback tail is the same 4 launches and the downsample batch norm runs on torch
-    got = R.train_steps(fused, data, per_step_launches=4 * R.SITES["resnet50"])
+    block, other = fused.layer2[0], fused.layer3[0]
+    if case == "hooked_relu":
+        # a plain downsample, but the tail also replaces the hooked ReLU's call
+        assert fused_norm._downsample_bn(block.downsample) is not None and fused_norm._skips_hooks(block.relu)
+    else:
+        assert fused_norm._downsample_bn(block.downsample) is None
+    assert fused_norm._downsample_bn(other.downsample) is not None
+    # the fallback tail is the same 4 launches and the downsample batch norm runs on torch; a hooked ReLU leaves the
+    # block's three sites on torch
+    sites = R.SITES["resnet50"] - (3 if case == "hooked_relu" else 0)
+    got = R.train_steps(fused, data, per_step_launches=4 * sites)
     R.assert_same_training(got, want, fused, ref)
+    if case == "hooked_relu":
+        calls = [sum(m is relu for m in seen) for relu in (ref.layer2[0].relu, block.relu)]
+        assert calls[0] > 0 and calls[1] == calls[0], calls

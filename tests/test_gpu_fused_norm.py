@@ -4,8 +4,9 @@ For every distinct batch-norm shape of ResNet-50, at batch 256 and 32, and for a
 a single-row grid, a partial channel tile and the scalar elementwise path): `BatchNorm2d` -> ReLU and
 `BatchNorm2d` -> `+= identity` -> ReLU on bf16 channels-last inputs, forward and backward.  The output, the
 running statistics, num_batches_tracked and the gradients of the input, the identity, the weight and the bias must
-have the same bits as eager torch's.  Sites that must not run fused (eval mode, fp32, NCHW) fall back without a
-native launch.
+have the same bits as eager torch's.  Sites that must not run fused (eval mode, fp32, NCHW, a hook on the ReLU, a
+full backward hook on the batch norm, a global module hook) fall back without a native launch, and call each hook as
+often as eager torch does.
 
 Beyond those shapes: one site per launch regime of the reducing kernels (gpu_common.BN_REGIME_SHAPES), operands
 whose data pointer is off the 16-byte grid (scalar elementwise kernels), an output gradient in NCHW layout, C = 1
@@ -412,7 +413,7 @@ def test_two_streams_with_their_own_scratch():
             assert same_bits(got[k], want[k]), k
 
 
-@pytest.mark.parametrize("case", ["eval", "fp32", "nchw"])
+@pytest.mark.parametrize("case", ["eval", "fp32", "nchw", "relu_hook", "bn_backward_hook", "global_hook"])
 def test_ineligible_sites_fall_back_to_torch(case):
     n, c, h, w = 8, 64, 14, 14
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -420,16 +421,55 @@ def test_ineligible_sites_fall_back_to_torch(case):
     fmt = torch.contiguous_format if case == "nchw" else CL
     x = torch.randn(n, c, h, w, device="cuda", generator=g).to(dtype).contiguous(memory_format=fmt)
     identity = torch.randn(n, c, h, w, device="cuda", generator=g).to(dtype).contiguous(memory_format=fmt)
+    dy = torch.randn(n, c, h, w, device="cuda", generator=g).to(dtype).contiguous(memory_format=fmt)
     ref_bn = make_bn(c, 1)
     fused_bn = copy.deepcopy(ref_bn)
     if case == "eval":
         ref_bn.eval()
         fused_bn.eval()
-    relu = nn.ReLU()
-    before = N.launch_count()
-    got = fused_norm.bn_add_relu(fused_bn, relu, x, identity)
-    assert N.launch_count() == before, "an ineligible site ran the fused kernels"
-    out = ref_bn(x)
-    out += identity
-    assert same_bits(got, relu(out))
+    ref_relu, fused_relu = nn.ReLU(), nn.ReLU()
+    calls = {"fused": 0, "ref": 0}
+    side = "fused"
+
+    def hook(*args):
+        calls[side] += 1
+
+    # hooks on each side's own modules (the global one sees both): training sites with a hook run torch's modules,
+    # which call it as often as eager torch does
+    handles = []
+    if case == "relu_hook":
+        handles = [r.register_forward_hook(hook) for r in (ref_relu, fused_relu)]
+    elif case == "bn_backward_hook":
+        handles = [b.register_full_backward_hook(hook) for b in (ref_bn, fused_bn)]
+    elif case == "global_hook":
+        handles = [torch.nn.modules.module.register_module_forward_hook(hook)]
+    hooked = bool(handles)
+
+    def site(bn, relu, t):
+        # torch forbids `+= identity` on the output of a module with a full backward hook: that case takes the ReLU site
+        return fused_norm.bn_relu(bn, relu, t) if case == "bn_backward_hook" else fused_norm.bn_add_relu(bn, relu, t, identity)
+
+    xf, xr = x.clone().requires_grad_(hooked), x.clone().requires_grad_(hooked)
+    try:
+        before = N.launch_count()
+        got = site(fused_bn, fused_relu, xf)
+        if hooked:
+            got.backward(dy)
+        torch.cuda.synchronize()
+        assert N.launch_count() == before, "an ineligible site ran the fused kernels"
+        side = "ref"
+        out = ref_bn(xr)
+        if case != "bn_backward_hook":
+            out += identity
+        want = ref_relu(out)
+        if hooked:
+            want.backward(dy)
+    finally:
+        for handle in handles:
+            handle.remove()
+    assert same_bits(got, want)
     assert same_bits(fused_bn.running_mean, ref_bn.running_mean) and same_bits(fused_bn.running_var, ref_bn.running_var)
+    if hooked:
+        assert calls["ref"] > 0 and calls["fused"] == calls["ref"], calls
+        for a, b in ((xf.grad, xr.grad), (fused_bn.weight.grad, ref_bn.weight.grad), (fused_bn.bias.grad, ref_bn.bias.grad)):
+            assert same_bits(a, b)

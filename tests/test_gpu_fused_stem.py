@@ -270,27 +270,45 @@ def test_resnet50_trace_runs_every_batch_norm_and_the_max_pool_natively():
 
 
 # ---- whole models: the fused stem and its fallbacks -------------------------------------------------------
-@pytest.mark.parametrize("case", ["ceil_mode", "hooked_pool", "padding_0"])
+@pytest.mark.parametrize("case", ["ceil_mode", "hooked_pool", "padding_0", "hooked_relu", "global_hook"])
 def test_other_maxpools_fall_back_with_the_same_bits(case):
     pytest.importorskip("torchvision")
     import test_gpu_fused_resnet as R
     from ant_ray_b200 import train
 
     base = R.make_model("resnet18").cuda().to(memory_format=CL)
+    seen = []
+    hook = lambda mod, args, out: seen.append(mod)  # noqa: E731
     if case == "ceil_mode":
         base.maxpool = nn.MaxPool2d(3, 2, 1, ceil_mode=True)
     elif case == "padding_0":
         base.maxpool = nn.MaxPool2d(3, 2, 0)
-    else:
+    elif case == "hooked_pool":
         base.maxpool.register_forward_hook(lambda mod, args, out: None)
+    elif case == "hooked_relu":
+        base.relu.register_forward_hook(hook)   # the stem's ReLU (each BasicBlock has its own); the copies share it
     data = R.batches()
     ref = copy.deepcopy(base)
-    want = R.train_steps(ref, data)
     fused = train.prepare_model(copy.deepcopy(base), parallel_strategy=None)
-    assert not fused_norm._pool_fusable(fused.maxpool)
-    # the stem runs as bn_relu: the same 4 launches per site
-    got = R.train_steps(fused, data, per_step_launches=4 * R.SITES["resnet18"])
+    # the stem runs as bn_relu, the same 4 launches per site, or with a hook on its ReLU on torch; with a global hook
+    # every site runs on torch
+    sites = {"hooked_relu": R.SITES["resnet18"] - 1, "global_hook": 0}.get(case, R.SITES["resnet18"])
+    handle = torch.nn.modules.module.register_module_forward_hook(hook) if case == "global_hook" else None
+    try:
+        if case in ("hooked_relu", "global_hook"):
+            # the ResNet max-pool, but the stem site also replaces the ReLU's call, whose hooks would be skipped
+            assert fused_norm._pool_fusable(fused.maxpool) and fused_norm._skips_hooks(fused.relu)
+        else:
+            assert not fused_norm._pool_fusable(fused.maxpool)
+        want = R.train_steps(ref, data)
+        calls_ref, seen[:] = len(seen), []
+        got = R.train_steps(fused, data, per_step_launches=4 * sites)
+    finally:
+        if handle is not None:
+            handle.remove()
     R.assert_same_training(got, want, fused, ref)
+    if case in ("hooked_relu", "global_hook"):
+        assert calls_ref > 0 and len(seen) == calls_ref, (len(seen), calls_ref)
 
 
 def test_fused_stem_trains_bit_identically_at_odd_input_sizes():

@@ -33,9 +33,9 @@ CL = torch.channels_last
 KINDS = ["relu", "tail", "tail2", "plain"]
 # Sites where the batch norm runs alone (its module forward) and torch's ops follow in place on its output: a
 # SyncBatchNorm followed by an inplace ReLU, and the fused blocks' fallbacks when the batch norm has a forward hook
-# (`relu(bn(x))` and `out = bn(x); out += identity; relu(out)` with the block's inplace ReLU).  Each is checked
-# against the reference of the site it computes.
-INPLACE_KINDS = {"seq_inplace_relu": "relu", "hooked_relu": "relu", "hooked_tail": "tail"}
+# (`relu(bn(x))` and `out = bn(x); out += identity; relu(out)` with the block's inplace ReLU) or the ReLU has one
+# (`relu(bn(x))`, the hook called on every rank).  Each is checked against the reference of the site it computes.
+INPLACE_KINDS = {"seq_inplace_relu": "relu", "hooked_relu": "relu", "hooked_tail": "tail", "hooked_relu_module": "relu"}
 GUARD = 64 << 10
 
 
@@ -146,6 +146,7 @@ def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=(), misalign_ranks=
     bns = [fused_norm.sync_batch_norm(copy.deepcopy(bn), world.comms[r]) for r in range(W)]
     relu = nn.ReLU(inplace=True)
     results = [None] * W
+    hook_ranks = []
     # inputs that require grad are leaves made on the current stream before the ranks' streams start
     # (an empty input keeps its own strides: see test_empty_rank_input_from_a_convolution)
     off = lambda r: misalign_ranks is None or r in misalign_ranks  # noqa: E731
@@ -173,6 +174,10 @@ def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=(), misalign_ranks=
         elif kind == "hooked_tail":
             bnr.register_forward_hook(lambda *a: None)
             outs, gs = [fused_norm.bn_add_relu(bnr, relu, xs[r], ids[r], pair=True)[0]], [dys[r]]
+        elif kind == "hooked_relu_module":
+            hooked = nn.ReLU(inplace=True)
+            hooked.register_forward_hook(lambda *a: hook_ranks.append(r))
+            outs, gs = [fused_norm.bn_relu(bnr, hooked, xs[r])], [dys[r]]
         else:
             outs, gs = [bnr(xs[r])], [dys[r]]
         torch.autograd.backward(outs, gs)
@@ -183,6 +188,8 @@ def run_native(world, bn, xs, ids, dys, dy2s, kind, misalign=(), misalign_ranks=
     torch.cuda.synchronize()
     launched = N.launch_count() - before
     world.check()
+    if kind == "hooked_relu_module":
+        assert sorted(hook_ranks) == list(range(W)), hook_ranks
     got = []
     for r in range(W):
         res = {"y": results[r].detach(), "dx": xs[r].grad, "dweight": bns[r].weight.grad, "dbias": bns[r].bias.grad,

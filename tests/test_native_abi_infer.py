@@ -69,7 +69,7 @@ def bn_infer_argument_checks():
 def test_a_training_or_cpu_site_is_not_an_eval_site():
     bn, relu = nn.BatchNorm2d(8), nn.ReLU()
     x = torch.zeros(2, 8, 4, 4, dtype=torch.bfloat16).contiguous(memory_format=torch.channels_last)
-    assert not fused_norm._infer_ok(bn, relu, x)           # training mode
+    assert fused_norm._site(bn, x, (relu,)) is not fused_norm._EVAL           # training mode
     bn.eval()
-    assert not fused_norm._infer_ok(bn, relu, x)           # a CPU tensor
-    assert not fused_norm._infer_ok(nn.BatchNorm2d(8, track_running_stats=False).eval(), relu, x)
+    assert fused_norm._site(bn, x, (relu,)) is not fused_norm._EVAL           # a CPU tensor
+    assert fused_norm._site(nn.BatchNorm2d(8, track_running_stats=False).eval(), x, (relu,)) is not fused_norm._EVAL

@@ -188,3 +188,24 @@ def test_prepare_model_attaches_a_norm_comm_only_for_world_sync_batch_norm(monke
     assert not made
     comm = T._attach_sync_norm(converted, cuda, 2)
     assert made == [cuda] and type(converted[1]) is fused_norm.FusedSyncBatchNorm and converted[1].b200_comm is comm
+
+
+def register_hook(mod, kind):
+    if kind == "global":
+        return torch.nn.modules.module.register_module_forward_hook(lambda *a: None)
+    return getattr(mod, f"register_{kind}_hook")(lambda *a: None)
+
+
+@pytest.mark.parametrize("kind", ["forward", "forward_pre", "full_backward", "full_backward_pre", "global"])
+def test_a_hook_on_any_replaced_module_keeps_the_modules(cpu_rows, kind):
+    # one rule at local and sync sites alike: any hook on the batch norm or on a module whose call the kernels replace
+    relu, x = nn.ReLU(), act(4)
+    for bn in (nn.BatchNorm2d(64), sync_bn()):
+        want = fused_norm._LOCAL if type(bn) is nn.BatchNorm2d else bn.b200_comm
+        for mod in (bn, relu):
+            assert fused_norm._site(bn, x, (relu,)) is want
+            h = register_hook(mod, kind)
+            assert fused_norm._site(bn, x, (relu,)) is None, (type(bn).__name__, type(mod).__name__)
+            h.remove()
+    # an entry point without a sync form leaves a sync batch norm to its own module forward
+    assert fused_norm._site(sync_bn(), x, (relu,), sync=False) is None

@@ -12,6 +12,7 @@
 #include <unistd.h>
 
 #include <atomic>
+#include <initializer_list>
 #include <mutex>
 
 #include "byte_kernels.cuh"
@@ -1746,6 +1747,70 @@ extern "C" int b200c_bn_infer_res(const void* x, const void* identity, void* y, 
   if (rc) return rc;
   if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer res: null buffer");
   RT(bn::infer_res({x, identity, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0},
+                   (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
+// A batch norm and ReLU over a channel concatenation (norm_cat.cuh): the shape (m >= 2 in training: torch's batch norm
+// takes more than one value per channel, and the running variance's m / (m - 1) needs it), the segment table, and
+// the 16-byte grid of every segment and of the whole-tensor operands `grid`.
+static int check_cat(const char* site, int min_m, int m, int c, const void* const* segs, const int* seg_channels, int nsegs,
+                     std::initializer_list<const void*> grid) {
+  if (m < min_m || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX) return fail(B200C_EINVAL, "%s: bad shape m=%d c=%d", site, m, c);
+  if (nsegs < 1 || nsegs > bn::kMaxCatSegs) return fail(B200C_EINVAL, "%s: nsegs=%d outside 1..%d", site, nsegs, bn::kMaxCatSegs);
+  if (!segs || !seg_channels) return fail(B200C_EINVAL, "%s: null segment table", site);
+  int64_t total = 0;
+  for (int s = 0; s < nsegs; s++) {
+    if (!segs[s]) return fail(B200C_EINVAL, "%s: segment %d is null", site, s);
+    if (seg_channels[s] < 8 || seg_channels[s] % 8) return fail(B200C_EINVAL, "%s: segment %d has %d channels, not a positive multiple of 8", site, s, seg_channels[s]);
+    if (reinterpret_cast<uintptr_t>(segs[s]) % 16) return fail(B200C_EINVAL, "%s: segment %d is off the 16-byte grid", site, s);
+    total += seg_channels[s];
+  }
+  if (total != c) return fail(B200C_EINVAL, "%s: the segments' channels sum to %lld, not channels=%d", site, (long long)total, c);
+  for (const void* p : grid)
+    if (reinterpret_cast<uintptr_t>(p) % 16) return fail(B200C_EINVAL, "%s: y, dy or dx is off the 16-byte grid", site);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_cat(const void* const* segs, const int* seg_channels, int nsegs, void* y, uint8_t* mask,
+                                    const float* weight, const float* bias, float* running_mean, float* running_var,
+                                    int64_t* num_batches_tracked, float* save_mean, float* save_invstd, int m, int channels,
+                                    float momentum, float eps, void* scratch, b200c_stream_t stream) {
+  if (!y || !mask || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !scratch)
+    return fail(B200C_EINVAL, "batch norm cat forward: null buffer");
+  int rc = check_cat("batch norm cat", 2, m, channels, segs, seg_channels, nsegs, {y});
+  if (rc) return rc;
+  const bn::FwdArgs a{nullptr, nullptr, y, mask, true, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  RT(bn::forward_cat({segs, seg_channels, nsegs}, a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_cat(const void* dy, const uint8_t* mask, const void* const* segs, const int* seg_channels, int nsegs,
+                                     void* dx, const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
+                                     float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream) {
+  if (!dy || !mask || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias || !scratch)
+    return fail(B200C_EINVAL, "batch norm cat backward: null buffer");
+  int rc = check_cat("batch norm cat", 2, m, channels, segs, seg_channels, nsegs, {dy, dx});
+  if (rc) return rc;
+  const bn::BwdArgs a{dy, nullptr, nullptr, mask, nullptr, nullptr, dx, true, weight, save_mean, save_invstd, nullptr, grad_weight,
+                      grad_bias, m, channels, scratch};
+  RT(bn::backward_cat({segs, seg_channels, nsegs}, a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_cat(const void* const* segs, const int* seg_channels, int nsegs, void* y, const void* weight,
+                                  const void* bias, const void* running_mean, const void* running_var, int param_bf16, float eps, int m,
+                                  int channels, b200c_stream_t stream) {
+  if (!y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer cat: null buffer");
+  int rc = check_infer("batch norm infer cat", param_bf16, m, channels);
+  if (!rc) rc = check_cat("batch norm infer cat", 1, m, channels, segs, seg_channels, nsegs, {y});
+  if (rc) return rc;
+  RT(bn::infer_cat({segs, seg_channels, nsegs}, {nullptr, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false,
+                                                 param_bf16 != 0, m, channels, 0, 0},
                    (cudaStream_t)stream));
   g_launches.fetch_add(1);
   return B200C_OK;

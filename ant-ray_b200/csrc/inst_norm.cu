@@ -1,10 +1,11 @@
-// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh); argument
+// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh); argument
 // checking lives in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
 
 #include "norm_act.cuh"
+#include "norm_cat.cuh"
 #include "norm_infer.cuh"
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
@@ -269,6 +270,12 @@ cudaError_t load_kernels() {
   auto load = [&](auto kernel) { if (kernel && e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel); };
   load(&k_bn_sync_merge);
   load(res_bwd_reduce_kernel());
+  load(&bn_cat::k_cat_stats);
+  load(&bn_cat::k_cat_transform);
+  load(&bn_cat::k_cat_bwd_reduce);
+  load(&bn_cat::k_cat_bwd_elemt);
+  load(&bn_cat::k_cat_infer<float>);
+  load(&bn_cat::k_cat_infer<bf16>);
   for (int src = 0; src < kGradSrcs; src++) {
     load(bwd_reduce_kernel(src, false));
     load(bwd_reduce_kernel(src, true));
@@ -680,6 +687,74 @@ cudaError_t sync_bwd_reduce(const BwdArgs& a, cudaStream_t st) {
 }
 
 cudaError_t sync_bwd_elemt(const BwdArgs& a, cudaStream_t st) { return a.m == 0 ? cudaSuccess : launch_bwd_elemt(a, st); }
+
+// ---- batch norm and ReLU over a channel concatenation (norm_cat.cuh) ----
+// Each launch takes its bn:: counterpart's vector launch shape for the concatenation's m and c: the caller has
+// checked every segment (C_s % 8 == 0, 16-byte grid) and the outputs onto the 16-byte grid, which is what vec_ok
+// decides for a tensor of c % 8 == 0.
+static bn_cat::CatSegs cat_segs(const CatSegments& in) {
+  bn_cat::CatSegs t{};
+  int c = 0;
+  for (int s = 0; s < in.n; s++) {
+    t.ptr[s] = static_cast<const bf16*>(in.ptrs[s]);
+    t.c0[s] = c;
+    c += in.channels[s];
+  }
+  t.c0[in.n] = c;
+  t.n = in.n;
+  return t;
+}
+
+cudaError_t forward_cat(const CatSegments& in, const FwdArgs& a, cudaStream_t st) {
+  const bn_cat::CatSegs segs = cat_segs(in);
+  Scratch s = carve(a.scratch, a.c);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  block.x /= kStatsVec;
+  StatsOut o{a.save_mean, a.save_invstd, a.running_mean, a.running_var, a.num_batches_tracked, a.momentum,
+             (float)((double)a.m / (double)(a.m - 1)), a.eps};
+  bn_cat::k_cat_stats<<<grid, block, stats_ring_bytes(block), st>>>(segs, o, s.staging, s.semaphores, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  bn_cat::k_cat_transform<<<grid, block, 0, st>>>(segs, static_cast<bf16*>(a.y), static_cast<uint8_t*>(a.mask), a.save_mean,
+                                                  a.save_invstd, a.weight, a.bias, a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t backward_cat(const CatSegments& in, const BwdArgs& a, cudaStream_t st) {
+  const bn_cat::CatSegs segs = cat_segs(in);
+  Scratch s = carve(a.scratch, a.c);
+  const void* ptrs[1] = {a.dy};
+  const BwdReduceLaunch l = bwd_reduce_launch(a.m, a.c, kGradBits, false, false, ptrs, 1);
+  if (l.vec != kBwdVec) return kNoKernel;
+  bn_cat::k_cat_bwd_reduce<<<l.grid, l.block, l.smem, st>>>(segs, static_cast<const bf16*>(a.dy), static_cast<const uint8_t*>(a.mask),
+                                                            a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight,
+                                                            a.grad_bias, s.staging, s.semaphores, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  dim3 block, grid;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  bn_cat::k_cat_bwd_elemt<<<grid, block, 0, st>>>(segs, static_cast<const bf16*>(a.dy), static_cast<const uint8_t*>(a.mask),
+                                                  static_cast<bf16*>(a.dx), a.save_mean, a.save_invstd, a.weight, s.sums, s.sums + a.c,
+                                                  (float)(1.0 / a.m), a.m, a.c);
+  return cudaGetLastError();
+}
+
+template <typename P>
+static cudaError_t launch_infer_cat(const CatSegments& in, const InferArgs& a, cudaStream_t st) {
+  dim3 block, grid;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  const InferParams& b = a.bn;
+  bn_cat::k_cat_infer<P><<<grid, block, 0, st>>>(cat_segs(in), static_cast<bf16*>(a.y), static_cast<const P*>(b.running_mean),
+                                                 static_cast<const P*>(b.running_var), static_cast<const P*>(b.weight),
+                                                 static_cast<const P*>(b.bias), b.eps, a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_cat(const CatSegments& in, const InferArgs& a, cudaStream_t st) {
+  return a.param_bf16 ? launch_infer_cat<bf16>(in, a, st) : launch_infer_cat<float>(in, a, st);
+}
 
 }  // namespace bn
 }  // namespace b200c

@@ -123,5 +123,21 @@ cudaError_t forward_res(const FwdArgs& a, const void* noise, int rows_per_sample
 cudaError_t backward_res(const BwdArgs& a, const void* noise, int rows_per_sample, cudaStream_t s);
 cudaError_t infer_res(const InferArgs& a, cudaStream_t s);
 
+// Batch norm followed by ReLU over the channel concatenation of `n` channels-last segments, read in place (norm_cat.cuh):
+// segment s is bf16 [m][channels[s]], channels[s] % 8 == 0, on the 16-byte grid, and the segments' channels sum to
+// the site's c.  A local training site: the forward reads FwdArgs without x, identity or stem and writes y and the
+// mask (2 kernels); the backward reads BwdArgs.dy and .mask instead of .x, .dy2, .y or .dy_masked, and writes the whole
+// [m][c] dx (2 kernels).  The eval site reads InferArgs without x, identity, downsample or stem (1 kernel).
+// densenet201's last block concatenates 49 segments.
+constexpr int kMaxCatSegs = 64;
+struct CatSegments {
+  const void* const* ptrs;
+  const int* channels;
+  int n;
+};
+cudaError_t forward_cat(const CatSegments& segs, const FwdArgs& a, cudaStream_t s);
+cudaError_t backward_cat(const CatSegments& segs, const BwdArgs& a, cudaStream_t s);
+cudaError_t infer_cat(const CatSegments& segs, const InferArgs& a, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

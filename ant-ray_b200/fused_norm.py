@@ -1,6 +1,6 @@
-"""Fused batch norm for the training step and eval forward of ResNets and of torchvision's Conv2dNormActivation blocks
-(libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh), and the squeeze-and-excitation of
-EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
+"""Fused batch norm for the training step and eval forward of ResNets, DenseNets and torchvision's Conv2dNormActivation
+blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh), and the
+squeeze-and-excitation of EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
 by nothing (a downsample branch).  In bf16 training torch runs the first two kinds as separate memory-bound
@@ -63,6 +63,16 @@ hook rule holds for it; otherwise the parent's forward runs.  A squeeze path tha
 anything but a bf16 [N, C, 1, 1] on x's device gets torch's `s * x`, and a gradient that arrives in another layout
 than channels-last torch's backward ops.
 
+DenseNet: `fuse_model` also swaps torchvision's `_DenseLayer`, `_DenseBlock` and `DenseNet` for subclasses whose
+`relu(bn(torch.cat(features, 1)))` sites (each dense layer's norm1 / relu1, each transition's norm / relu, and norm5
+with DenseNet's functional ReLU) run as concatenation sites (`bn_relu_cat`, norm_cat.cuh) that read the earlier feature
+maps where they lie: no concatenation is written or saved, and each feature map's gradient is its channels of the
+one dx the backward writes, as torch's CatBackward hands them out.  The site runs where every segment is a bf16
+channels-last CUDA tensor with a channel stride of 1, a multiple of 8 channels and a data pointer on the 16-byte grid,
+alike in N, H, W and device, at most 64 of them, and the batch norm, decided on a tensor of the concatenation's shape
+and layout, is an eval or a local site by the rules above; anything else, a sync site included, runs torch.cat and
+bn_relu.  Each norm2 / relu2 is a bn_relu site and the stem a bn_relu_maxpool site.
+
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
 more than one rank (a "sync site"), its statistics are gathered and its gradient sums reduced over that
@@ -74,11 +84,13 @@ the hook rule fails, the block calls the FusedSyncBatchNorm, whose own forward i
 SyncBatchNorm that torch would not synchronise (no process group, or one rank) runs the local fused site above,
 which is what torch's F.batch_norm computes.
 """
+import ctypes
 import numbers
 
 import torch
 import torch.distributed as dist
 import torch.nn as nn
+import torch.nn.functional as F
 from torch.autograd.function import once_differentiable
 
 from . import _native as N
@@ -523,19 +535,20 @@ def _skips_hooks(*mods):
 _EVAL, _LOCAL = "eval", "local"
 
 
-def _site(bn, x, mods=(), operands=(), sync=True):
+def _site(bn, x, mods=(), operands=(), sync=True, inputs=()):
     """How the site of batch norm `bn` on input x runs, by the module docstring's conditions: _EVAL (one launch on the
     eval kernels), _LOCAL (a local training site), the communicator of a sync site, or None: the modules run.  `mods`
     are the other modules whose calls the kernels replace, `operands` the other tensors they read (the identity).
     Where the entry point has no sync form (`sync` False), a sync batch norm gets None and runs its own module forward,
-    FusedSyncBatchNorm's sync site."""
+    FusedSyncBatchNorm's sync site.  `inputs` are the tensors x stands for (a concatenation's segments): an eval site
+    must not record a gradient for them either."""
     if _skips_hooks(bn, *mods):
         return None
     for t in operands:
         # _rows: an eval or local site has rows, and so then has an operand of x's shape, where _rows is _activation
         if t.shape != x.shape or t.device != x.device or not _rows(t):
             return None
-    if _infer_bn_ok(bn, x, *operands):
+    if _infer_bn_ok(bn, x, *operands, *inputs):
         return _EVAL
     comm = _sync_comm(bn, x)
     if comm is not None:
@@ -552,6 +565,96 @@ def bn_relu(bn, relu, x):
     if site is not None:
         return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, None if site is _LOCAL else site, True)
     return relu(bn(x))
+
+
+# the most segments a concatenation site takes (the library's kMaxCatSegs)
+_MAX_CAT_SEGS = 64
+
+
+def _cat_segments_ok(features):
+    """Whether a concatenation site can read `features` in place: 1..64 segments, each passing _activation with the
+    first one's N, H, W and device, a multiple of 8 channels and a data pointer on the 16-byte grid."""
+    if not 1 <= len(features) <= _MAX_CAT_SEGS:
+        return False
+    f0 = features[0]
+    n, _, h, w = f0.shape if f0.dim() == 4 else (None,) * 4
+    for t in features:
+        if not _activation(t) or t.device != f0.device or t.shape[0] != n or t.shape[2] != h or t.shape[3] != w:
+            return False
+        if t.shape[1] % 8 or t.data_ptr() % 16:
+            return False
+    return True
+
+
+def _cat_table(features):
+    """The C-ABI's segment table of `features`: pointers, channels and their count."""
+    k = len(features)
+    return ((ctypes.c_void_p * k)(*(t.data_ptr() for t in features)), (ctypes.c_int * k)(*(t.shape[1] for t in features)), k)
+
+
+class _FusedBatchNormCat(torch.autograd.Function):
+    """relu(bn(torch.cat(features, 1))) in training mode, reading the segments where they lie: no concatenation is
+    written, and the segments themselves (not a copy) are saved for the backward.  The forward writes y and the ReLU's
+    mask bits; the backward writes the whole dx once and returns each segment's gradient as the view
+    dx.narrow(1, c0, C_s), as torch's CatBackward does, so autograd accumulates each feature map's gradients as it
+    would in eager torch."""
+
+    @staticmethod
+    def forward(ctx, y, weight, bias, bn, *features):
+        # y: the empty output, of the concatenation's shape and layout
+        n, c, h, w = y.shape
+        m = n * h * w
+        mask = torch.empty(m * c // 8, dtype=torch.uint8, device=y.device)
+        stats, params, stream, scratch = _forward_args(y, bn, weight, bias)
+        N.check(_native_lib().b200c_bn_forward_cat(*_cat_table(features), y.data_ptr(), mask.data_ptr(), *params, m, c, bn.momentum,
+                                                   bn.eps, scratch, stream))
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(mask, weight, stats, *features)
+        ctx.mark_dirty(y)   # the output buffer the site was decided on, written here
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        mask, weight, stats, *features = ctx.saved_tensors
+        if dy is None:
+            return (None,) * (4 + len(features))
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        n, c, h, w = dy.shape
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(dy)
+        mean = stats.data_ptr()
+        N.check(_native_lib().b200c_bn_backward_cat(dy.data_ptr(), mask.data_ptr(), *_cat_table(features), dx.data_ptr(),
+                                                    weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
+                                                    grad_bias.data_ptr(), n * h * w, c, scratch, stream))
+        grads, c0 = [], 0
+        for t in features:
+            grads.append(dx.narrow(1, c0, t.shape[1]))
+            c0 += t.shape[1]
+        return (None, grad_weight, grad_bias, None, *grads)
+
+
+def bn_relu_cat(bn, relu, features):
+    """relu(bn(torch.cat(features, 1))), `relu` an nn.ReLU module or None for the functional F.relu, fused when the
+    site allows it: where every segment can be read in place (_cat_segments_ok), the batch norm is decided by `_site`
+    on a tensor of the concatenation's shape and layout (the output, allocated first), with the hook rule covering the
+    batch norm and the ReLU module, and runs as an eval launch or a local training site over the segments.  Anything
+    else, a sync site included, concatenates with torch.cat and runs bn_relu."""
+    features = list(features)
+    if (relu is None or type(relu) is nn.ReLU) and _cat_segments_ok(features):
+        n, _, h, w = features[0].shape
+        c = sum(t.shape[1] for t in features)
+        y = torch.empty((n, c, h, w), dtype=torch.bfloat16, device=features[0].device, memory_format=torch.channels_last)
+        site = _site(bn, y, () if relu is None else (relu,), inputs=features)
+        if site is _EVAL:
+            N.check(_native_lib().b200c_bn_infer_cat(*_cat_table(features), y.data_ptr(), *_infer_params(bn), bn.eps, n * h * w, c,
+                                                     _raw_stream(y.device.index)))
+            return y
+        if site is _LOCAL:
+            return _FusedBatchNormCat.apply(y, bn.weight, bn.bias, bn, *features)
+    x = torch.cat(features, 1)
+    if relu is None:
+        return torch.relu_(bn(x))
+    return bn_relu(bn, relu, x)
 
 
 # activations with native batch-norm sites of their own, by their b200c_act_t (ReLU runs on bn_relu's sites)
@@ -878,6 +981,81 @@ else:
                  efficientnet.MBConv: FusedMBConv}
 
 
+try:
+    from torchvision.models import densenet
+except ImportError:  # without torchvision there is nothing to rewrite
+    _DENSE_SWAP = {}
+else:
+
+    class FusedDenseLayer(densenet._DenseLayer):
+        """torchvision's dense layer whose `relu1(norm1(torch.cat(features, 1)))` is one concatenation site
+        (`bn_relu_cat`) that reads the earlier feature maps in place, and whose norm2 / relu2 is a bn_relu site; the
+        convolutions and the dropout run as torchvision runs them.  Where torchvision would checkpoint the bottleneck
+        (`memory_efficient` with a gradient needed), and in eval with gradients recorded, the parent's forward runs."""
+
+        def forward(self, input):
+            prev = [input] if isinstance(input, torch.Tensor) else input
+            if (self.memory_efficient and self.any_requires_grad(prev)) or (not self.training and torch.is_grad_enabled()):
+                return super().forward(input)
+            out = self.conv1(bn_relu_cat(self.norm1, self.relu1, prev))
+            out = self.conv2(bn_relu(self.norm2, self.relu2, out))
+            if self.drop_rate > 0:
+                out = F.dropout(out, p=self.drop_rate, training=self.training)
+            return out
+
+    class FusedDenseBlock(densenet._DenseBlock):
+        """torchvision's dense block, with `forward_features`: the list of feature maps its forward would concatenate."""
+
+        def forward_features(self, init_features):
+            """[init_features, each layer's output]: the layers called as torchvision's forward calls them, without the
+            final torch.cat."""
+            features = [init_features]
+            for _, layer in self.items():
+                features.append(layer(features))
+            return features
+
+    def _dense_walk(features):
+        """The (block, transition or None) pairs of a DenseNet's `features` that FusedDenseNet.forward walks: `features`
+        an nn.Sequential of exactly conv0, norm0, relu0, pool0, then FusedDenseBlocks and torchvision _Transitions
+        (norm, relu, conv, pool) in turn, ending in a block and norm5, where neither `features` nor a block or
+        transition has a hook of its own (calling their parts skips their calls); else None."""
+        if type(features) is not nn.Sequential or _hooked(features):
+            return None
+        names, mods = zip(*features.named_children()) if len(features) else ((), ())
+        if names[:4] != ("conv0", "norm0", "relu0", "pool0") or names[-1] != "norm5" or len(names) % 2:
+            return None
+        body = mods[4:-1]
+        for i, mod in enumerate(body):
+            if type(mod) is not (FusedDenseBlock if i % 2 == 0 else densenet._Transition) or _hooked(mod):
+                return None
+            if i % 2 and tuple(k for k, _ in mod.named_children()) != ("norm", "relu", "conv", "pool"):
+                return None
+        return [(body[i], body[i + 1] if i + 1 < len(body) else None) for i in range(0, len(body), 2)]
+
+    class FusedDenseNet(densenet.DenseNet):
+        """torchvision's DenseNet whose forward skips the concatenations: the stem is one bn_relu_maxpool site, each
+        block hands its transition (or norm5) the list of its feature maps, and each transition's norm / relu and
+        norm5 with DenseNet's functional ReLU are concatenation sites (`bn_relu_cat`).  Where `_dense_walk` finds no
+        walk, a global module hook is registered, or in eval with gradients recorded, the parent's forward runs (whose
+        dense layers still fuse)."""
+
+        def forward(self, x):
+            walk = None if not self.training and torch.is_grad_enabled() else _dense_walk(self.features)
+            if walk is None or _global_hooks():
+                return super().forward(x)
+            f = self.features
+            x = bn_relu_maxpool(f.norm0, f.relu0, f.pool0, f.conv0(x))
+            for block, transition in walk:
+                features = block.forward_features(x)
+                if transition is not None:
+                    x = transition.pool(transition.conv(bn_relu_cat(transition.norm, transition.relu, features)))
+            out = bn_relu_cat(f.norm5, None, features)
+            out = torch.flatten(F.adaptive_avg_pool2d(out, (1, 1)), 1)
+            return self.classifier(out)
+
+    _DENSE_SWAP = {densenet._DenseLayer: FusedDenseLayer, densenet._DenseBlock: FusedDenseBlock, densenet.DenseNet: FusedDenseNet}
+
+
 # Torch sums a tensor of fewer elements than this (2^31 bytes of bf16) in one launch of its reduce kernel, whose order
 # the squeeze-excitation kernels restate; a larger one it splits into 32-bit-indexed pieces.
 _SE_MAX_NUMEL = 2 ** 30
@@ -1058,7 +1236,9 @@ def fuse_model(model):
     becomes a FusedConv2dNormActivation.  Every module whose class is exactly torchvision's MobileNetV2 or MobileNetV3
     InvertedResidual or EfficientNet's MBConv gets the fused subclass, whose projection batch norm (with the stochastic
     depth and residual add after it) runs as one bn_res site, and every SqueezeExcitation (exactly that class) inside such
-an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Parameters, buffers, state_dict keys, hooks and the
+an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module whose class is exactly torchvision's
+    DenseNet, _DenseBlock or _DenseLayer gets the fused subclass, whose concatenating batch norms run as concatenation
+    sites (`bn_relu_cat`).  Parameters, buffers, state_dict keys, hooks and the
     object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
     training and in eval (see `fuse_resnet` for inference).
 
@@ -1071,8 +1251,9 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Parameters, bu
         for mod in model.modules():
             if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
                 mod.__class__ = FusedConv2dNormActivation
+    swap = {**_RES_SWAP, **_DENSE_SWAP}
     for mod in model.modules():
-        cls = _RES_SWAP.get(type(mod))
+        cls = swap.get(type(mod))
         if cls is not None:
             mod.__class__ = cls
     if SqueezeExcitation is not None and _RES_SWAP:

@@ -431,6 +431,30 @@ int b200c_bn_backward_res(const void* dy, const void* noise, int rows_per_sample
 int b200c_bn_infer_res(const void* x, const void* identity, void* y, const void* weight, const void* bias, const void* running_mean,
                        const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
 
+/* ---- fused batch norm and ReLU over a channel concatenation (DenseNet) ----
+ * y = relu(bn(cat(segs, 1))) over channels-last bf16 activations without the cat: segment s is bf16 [m][seg_channels[s]]
+ * (channels-last rows, m = N * H * W alike for every segment), with seg_channels[s] % 8 == 0 and segs[s] on the 16-byte
+ * grid; the nsegs (1..64) segments' channels sum to `channels` (1..131072); m * channels < 2^31.  Results have the bits
+ * of b200c_bn_forward_mask / b200c_bn_backward_mask / b200c_bn_infer over the concatenated tensor, which are eager
+ * torch's.  y, mask, dy and dx are whole [m][channels] tensors; y, dy and dx sit on the 16-byte grid.  Every argument
+ * is checked before the first launch.
+ *
+ * b200c_bn_forward_cat: the training forward of b200c_bn_forward_mask (statistics, running statistics,
+ * num_batches_tracked, mask bits, scratch of b200c_bn_scratch_bytes(channels)), m >= 2.  2 kernels.
+ * b200c_bn_backward_cat: from dy (the gradient of y), the mask, the segments, weight and the saved statistics, writes
+ * the whole dx, grad_weight and grad_bias; a segment's gradient is its channels of dx.  2 kernels.
+ * b200c_bn_infer_cat: the eval site of b200c_bn_infer without identity, with weight, bias and running statistics of
+ * fp32, or of bf16 with param_bf16.  1 kernel. */
+int b200c_bn_forward_cat(const void* const* segs, const int* seg_channels, int nsegs, void* y, uint8_t* mask, const float* weight,
+                         const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                         float* save_invstd, int m, int channels, float momentum, float eps, void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_cat(const void* dy, const uint8_t* mask, const void* const* segs, const int* seg_channels, int nsegs, void* dx,
+                          const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias,
+                          int m, int channels, void* scratch, b200c_stream_t stream);
+int b200c_bn_infer_cat(const void* const* segs, const int* seg_channels, int nsegs, void* y, const void* weight, const void* bias,
+                       const void* running_mean, const void* running_var, int param_bf16, float eps, int m, int channels,
+                       b200c_stream_t stream);
+
 /* ---- squeeze-and-excitation (torchvision's SqueezeExcitation without its squeeze path) ----
  * Over channels-last bf16 activations x, y, dy, dx of n samples, hw = H * W rows per sample and `channels` channels
  * ([n][hw][channels]), and bf16 per-sample vectors pooled, s, ds, gp of [n][channels]; bit-identical to eager torch:

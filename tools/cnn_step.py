@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Training step and eval forward of torchvision CNNs whose batch norms sit in Conv2dNormActivation blocks
-(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf), with and without
+(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf) or in DenseNet's dense layers
+(densenet121, densenet161, densenet169, densenet201, by `--models` only), with and without
 `fused_norm.fuse_model`.  The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model), "act_only"
 (fuse_model without the inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused) and
 "no_se" (fuse_model with the squeeze-excitation modules back on torchvision's class).
@@ -37,6 +38,8 @@ from step_profile import gpu_identity  # noqa: E402
 MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "efficientnet_v2_s", "regnet_y_400mf"]
 # first match wins
 FAMILIES = [
+    ("bn_cat", r"b200c::bn_cat::k_cat"),             # DenseNet's concatenation sites, every direction
+    ("torch_cat", r"CatArrayBatchedCopy"),
     ("bn_stats", r"k_bn_stats|batch_norm_collect_statistics"),
     ("bn_transform_act", r"k_act_transform|k_act_infer|k_res_transform|k_res_infer|k_bn_transform|k_infer_transform"
                          r"|batch_norm_transform_input"),

@@ -178,16 +178,11 @@ __device__ __forceinline__ void reduce_run(const bf16* __restrict__ a, const bf1
     }
     block_y_reduce<V>(value, shared);
   }
+  // One bf16 store per output, as set_results_to_output stores them: V follows the inputs, so `out` may sit anywhere on
+  // the 2-byte grid.
   if (should_store) {
-    if (V == 4) {
-      SVec<4> o;
 #pragma unroll
-      for (int j = 0; j < 4; j++) o.v[j] = __float2bfloat16(kProduct ? value[j] : value[j] * scale);
-      *reinterpret_cast<SVec<4>*>(out + output_idx) = o;
-    } else {
-#pragma unroll
-      for (int j = 0; j < V; j++) out[output_idx + j] = __float2bfloat16(kProduct ? value[j] : value[j] * scale);
-    }
+    for (int j = 0; j < V; j++) out[output_idx + j] = __float2bfloat16(kProduct ? value[j] : value[j] * scale);
   }
 }
 

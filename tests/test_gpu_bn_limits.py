@@ -10,19 +10,32 @@ iterations of a 128-row grid), and at (16383, 131072), the most channels:
   walk, and the noise read at row / rows_per_sample): 18631 samples of 1801 rows at the first shape, one row per
   sample at the second;
 - eval sites at the first shape: b200c_bn_infer with an identity (fp32 parameters), and b200c_bn_infer_act (Hardswish)
-  and b200c_bn_infer_res with an identity (bf16 parameters).
+  and b200c_bn_infer_res with an identity (bf16 parameters);
+- concatenation sites (b200c_bn_forward_cat / b200c_bn_backward_cat / b200c_bn_infer_cat) at both shapes: segments of
+  (8, 16, 40) channels at the first, 64 segments of 2048 at the second.
 Every output is filled with all-ones bits (a NaN) before its call, so an element no thread writes shows.
+
+The squeeze-and-excitation calls admit n * c * hw up to 2^31 - 1, where torch splits its own reduction (so no torch
+bits exist for the sums).  They run at (n, c, hw) = (2, 128, 8388607), (85, 3, 8388607) and (1, 2, 2^30 - 1), where
+se_reduce_config gives a 132-SM H100 8192, 2048 and 16384 blocks per output (vec 4, 1 and 2), and at (16383, 131072,
+1), one row per sample.  Their inputs are integers whose sums are exact in any order (sum |x| and sum |dy x| at most
+2^24 per output): pooled must be bf16(fp32(S) * factor) and ds bf16(S) for the float64 row sums S; y and dx are
+elementwise and are compared with torch's ops at full size.
 
 Each tensor is 4 GiB.  Comparisons stay on the device (torch.equal of int16 views, the mask byte by byte in slices),
 and the work runs in phases that free what they no longer need.  Each test prints its peak allocation.  On an NVIDIA
 H100 80GB HBM3 (700 W power limit) they peaked at 30.3 and 30.5 GiB for the ReLU sites, 30.0 and 30.2 GiB for the
-SiLU sites, 30.1 and 30.2 GiB for the stochastic-depth sites, and 18.0 GiB for each eval test.  The tests skip, saying
+SiLU sites, 30.1 and 30.2 GiB for the stochastic-depth sites, 18.0 GiB for each eval test, 30.0 and 30.2 GiB for the
+concatenation sites, and 14.0, 14.0, 14.0 and 24.0 GiB for the squeeze-and-excitation sites.  The tests skip, saying
 so, where the GPU has less than NEED free."""
+import ctypes
+
 import pytest
 import torch
 import torch.nn.functional as F
 
 from ant_ray_b200 import _native as N
+from test_fused_se_cpu import se_reduce_config
 from test_gpu_bn_act_res_abi import row_noise
 from test_gpu_fused_norm import GUARD, check_scratch, check_stats_against_float64, make_bn
 
@@ -272,3 +285,171 @@ def test_largest_eval_act_and_res_sites_match_torch(room):
         want = bn(x4)
         want += identity.view(m, c, 1, 1)
     same(y, want.view(m, c), "y of the residual add")
+
+
+# ---- concatenation sites ------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("m,chans", [(SITES[0][0], (8, 16, 40)), (SITES[1][0], (2048,) * 64)], ids=["3_segments", "64_segments"])
+def test_largest_cat_site_matches_torch(room, m, chans):
+    c = sum(chans)
+    assert (m, c) in SITES
+    lib = N.load()
+    s = torch.cuda.current_stream().cuda_stream
+    bn = make_bn(c, 20)
+    w, b = bn.weight.detach(), bn.bias.detach()
+    segs = [seeded(m, k, 21 + i, 2.0, 0.5) for i, k in enumerate(chans)]
+    table = ((ctypes.c_void_p * len(segs))(*(t.data_ptr() for t in segs)), (ctypes.c_int * len(chans))(*chans), len(chans))
+    buf, need = scratch(c)
+
+    # forward: the native site, then torch's batch norm and ReLU on the concatenation, compared and freed
+    rm, rv, nbt = bn.running_mean.clone(), bn.running_var.clone(), bn.num_batches_tracked.clone()
+    mean, invstd = nan_filled(c, dtype=torch.float32), nan_filled(c, dtype=torch.float32)
+    y, mask = nan_filled(m, c), nan_filled(m * c // 8, dtype=torch.uint8)
+    N.check(lib.b200c_bn_forward_cat(*table, y.data_ptr(), mask.data_ptr(), w.data_ptr(), b.data_ptr(), rm.data_ptr(), rv.data_ptr(),
+                                     nbt.data_ptr(), mean.data_ptr(), invstd.data_ptr(), m, c, 0.1, 1e-5, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    assert int(nbt) == int(bn.num_batches_tracked) + 1
+    x = torch.cat(segs, 1)
+    check_stats_against_float64(x, {"mean": mean, "invstd": invstd})
+    rm_t, rv_t = bn.running_mean.clone(), bn.running_var.clone()
+    x4 = x.view(m, c, 1, 1)   # NCHW strides with stride(1) == 1: torch's channels-last kernels
+    y_t, mean_t, invstd_t = torch.native_batch_norm(x4, w, b, rm_t, rv_t, True, 0.1, 1e-5)
+    torch.relu_(y_t)
+    for got, want, what in ((mean, mean_t, "save_mean"), (invstd, invstd_t, "save_invstd"), (rm, rm_t, "running_mean"),
+                            (rv, rv_t, "running_var"), (y, y_t.view(m, c), "y")):
+        same(got, want, what)
+    check_mask(mask, y)
+    del y_t
+
+    # backward: torch's g first (it needs y, which is then freed), the native call, torch's dx
+    dy = seeded(m, c, 22, 1.0, 0.0)
+    g_t = torch.ops.aten.threshold_backward(dy.view(m, c, 1, 1), y.view(m, c, 1, 1), 0)
+    del y
+    dx = nan_filled(m, c)
+    dw, db = nan_filled(c, dtype=torch.float32), nan_filled(c, dtype=torch.float32)
+    N.check(lib.b200c_bn_backward_cat(dy.data_ptr(), mask.data_ptr(), *table, dx.data_ptr(), w.data_ptr(), mean.data_ptr(),
+                                      invstd.data_ptr(), dw.data_ptr(), db.data_ptr(), m, c, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    del dy, mask
+    dx_t, dw_t, db_t = torch.ops.aten.native_batch_norm_backward(g_t, x4, w, rm_t, rv_t, mean_t, invstd_t, True, 1e-5,
+                                                                 [True, True, True])
+    same(dx, dx_t.view(m, c), "dx")   # every segment's gradient is its channels of dx
+    same(dw, dw_t, "dweight")
+    same(db, db_t, "dbias")
+    del dx, dx_t, g_t
+
+    # eval: fp32 parameters, eager torch's eval-mode module and ReLU
+    y = nan_filled(m, c)
+    N.check(lib.b200c_bn_infer_cat(*table, y.data_ptr(), w.data_ptr(), b.data_ptr(), bn.running_mean.data_ptr(),
+                                   bn.running_var.data_ptr(), 0, 1e-5, m, c, s))
+    with torch.no_grad():
+        want = torch.relu_(bn.eval()(x4))
+    same(y, want.view(m, c), "eval y")
+
+
+# ---- squeeze-and-excitation sites ---------------------------------------------------------------------------------
+SE_SITES = [(2, 128, 8388607), (85, 3, 8388607), (1, 2, 2 ** 30 - 1), (16383, 131072, 1)]
+SE_LAUNCH = {(2, 128, 8388607): (4, 8192), (85, 3, 8388607): (1, 2048), (1, 2, 2 ** 30 - 1): (2, 16384),
+             (16383, 131072, 1): (4, 1)}   # (vec, blocks per output) at 132 SMs of 2048 threads
+
+
+def se_ints(n, c, hw, seed, lo, hi, sparse=False):
+    """Integer-valued bf16 [n * hw, c] rows in lo .. hi - 1, written slice by slice; with `sparse`, +-1 on the rows
+    whose index within the sample is (37 c + 11) mod 128 for channel c and 0 elsewhere, so that no output sums more
+    than 2^24 / 2^7 of them."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    t = torch.empty(n * hw, c, dtype=torch.bfloat16, device="cuda")
+    rows = max(1, CHUNK // c)
+    residue = (torch.arange(c, device="cuda") * 37 + 11) % 128
+    for i in range(0, n * hw, rows):
+        j = min(n * hw, i + rows)
+        if sparse:
+            sign = torch.randint(0, 2, (j - i, c), device="cuda", generator=g, dtype=torch.int8) * 2 - 1
+            on = (torch.arange(i, j, device="cuda") % hw % 128).view(-1, 1) == residue
+            t[i:j] = torch.where(on, sign, 0)
+        else:
+            t[i:j] = torch.randint(lo, hi, (j - i, c), device="cuda", generator=g, dtype=torch.int8)
+    return t
+
+
+def row_sums(a, n, c, hw, b=None):
+    """The float64 sums over each sample's rows of a, or of the bf16 product a * b, and of their magnitudes, in slices:
+    two [n, c]."""
+    out = torch.zeros(n, c, dtype=torch.float64, device="cuda")
+    mag = torch.zeros_like(out)
+    a3, b3 = a.view(n, hw, c), None if b is None else b.view(n, hw, c)
+    per, rows = max(1, CHUNK // (hw * c)), max(1, CHUNK // c)
+    for i in range(0, n, per):
+        for r in range(0, hw, rows):
+            t = a3[i:i + per, r:r + rows]
+            if b3 is not None:
+                t = t * b3[i:i + per, r:r + rows]
+            t = t.double()
+            out[i:i + per] += t.sum(1)
+            mag[i:i + per] += t.abs_().sum(1)
+    return out, mag
+
+
+@pytest.mark.parametrize("n,c,hw", SE_SITES)
+def test_largest_se_site_sums_exactly(room, n, c, hw):
+    assert 2 ** 31 - 2 ** 24 < n * c * hw <= 2 ** 31 - 1
+    lib = N.load()
+    st = torch.cuda.current_stream().cuda_stream
+    props = torch.cuda.get_device_properties(torch.cuda.current_device())
+    launch = se_reduce_config(n, c, hw, 0, props.multi_processor_count, props.max_threads_per_multi_processor)
+    print(f"launch {launch}")
+    if (props.multi_processor_count, props.max_threads_per_multi_processor) == (132, 2048):
+        assert (launch.vec, launch.ctas) == SE_LAUNCH[(n, c, hw)]
+    need = int(lib.b200c_se_scratch_bytes(n, c, hw))
+    buf = torch.empty(need + GUARD, dtype=torch.uint8, device="cuda")
+    buf[:need].zero_()
+    buf[need:].fill_(0xA5)
+    x = se_ints(n, c, hw, 30, -2, 3, sparse=hw > 2 ** 23)
+    x3 = x.view(n, hw, c)
+
+    # pool: bf16(fp32(S) * factor), factor = float(n * c) / float(n * c * hw) in fp32 as the launcher computes it
+    pooled = nan_filled(n, c)
+    N.check(lib.b200c_se_pool(x.data_ptr(), pooled.data_ptr(), n, c, hw, buf.data_ptr(), need, st))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    factor = (torch.tensor(n * c, dtype=torch.float32) / torch.tensor(n * c * hw, dtype=torch.float32)).item()
+    if hw == 1:
+        assert factor == 1.0
+        want = x.view(n, c)   # one row: S is x itself (and pooled has x's 2^31 - 2^17 elements, too many for float64 sums)
+    else:
+        sums, abs_sums = row_sums(x, n, c, hw)
+        assert float(abs_sums.max()) <= 2 ** 24   # every partial sum, in any order, is an integer fp32 holds
+        want = (sums.float() * factor).to(torch.bfloat16)
+    same(pooled, want, "pooled")
+    del pooled
+
+    # scale: torch's s * x at full size
+    s = seeded(n, c, 31, 0.25, 0.5)   # n * c reaches 2^31 - 2^17 at one row per sample: written slice by slice
+    y = nan_filled(n * hw, c)
+    N.check(lib.b200c_se_scale(x.data_ptr(), s.data_ptr(), y.data_ptr(), n, c, hw, st))
+    same(y, (x3 * s.view(n, 1, c)).view(n * hw, c), "y")
+    del y
+
+    # backward reduce: bf16(S) of the products, or with one row the product itself
+    dy = se_ints(n, c, hw, 32, -1, 2)
+    ds = nan_filled(n, c)
+    N.check(lib.b200c_se_backward_reduce(dy.data_ptr(), x.data_ptr(), ds.data_ptr(), n, c, hw, buf.data_ptr(), need, st))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    if hw == 1:
+        want = (dy * x).view(n, c)
+    else:
+        sums, abs_sums = row_sums(dy, n, c, hw, x)
+        assert float(abs_sums.max()) <= 2 ** 24
+        want = sums.float().to(torch.bfloat16)
+    same(ds, want, "ds")
+    del x, x3, ds, want
+
+    # backward elementwise: torch's dy * s, then + gp / hw
+    gp = seeded(n, c, 33, 0.5, 0.0)
+    dx = nan_filled(n * hw, c)
+    N.check(lib.b200c_se_backward_elemt(dy.data_ptr(), s.data_ptr(), gp.data_ptr(), dx.data_ptr(), n, c, hw, st))
+    dx_t = dy.view(n, hw, c) * s.view(n, 1, c)
+    dx_t.add_(gp.view(n, 1, c) / hw)
+    same(dx, dx_t.view(n * hw, c), "dx")

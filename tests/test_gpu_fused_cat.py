@@ -3,7 +3,7 @@
 dweight, dbias and every segment's gradient with its strides.
 
 Shapes: every concatenation site of densenet121/161/169/201 at batch 32 and 224 x 224, densenet121's at batch 256,
-1, 2 and 49 segments, and the launch regimes of gpu_common.BN_REGIME_SHAPES realised as segment splits.  Value edges
+1, 2, 49 and 64 segments, and the launch regimes of gpu_common.BN_REGIME_SHAPES realised as segment splits.  Value edges
 and the momentum / eps range of test_gpu_fused_norm, an NCHW output gradient, eval under no_grad and inference_mode
 with fp32 and bf16 parameters, the fallbacks (a segment of C_s % 8 != 0, a segment off the 16-byte grid, 65
 segments: torch.cat and bn_relu, no concatenation call), direct C-ABI calls with guard bytes past the scratch, and the
@@ -123,7 +123,7 @@ def test_densenet121_sites_at_batch_256(spy):
         check_shape(256, chans, h, w, spy)
 
 
-@pytest.mark.parametrize("chans", [(64,), (64, 32), (64,) + (32,) * 48], ids=["1", "2", "49"])
+@pytest.mark.parametrize("chans", [(64,), (64, 32), (64,) + (32,) * 48, (64,) + (32,) * 63], ids=["1", "2", "49", "64"])
 def test_segment_counts(chans, spy):
     check_shape(4, chans, 7, 7, spy)
 

@@ -129,6 +129,9 @@ SYMBOLS = {
     "b200c_bn_backward_cat": (c_int, [c_void_p] * 2 + [POINTER(c_void_p), POINTER(c_int), c_int] + [c_void_p] * 6 + [c_int, c_int, c_void_p,
                                                                                                                   c_void_p]),
     "b200c_bn_infer_cat": (c_int, [POINTER(c_void_p), POINTER(c_int), c_int] + [c_void_p] * 5 + [c_int, c_float, c_int, c_int, c_void_p]),
+    "b200c_bn_forward_slice": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "b200c_bn_backward_slice": (c_int, [c_void_p, c_int] + [c_void_p] * 8 + [c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_infer_slice": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_float, c_int, c_int, c_void_p]),
     "b200c_se_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200c_se_pool": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p]),
     "b200c_se_scale": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p]),

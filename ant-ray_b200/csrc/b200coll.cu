@@ -1816,6 +1816,60 @@ extern "C" int b200c_bn_infer_cat(const void* const* segs, const int* seg_channe
   return B200C_OK;
 }
 
+// A batch norm and ReLU whose output is a channel slice of a wider tensor (norm_slice.cuh): the shape (m >= min_m; m * c
+// and m * ld below 2^31), c % 8 == 0, the row stride `ld` of y or dy (a multiple of 8, at least c), and the 16-byte
+// grid of every bf16 operand `grid`.
+static int check_slice(const char* site, int min_m, int m, int c, int ld, std::initializer_list<const void*> grid) {
+  if (m < min_m || c < 1 || c > bn::kMaxChannels || (int64_t)m * c > INT32_MAX) return fail(B200C_EINVAL, "%s: bad shape m=%d c=%d", site, m, c);
+  if (c % 8) return fail(B200C_EINVAL, "%s: channels=%d is not a multiple of 8", site, c);
+  if (ld < c || ld % 8 || (int64_t)m * ld > INT32_MAX)
+    return fail(B200C_EINVAL, "%s: row stride %d is not a multiple of 8 of at least channels=%d with m * stride below 2^31", site, ld, c);
+  for (const void* p : grid)
+    if (reinterpret_cast<uintptr_t>(p) % 16) return fail(B200C_EINVAL, "%s: x, y, dy or dx is off the 16-byte grid", site);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_slice(const void* x, void* y, int ldy, uint8_t* mask, const float* weight, const float* bias,
+                                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                      float* save_invstd, int m, int channels, float momentum, float eps, void* scratch,
+                                      b200c_stream_t stream) {
+  if (!x || !y || !mask || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !scratch)
+    return fail(B200C_EINVAL, "batch norm slice forward: null buffer");
+  int rc = check_slice("batch norm slice", 2, m, channels, ldy, {x, y});
+  if (rc) return rc;
+  const bn::FwdArgs a{x, nullptr, y, mask, true, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  RT(bn::forward_slice(a, ldy, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_slice(const void* dy, int lddy, const uint8_t* mask, const void* x, void* dx, const float* weight,
+                                       const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m,
+                                       int channels, void* scratch, b200c_stream_t stream) {
+  if (!dy || !mask || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias || !scratch)
+    return fail(B200C_EINVAL, "batch norm slice backward: null buffer");
+  int rc = check_slice("batch norm slice", 2, m, channels, lddy, {dy, x, dx});
+  if (rc) return rc;
+  const bn::BwdArgs a{dy, nullptr, nullptr, mask, x, nullptr, dx, true, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                      m, channels, scratch};
+  RT(bn::backward_slice(a, lddy, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_slice(const void* x, void* y, int ldy, const void* weight, const void* bias, const void* running_mean,
+                                    const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream) {
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "batch norm infer slice: null buffer");
+  int rc = check_infer("batch norm infer slice", param_bf16, m, channels);
+  if (!rc) rc = check_slice("batch norm infer slice", 1, m, channels, ldy, {x, y});
+  if (rc) return rc;
+  RT(bn::infer_slice({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, 0, 0}, ldy,
+                     (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // squeeze-and-excitation (se_kernels.cuh, launched by inst_se.cu): one kernel per call
 // ------------------------------------------------------------------------------------------------

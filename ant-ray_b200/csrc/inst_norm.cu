@@ -1,5 +1,5 @@
-// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh); argument
-// checking lives in b200coll.cu.
+// Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh,
+// norm_slice.cuh); argument checking lives in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
@@ -10,6 +10,7 @@
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
 #include "norm_res.cuh"
+#include "norm_slice.cuh"
 
 namespace b200c {
 namespace bn {
@@ -276,6 +277,11 @@ cudaError_t load_kernels() {
   load(&bn_cat::k_cat_bwd_elemt);
   load(&bn_cat::k_cat_infer<float>);
   load(&bn_cat::k_cat_infer<bf16>);
+  load(&bn_slice::k_slice_transform);
+  load(&bn_slice::k_slice_bwd_reduce);
+  load(&bn_slice::k_slice_bwd_elemt);
+  load(&bn_slice::k_slice_infer<float>);
+  load(&bn_slice::k_slice_infer<bf16>);
   for (int src = 0; src < kGradSrcs; src++) {
     load(bwd_reduce_kernel(src, false));
     load(bwd_reduce_kernel(src, true));
@@ -754,6 +760,55 @@ static cudaError_t launch_infer_cat(const CatSegments& in, const InferArgs& a, c
 
 cudaError_t infer_cat(const CatSegments& in, const InferArgs& a, cudaStream_t st) {
   return a.param_bf16 ? launch_infer_cat<bf16>(in, a, st) : launch_infer_cat<float>(in, a, st);
+}
+
+// ---- batch norm and ReLU into a channel slice of a wider output (norm_slice.cuh) ----
+// The statistics are the local site's (k_bn_stats on x); every other launch takes its bn:: counterpart's vector launch
+// shape for the branch's m and c: the caller has checked C % 8 == 0 and x, y, dy and dx onto the 16-byte grid, which
+// is what vec_ok decides for a tensor of c % 8 == 0.
+cudaError_t forward_slice(const FwdArgs& a, int ldy, cudaStream_t st) {
+  const cudaError_t e = launch_stats(a, nullptr, st);
+  if (e != cudaSuccess) return e;
+  dim3 block, grid;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  bn_slice::k_slice_transform<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), ldy,
+                                                      static_cast<uint8_t*>(a.mask), a.save_mean, a.save_invstd, a.weight, a.bias,
+                                                      a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t backward_slice(const BwdArgs& a, int lddy, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  const void* ptrs[2] = {a.x, a.dy};
+  const BwdReduceLaunch l = bwd_reduce_launch(a.m, a.c, kGradBits, false, false, ptrs, 2);
+  if (l.vec != kBwdVec) return kNoKernel;
+  bn_slice::k_slice_bwd_reduce<<<l.grid, l.block, l.smem, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(a.dy), lddy,
+                                                                static_cast<const uint8_t*>(a.mask), a.save_mean, a.save_invstd, s.sums,
+                                                                s.sums + a.c, a.grad_weight, a.grad_bias, s.staging, s.semaphores, a.m,
+                                                                a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  dim3 block, grid;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  bn_slice::k_slice_bwd_elemt<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.dy), lddy, static_cast<const uint8_t*>(a.mask),
+                                                      static_cast<const bf16*>(a.x), static_cast<bf16*>(a.dx), a.save_mean, a.save_invstd,
+                                                      a.weight, s.sums, s.sums + a.c, (float)(1.0 / a.m), a.m, a.c);
+  return cudaGetLastError();
+}
+
+template <typename P>
+static cudaError_t launch_infer_slice(const InferArgs& a, int ldy, cudaStream_t st) {
+  dim3 block, grid;
+  ew_config(a.m, a.c, kEwVec, &block, &grid);
+  const InferParams& b = a.bn;
+  bn_slice::k_slice_infer<P><<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), ldy,
+                                                     static_cast<const P*>(b.running_mean), static_cast<const P*>(b.running_var),
+                                                     static_cast<const P*>(b.weight), static_cast<const P*>(b.bias), b.eps, a.m, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_slice(const InferArgs& a, int ldy, cudaStream_t st) {
+  return a.param_bf16 ? launch_infer_slice<bf16>(a, ldy, st) : launch_infer_slice<float>(a, ldy, st);
 }
 
 }  // namespace bn

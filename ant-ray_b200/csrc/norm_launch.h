@@ -139,5 +139,15 @@ cudaError_t forward_cat(const CatSegments& segs, const FwdArgs& a, cudaStream_t 
 cudaError_t backward_cat(const CatSegments& segs, const BwdArgs& a, cudaStream_t s);
 cudaError_t infer_cat(const CatSegments& segs, const InferArgs& a, cudaStream_t s);
 
+// Batch norm followed by ReLU whose output y is a channel slice of a wider channels-last tensor (norm_slice.cuh): x is
+// the branch's bf16 [m][c], y row r sits at y + r * ldy, and the backward's dy at dy + r * lddy; c, ldy and lddy are
+// multiples of 8 and x, y, dy and dx sit on the 16-byte grid.  A local training site: the forward reads FwdArgs
+// without identity or stem and writes y's slice and the branch's mask (2 kernels); the backward reads BwdArgs.dy, .mask
+// and .x instead of .dy2, .y or .dy_masked and writes dx (2 kernels).  The eval site reads InferArgs without identity,
+// downsample or stem (1 kernel).
+cudaError_t forward_slice(const FwdArgs& a, int ldy, cudaStream_t s);
+cudaError_t backward_slice(const BwdArgs& a, int lddy, cudaStream_t s);
+cudaError_t infer_slice(const InferArgs& a, int ldy, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

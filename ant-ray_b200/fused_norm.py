@@ -1,5 +1,6 @@
-"""Fused batch norm for the training step and eval forward of ResNets, DenseNets and torchvision's Conv2dNormActivation
-blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh), and the
+"""Fused batch norm for the training step and eval forward of ResNets, DenseNets, Inception v3, GoogLeNet and
+torchvision's Conv2dNormActivation blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh,
+norm_cat.cuh, norm_slice.cuh), and the
 squeeze-and-excitation of EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
@@ -72,6 +73,20 @@ channels-last CUDA tensor with a channel stride of 1, a multiple of 8 channels a
 alike in N, H, W and device, at most 64 of them, and the batch norm, decided on a tensor of the concatenation's shape
 and layout, is an eval or a local site by the rules above; anything else, a sync site included, runs torch.cat and
 bn_relu.  Each norm2 / relu2 is a bn_relu site and the stem a bn_relu_maxpool site.
+
+Inception v3 and GoogLeNet: `fuse_model` also swaps torchvision's `BasicConv2d` (of both models), whose
+`F.relu(bn(conv(x)), inplace=True)` then runs as a bn_relu eval or local site (a sync batch norm keeps the module's
+forward), and the Inception modules (`InceptionA` to `InceptionE`, GoogLeNet's `Inception`), whose `torch.cat` of their
+branches is built in place: each branch's last batch norm and ReLU is a slice site (`bn_relu_concat`, norm_slice.cuh)
+that writes its output straight into its channels of the module's channels-last output, and a max-pool branch is
+copied there as torch.cat copies it; InceptionE's inner concatenations flatten into the outer one.  No branch output is
+written or kept for the backward, whose gradient reads each site's channels of dy in place, and every result is eager
+torch's bits.  A module runs there when every branch operand is a bf16 channels-last CUDA tensor with a multiple of 8
+channels on the 16-byte grid and every site is an eval or a local site by the rules above; where a branch-ending
+BasicConv2d, its batch norm or a GoogLeNet branch Sequential has a hook, a global hook is registered, or in eval with
+gradients recorded, the module runs its parent's forward, and where only the operands or the sites fail, it runs the
+batch norms and ReLUs as modules and torch.cat.  The convolutions run in torchvision's order before any branch's last
+batch norm, so the backward adds the module input's branch gradients in eager torch's order.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -556,14 +571,18 @@ def _site(bn, x, mods=(), operands=(), sync=True, inputs=()):
     return _LOCAL if _local_ok(bn, x) else None
 
 
-def bn_relu(bn, relu, x):
-    """relu(bn(x)), fused when the site allows it."""
-    site = _site(bn, x, (relu,)) if type(relu) is nn.ReLU else None
+def bn_relu(bn, relu, x, sync=True):
+    """relu(bn(x)), fused when the site allows it.  `relu` None stands for torchvision BasicConv2d's functional
+    F.relu(..., inplace=True); with `sync` False a sync batch norm runs its own module forward (FusedSyncBatchNorm's
+    sync site) and then the ReLU."""
+    site = _site(bn, x, () if relu is None else (relu,), sync=sync) if relu is None or type(relu) is nn.ReLU else None
     if site is _EVAL:
         c = x.shape[1]
         return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer(x.data_ptr(), None, y, *p, bn.eps, x.numel() // c, c, s))
     if site is not None:
         return _FusedBatchNorm.apply(x, None, bn.weight, bn.bias, bn, False, None if site is _LOCAL else site, True)
+    if relu is None:
+        return F.relu(bn(x), inplace=True)
     return relu(bn(x))
 
 
@@ -655,6 +674,157 @@ def bn_relu_cat(bn, relu, features):
     if relu is None:
         return torch.relu_(bn(x))
     return bn_relu(bn, relu, x)
+
+
+def _cat_format(tensors):
+    """The memory format torch.cat gives its output: the operands' common suggested format, else contiguous."""
+    formats = {torch._prims_common.suggest_memory_format(t) for t in tensors}
+    return formats.pop() if len(formats) == 1 else torch.contiguous_format
+
+
+def _slice_operands_ok(tensors):
+    """Whether `tensors` (a module's branch outputs, in output order) can be the operands of slice sites: each passes
+    _activation with the first one's N, H, W and device, has a multiple of 8 channels (so every slice starts on the
+    16-byte grid of the output's rows) and a data pointer on the 16-byte grid, the output has fewer than 2^31 elements,
+    and torch.cat would lay it out as rows of channels: channels-last, or either format over one row per sample, where
+    both lay out memory alike.  (A channels-last tensor whose strides also fit another order, as N = 1 with W = 1 can
+    after a view, may make torch.cat choose the contiguous format.)"""
+    t0 = tensors[0]
+    if t0.dim() != 4:
+        return False
+    n, _, h, w = t0.shape
+    for t in tensors:
+        if not _activation(t) or t.device != t0.device or t.shape[0] != n or t.shape[2] != h or t.shape[3] != w:
+            return False
+        if t.shape[1] % 8 or t.data_ptr() % 16:
+            return False
+    if h * w > 1 and _cat_format(tensors) != torch.channels_last:
+        return False
+    return n * h * w * sum(t.shape[1] for t in tensors) < 2 ** 31
+
+
+def _concat_like(operands):
+    """The empty bf16 output of torch.cat(operands, 1) with the strides torch.cat gives it (_cat_format)."""
+    t0 = operands[0]
+    n, _, h, w = t0.shape
+    return torch.empty((n, sum(t.shape[1] for t in operands), h, w), dtype=torch.bfloat16, device=t0.device,
+                       memory_format=_cat_format(operands))
+
+
+def _rows_of(dy):
+    """dy as the slice sites' backward reads it: channels-last with a channel stride of 1 on the 16-byte grid, a copy
+    where it arrives otherwise.  The copy is exact: eager torch's threshold_backward writes g in y's layout, which is
+    channels-last, whatever the layout of the gradient it is given."""
+    if _activation(dy) and dy.data_ptr() % 16 == 0:
+        return dy
+    return dy.clone(memory_format=torch.channels_last)
+
+
+class _FusedBatchNormSlices(torch.autograd.Function):
+    """torch.cat([relu(bn_b(x_b)) for each site b, or a ready tensor], 1) in training mode: one autograd node for a
+    whole Inception module.  `spec` gives, in output order, each branch's batch norm (a site, whose x, weight and bias
+    are the next three tensors) or None (a ready tensor, the next one).  Each site writes its output straight into its
+    channels of the output and its ReLU's mask bits (b200c_bn_forward_slice); a ready tensor is copied into its
+    channels, exactly as torch.cat copies it.  The backward reads each site's channels of dy in place
+    (b200c_bn_backward_slice) and returns each ready tensor's gradient as dy.narrow(1, c0, C) of dy as it arrived, which
+    is what torch's CatBackward returns, so the ops consuming it (a max-pool backward picks its kernel by layout) see
+    what they see in eager torch."""
+
+    @staticmethod
+    def forward(ctx, spec, *tensors):
+        lib = _native_lib()
+        parts, it = [], iter(tensors)
+        for bn in spec:
+            parts.append((bn, next(it), next(it), next(it)) if bn is not None else (None, next(it), None, None))
+        out = _concat_like([x for _, x, _, _ in parts])
+        n, ctot, h, w = out.shape
+        m = n * h * w
+        saved, layout, c0 = [], [], 0
+        for bn, x, weight, bias in parts:
+            c = x.shape[1]
+            if bn is None:
+                out.narrow(1, c0, c).copy_(x)
+            else:
+                mask = torch.empty(m * c // 8, dtype=torch.uint8, device=x.device)
+                stats, params, stream, scratch = _forward_args(x, bn, weight, bias)
+                N.check(lib.b200c_bn_forward_slice(x.data_ptr(), out.data_ptr() + 2 * c0, ctot, mask.data_ptr(), *params, m, c,
+                                                   bn.momentum, bn.eps, scratch, stream))
+                saved += [x, mask, weight, stats]
+            layout.append((bn is not None, c0, c))
+            c0 += c
+        ctx.layout = layout
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(*saved)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        layout = ctx.layout
+        if dy is None:
+            return (None,) + tuple(None for site, _, _ in layout for _ in range(3 if site else 1))
+        lib = _native_lib()
+        saved = iter(ctx.saved_tensors)
+        g = _rows_of(dy)
+        ctot = g.shape[1]
+        grads = [None]
+        for site, c0, c in layout:
+            if not site:
+                grads.append(dy.narrow(1, c0, c))
+                continue
+            x, mask, weight, stats = next(saved), next(saved), next(saved), next(saved)
+            dx, grad_weight, grad_bias, stream, scratch = _backward_args(x)
+            mean = stats.data_ptr()
+            N.check(lib.b200c_bn_backward_slice(g.data_ptr() + 2 * c0, ctot, mask.data_ptr(), x.data_ptr(), dx.data_ptr(),
+                                                weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(),
+                                                x.numel() // c, c, scratch, stream))
+            grads += [dx, grad_weight, grad_bias]
+        return tuple(grads)
+
+
+def bn_relu_concat(branches):
+    """torch.cat(outputs, 1) of a module whose branches, in output order, are each a batch-norm site `(bn, x)` or
+    `(bn, x, mods)` standing for F.relu(bn(x), inplace=True) (torchvision's BasicConv2d after its convolution; `mods`
+    the other modules whose calls the site replaces), or a ready tensor, with eager torch's bits.  The output is
+    allocated once in torch.cat's layout and each site writes its channels of it in place.
+
+    Every site is decided by `_site` (never a sync site), with the ready tensors as inputs an eval site must not record
+    a gradient for.  Where every site is an eval site, each runs one b200c_bn_infer_slice launch and each ready tensor
+    is copied into its channels; where every site is a local training site, one _FusedBatchNormSlices node runs them
+    all.  Anything else (operands _slice_operands_ok refuses, a site that runs its modules, or eval and training sites
+    mixed) runs each site's batch norm and ReLU as modules and then torch.cat."""
+    sites = [(b[0], b[1], b[2] if len(b) > 2 else ()) for b in branches if isinstance(b, tuple)]
+    ready = [b for b in branches if not isinstance(b, tuple)]
+    operands = [b[1] if isinstance(b, tuple) else b for b in branches]
+    kinds = set()
+    if sites and _slice_operands_ok(operands):
+        kinds = {_site(bn, x, mods, sync=False, inputs=ready) for bn, x, mods in sites}
+    if kinds == {_EVAL}:
+        out = _concat_like(operands)
+        n, ctot, h, w = out.shape
+        m = n * h * w
+        lib, stream, c0 = _native_lib(), _raw_stream(out.device.index), 0
+        for b in branches:
+            if isinstance(b, tuple):
+                bn, x = b[0], b[1]
+                c = x.shape[1]
+                N.check(lib.b200c_bn_infer_slice(x.data_ptr(), out.data_ptr() + 2 * c0, ctot, *_infer_params(bn), bn.eps, m, c, stream))
+            else:
+                c = b.shape[1]
+                out.narrow(1, c0, c).copy_(b)
+            c0 += c
+        return out
+    if kinds == {_LOCAL}:
+        spec, tensors = [], []
+        for b in branches:
+            if isinstance(b, tuple):
+                spec.append(b[0])
+                tensors += [b[1], b[0].weight, b[0].bias]
+            else:
+                spec.append(None)
+                tensors.append(b)
+        return _FusedBatchNormSlices.apply(tuple(spec), *tensors)
+    return torch.cat([F.relu(b[0](b[1]), inplace=True) if isinstance(b, tuple) else b for b in branches], 1)
 
 
 # activations with native batch-norm sites of their own, by their b200c_act_t (ReLU runs on bn_relu's sites)
@@ -1056,6 +1226,146 @@ else:
     _DENSE_SWAP = {densenet._DenseLayer: FusedDenseLayer, densenet._DenseBlock: FusedDenseBlock, densenet.DenseNet: FusedDenseNet}
 
 
+try:
+    import importlib
+
+    # torchvision.models re-exports the builder functions under the modules' names, so the modules come from importlib
+    _inception = importlib.import_module("torchvision.models.inception")
+    _googlenet = importlib.import_module("torchvision.models.googlenet")
+except ImportError:  # without torchvision there is nothing to rewrite
+    _SLICE_SWAP = {}
+else:
+
+    def _basic_conv_forward(self, x):
+        return bn_relu(self.bn, None, self.conv(x), sync=False)
+
+    class FusedInceptionBasicConv2d(_inception.BasicConv2d):
+        """Inception3's BasicConv2d, `F.relu(bn(conv(x)), inplace=True)`, whose batch norm and ReLU run as a bn_relu eval
+        or local site; a sync batch norm, or anything else, runs the module ops."""
+
+        forward = _basic_conv_forward
+
+    class FusedGoogLeNetBasicConv2d(_googlenet.BasicConv2d):
+        """GoogLeNet's BasicConv2d, as FusedInceptionBasicConv2d."""
+
+        forward = _basic_conv_forward
+
+    _BASIC_CONVS = (FusedInceptionBasicConv2d, FusedGoogLeNetBasicConv2d)
+
+    def _tail(blk, x, *mods):
+        """The slice site of a branch's last block `blk` on its input x: its convolution called as a module, then
+        bn_relu_concat's site for its batch norm and ReLU.  `mods` are the other modules whose calls the site replaces
+        (a GoogLeNet branch's Sequential)."""
+        return (blk.bn, blk.conv(x), (blk, *mods))
+
+    def _seq_tail(seq, x):
+        """The slice site of a GoogLeNet branch Sequential: every module but the last called in turn, then _tail."""
+        for mod in list(seq)[:-1]:
+            x = mod(x)
+        return _tail(seq[-1], x, seq)
+
+    def _slice_forward(module, tails, seqs, branches):
+        """An Inception module's output from `branches()`, its branch outputs in output order as bn_relu_concat takes
+        them, or None where the parent's forward must run: eval with gradients recorded, a branch-ending block `tails`
+        that is not a fused BasicConv2d, or a hook that the bypassed calls would skip (on a tail, its batch norm, a
+        branch Sequential of `seqs`, or a global one).  branches() calls every convolution in torchvision's order and
+        leaves each branch's last batch norm to bn_relu_concat, after all of them: so the backward runs each branch's
+        chain in eager torch's order, and the module input's gradient, a bf16 sum over the branches, adds them in eager
+        torch's order."""
+        if not module.training and torch.is_grad_enabled():
+            return None
+        if any(type(t) not in _BASIC_CONVS for t in tails) or _skips_hooks(*tails, *(t.bn for t in tails), *seqs):
+            return None
+        return bn_relu_concat(branches())
+
+    def _avg_pool(x):
+        return F.avg_pool2d(x, kernel_size=3, stride=1, padding=1)
+
+    def _max_pool(x):
+        return F.max_pool2d(x, kernel_size=3, stride=2)
+
+    class FusedInceptionA(_inception.InceptionA):
+        """Inception3's InceptionA whose four branches end in slice sites of one output (bn_relu_concat)."""
+
+        def forward(self, x):
+            out = _slice_forward(self, (self.branch1x1, self.branch5x5_2, self.branch3x3dbl_3, self.branch_pool), (), lambda: [
+                _tail(self.branch1x1, x),
+                _tail(self.branch5x5_2, self.branch5x5_1(x)),
+                _tail(self.branch3x3dbl_3, self.branch3x3dbl_2(self.branch3x3dbl_1(x))),
+                _tail(self.branch_pool, _avg_pool(x)),
+            ])
+            return super().forward(x) if out is None else out
+
+    class FusedInceptionB(_inception.InceptionB):
+        """Inception3's InceptionB: two slice sites and the max-pool branch as a ready tensor."""
+
+        def forward(self, x):
+            out = _slice_forward(self, (self.branch3x3, self.branch3x3dbl_3), (), lambda: [
+                _tail(self.branch3x3, x),
+                _tail(self.branch3x3dbl_3, self.branch3x3dbl_2(self.branch3x3dbl_1(x))),
+                _max_pool(x),
+            ])
+            return super().forward(x) if out is None else out
+
+    class FusedInceptionC(_inception.InceptionC):
+        """Inception3's InceptionC whose four branches end in slice sites of one output."""
+
+        def forward(self, x):
+            out = _slice_forward(self, (self.branch1x1, self.branch7x7_3, self.branch7x7dbl_5, self.branch_pool), (), lambda: [
+                _tail(self.branch1x1, x),
+                _tail(self.branch7x7_3, self.branch7x7_2(self.branch7x7_1(x))),
+                _tail(self.branch7x7dbl_5, self.branch7x7dbl_4(self.branch7x7dbl_3(self.branch7x7dbl_2(self.branch7x7dbl_1(x))))),
+                _tail(self.branch_pool, _avg_pool(x)),
+            ])
+            return super().forward(x) if out is None else out
+
+    class FusedInceptionD(_inception.InceptionD):
+        """Inception3's InceptionD: two slice sites and the max-pool branch as a ready tensor."""
+
+        def forward(self, x):
+            out = _slice_forward(self, (self.branch3x3_2, self.branch7x7x3_4), (), lambda: [
+                _tail(self.branch3x3_2, self.branch3x3_1(x)),
+                _tail(self.branch7x7x3_4, self.branch7x7x3_3(self.branch7x7x3_2(self.branch7x7x3_1(x)))),
+                _max_pool(x),
+            ])
+            return super().forward(x) if out is None else out
+
+    class FusedInceptionE(_inception.InceptionE):
+        """Inception3's InceptionE, whose inner concatenations flatten into the outer one: six slice sites, 2a / 2b and
+        3a / 3b at their final offsets."""
+
+        def forward(self, x):
+            def branches():
+                b1 = _tail(self.branch1x1, x)
+                t = self.branch3x3_1(x)
+                b2a, b2b = _tail(self.branch3x3_2a, t), _tail(self.branch3x3_2b, t)
+                t = self.branch3x3dbl_2(self.branch3x3dbl_1(x))
+                b3a, b3b = _tail(self.branch3x3dbl_3a, t), _tail(self.branch3x3dbl_3b, t)
+                return [b1, b2a, b2b, b3a, b3b, _tail(self.branch_pool, _avg_pool(x))]
+
+            tails = (self.branch1x1, self.branch3x3_2a, self.branch3x3_2b, self.branch3x3dbl_3a, self.branch3x3dbl_3b, self.branch_pool)
+            out = _slice_forward(self, tails, (), branches)
+            return super().forward(x) if out is None else out
+
+    class FusedInception(_googlenet.Inception):
+        """GoogLeNet's Inception module whose four branches end in slice sites of one output; the Sequentials of
+        branches 2 to 4 are walked module by module."""
+
+        def forward(self, x):
+            seqs = (self.branch2, self.branch3, self.branch4)
+            out = None
+            if all(type(s) is nn.Sequential and len(s) > 0 for s in seqs):
+                out = _slice_forward(self, (self.branch1, *(s[-1] for s in seqs)), seqs, lambda: [
+                    _tail(self.branch1, x), _seq_tail(self.branch2, x), _seq_tail(self.branch3, x), _seq_tail(self.branch4, x),
+                ])
+            return super().forward(x) if out is None else out
+
+    _SLICE_SWAP = {_inception.BasicConv2d: FusedInceptionBasicConv2d, _googlenet.BasicConv2d: FusedGoogLeNetBasicConv2d,
+                   _inception.InceptionA: FusedInceptionA, _inception.InceptionB: FusedInceptionB,
+                   _inception.InceptionC: FusedInceptionC, _inception.InceptionD: FusedInceptionD,
+                   _inception.InceptionE: FusedInceptionE, _googlenet.Inception: FusedInception}
+
+
 # Torch sums a tensor of fewer elements than this (2^31 bytes of bf16) in one launch of its reduce kernel, whose order
 # the squeeze-excitation kernels restate; a larger one it splits into 32-bit-indexed pieces.
 _SE_MAX_NUMEL = 2 ** 30
@@ -1238,7 +1548,10 @@ def fuse_model(model):
     depth and residual add after it) runs as one bn_res site, and every SqueezeExcitation (exactly that class) inside such
 an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module whose class is exactly torchvision's
     DenseNet, _DenseBlock or _DenseLayer gets the fused subclass, whose concatenating batch norms run as concatenation
-    sites (`bn_relu_cat`).  Parameters, buffers, state_dict keys, hooks and the
+    sites (`bn_relu_cat`).  Every module whose class is exactly torchvision's Inception v3 or GoogLeNet BasicConv2d,
+    InceptionA to InceptionE or GoogLeNet's Inception gets the fused subclass: BasicConv2d's batch norm and ReLU run as
+    a bn_relu site, and each Inception module's branches write their last batch norm and ReLU into their channels of the
+    module's output (`bn_relu_concat`).  Parameters, buffers, state_dict keys, hooks and the
     object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
     training and in eval (see `fuse_resnet` for inference).
 
@@ -1251,7 +1564,7 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module w
         for mod in model.modules():
             if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
                 mod.__class__ = FusedConv2dNormActivation
-    swap = {**_RES_SWAP, **_DENSE_SWAP}
+    swap = {**_RES_SWAP, **_DENSE_SWAP, **_SLICE_SWAP}
     for mod in model.modules():
         cls = swap.get(type(mod))
         if cls is not None:

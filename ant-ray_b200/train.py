@@ -126,8 +126,9 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     the backend config's wire type, `wrap_single` wraps in DDP / FSDP even at world size 1 (the
     reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
     torchvision ResNet, every torchvision Conv2dNormActivation ending in ReLU6, SiLU or Hardswish (MobileNetV2 / V3,
-    EfficientNet), the inverted-residual blocks with their projection batch norm and squeeze-and-excitation, and a
-    torchvision DenseNet (whose concatenating batch norms then read the feature maps in place), is first
+    EfficientNet), the inverted-residual blocks with their projection batch norm and squeeze-and-excitation, a
+    torchvision DenseNet (whose concatenating batch norms then read the feature maps in place), and torchvision's
+    Inception v3 and GoogLeNet (whose Inception modules' branches then write into their concatenation in place), is first
     rewritten in place by `fused_norm.fuse_model`, and with more than one rank the
     model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
     communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten blocks'

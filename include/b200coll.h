@@ -455,6 +455,30 @@ int b200c_bn_infer_cat(const void* const* segs, const int* seg_channels, int nse
                        const void* running_mean, const void* running_var, int param_bf16, float eps, int m, int channels,
                        b200c_stream_t stream);
 
+/* ---- fused batch norm and ReLU into a channel slice of a wider output (Inception, GoogLeNet) ----
+ * y = relu(bn(x)) over a branch's channels-last bf16 x of [m][channels] (channels 1..131072, a multiple of 8), written
+ * into a channel slice of a wider channels-last output: row r of the branch lands at y + r * ldy, y pointing at the
+ * slice's first channel, so the branch outputs of a concatenation are written in place and never copied.  ldy (and
+ * the backward's lddy) is a multiple of 8 of at least `channels`, with m * ldy and m * channels below 2^31.  x, y, dy
+ * and dx sit on the 16-byte grid; the mask is the branch's own m * channels / 8 bytes.  Nothing outside the slice is
+ * written.  Results have the bits of b200c_bn_forward_mask / b200c_bn_backward_mask / b200c_bn_infer over the branch,
+ * which are eager torch's.  Every argument is checked before the first launch.
+ *
+ * b200c_bn_forward_slice: the training forward of b200c_bn_forward_mask without identity (statistics, running
+ * statistics, num_batches_tracked, mask bits, scratch of b200c_bn_scratch_bytes(channels)), m >= 2.  2 kernels.
+ * b200c_bn_backward_slice: from dy (the gradient of y, rows lddy apart), the mask, x, weight and the saved statistics,
+ * writes dx, grad_weight and grad_bias.  2 kernels.
+ * b200c_bn_infer_slice: the eval site of b200c_bn_infer without identity, with weight, bias and running statistics of
+ * fp32, or of bf16 with param_bf16, m >= 1.  1 kernel. */
+int b200c_bn_forward_slice(const void* x, void* y, int ldy, uint8_t* mask, const float* weight, const float* bias, float* running_mean,
+                           float* running_var, int64_t* num_batches_tracked, float* save_mean, float* save_invstd, int m, int channels,
+                           float momentum, float eps, void* scratch, b200c_stream_t stream);
+int b200c_bn_backward_slice(const void* dy, int lddy, const uint8_t* mask, const void* x, void* dx, const float* weight,
+                            const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int m, int channels,
+                            void* scratch, b200c_stream_t stream);
+int b200c_bn_infer_slice(const void* x, void* y, int ldy, const void* weight, const void* bias, const void* running_mean,
+                         const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
+
 /* ---- squeeze-and-excitation (torchvision's SqueezeExcitation without its squeeze path) ----
  * Over channels-last bf16 activations x, y, dy, dx of n samples, hw = H * W rows per sample and `channels` channels
  * ([n][hw][channels]), and bf16 per-sample vectors pooled, s, ds, gp of [n][channels]; bit-identical to eager torch:

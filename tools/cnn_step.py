@@ -1,19 +1,22 @@
 #!/usr/bin/env python
 """Training step and eval forward of torchvision CNNs whose batch norms sit in Conv2dNormActivation blocks
-(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf) or in DenseNet's dense layers
-(densenet121, densenet161, densenet169, densenet201, by `--models` only), with and without
+(mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf), in DenseNet's dense layers
+(densenet121, densenet161, densenet169, densenet201, by `--models` only) or in Inception's BasicConv2d blocks
+(inception_v3 at 299 x 299 and googlenet, aux heads on, by `--models` only), with and without
 `fused_norm.fuse_model`.  The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model), "act_only"
 (fuse_model without the inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused) and
 "no_se" (fuse_model with the squeeze-excitation modules back on torchvision's class).
 
-Batch `--batch` (256) at 224 x 224, bf16 autocast with fp32 parameters, channels-last, SGD with momentum.  Per model,
+Batch `--batch` (256) at 224 x 224 (inception_v3: 299 x 299), bf16 autocast with fp32 parameters, channels-last, SGD
+with momentum; the training loss sums the cross-entropies of the main and aux logits.  Per model,
 alternating the builds in one process, `--runs` times each, the order reversed every run (ABBA):
   train_images_per_sec   `--iters` training steps between device events, after `--warmup` steps
   eval_images_per_sec    `--iters` forwards under inference_mode, the same way
 All builds start from the same weights and train on the same batches, reseeded per step, so after the timed runs
 their parameters and eval logits must have identical bits ("identical", each build against the first).  Then the host's time per training step
 (forward and backward, no optimizer step): the wall time per step at batch `--host-batch` (4), where the GPU work is
-too small to set the pace.  Then, in a separate profiled run per build, the kernel time per step by family.
+too small to set the pace.  Then the peak of torch.cuda.max_memory_allocated over one training step, and, in a
+separate profiled run per build, the kernel time per step by family.
 
 Writes OUT/cnn_step.json; prints the summary.  The card's name and power limit are read in the same run.
 
@@ -39,6 +42,7 @@ MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "efficientnet
 # first match wins
 FAMILIES = [
     ("bn_cat", r"b200c::bn_cat::k_cat"),             # DenseNet's concatenation sites, every direction
+    ("bn_slice", r"b200c::bn_slice::k_slice"),       # Inception's slice sites, every direction but the statistics
     ("torch_cat", r"CatArrayBatchedCopy"),
     ("bn_stats", r"k_bn_stats|batch_norm_collect_statistics"),
     ("bn_transform_act", r"k_act_transform|k_act_infer|k_res_transform|k_res_infer|k_bn_transform|k_infer_transform"
@@ -51,6 +55,19 @@ FAMILIES = [
     ("torch_act", r"silu|hardswish|hardsigmoid|clamp|hardtanh|threshold|relu"),
     ("conv", r"conv|cudnn|xmma|gemm|nvjet|cutlass|fprop|dgrad|wgrad|implicit_|nhwc|nchw|sm90_"),
 ]
+
+
+# input size per model, where it is not 224
+SIZES = {"inception_v3": 299}
+
+
+def loss_of(out, y):
+    """The cross-entropy of the main logits plus those of the aux heads (Inception v3, GoogLeNet) in training."""
+    import torch
+    import torch.nn.functional as F
+
+    logits = [out] if isinstance(out, torch.Tensor) else [t for t in out if t is not None]
+    return sum(F.cross_entropy(t.float(), y) for t in logits)
 
 
 def family_of(name):
@@ -85,11 +102,14 @@ def main():
     torch.backends.cudnn.deterministic = True   # the two builds' results are compared bit for bit
     device = torch.device("cuda", 0)
     g = torch.Generator(device=device).manual_seed(3)
-    x = torch.randn(args.batch, 3, 224, 224, device=device, generator=g).contiguous(memory_format=torch.channels_last)
+    inputs = {}
+    for size in {SIZES.get(a, 224) for a in args.models.split(",")}:
+        inputs[size] = torch.randn(args.batch, 3, size, size, device=device, generator=g).contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, 1000, (args.batch,), device=device, generator=g)
     out = {**gpu_identity(), "batch": args.batch, "runs": args.runs, "iters": args.iters, "models": {}}
 
     for arch in args.models.split(","):
+        x = inputs[SIZES.get(arch, 224)]
         torch.manual_seed(0)
         base = getattr(torchvision.models, arch)(weights=None).to(device).to(memory_format=torch.channels_last)
         builds = args.builds.split(",")
@@ -115,7 +135,7 @@ def main():
             torch.manual_seed(1000 + steps[b])   # dropout and stochastic depth draw the same masks in both builds
             steps[b] += 1
             with torch.autocast("cuda", dtype=torch.bfloat16):
-                loss = F.cross_entropy(models[b](x).float(), y)
+                loss = loss_of(models[b](x), y)
             opts[b].zero_grad(set_to_none=True)
             loss.backward()
             opts[b].step()
@@ -158,7 +178,7 @@ def main():
         def host_step(b):
             torch.manual_seed(0)
             with torch.autocast("cuda", dtype=torch.bfloat16):
-                loss = F.cross_entropy(models[b](xs).float(), ys)
+                loss = loss_of(models[b](xs), ys)
             opts[b].zero_grad(set_to_none=True)
             loss.backward()
 
@@ -175,6 +195,15 @@ def main():
                 torch.cuda.synchronize()
                 host[b].append(round((time.perf_counter() - t0) / args.iters * 1e3, 2))
         entry["host_ms_per_step"] = {"batch": args.host_batch, **host}
+        peak = {}
+        for b in models:
+            models[b].train()
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            train_step(b)
+            torch.cuda.synchronize()
+            peak[b] = torch.cuda.max_memory_allocated()
+        entry["peak_train_bytes"] = peak
         profiled = {}
         for b in models:
             models[b].train()

@@ -132,6 +132,12 @@ SYMBOLS = {
     "b200c_bn_forward_slice": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_backward_slice": (c_int, [c_void_p, c_int] + [c_void_p] * 8 + [c_int, c_int, c_void_p, c_void_p]),
     "b200c_bn_infer_slice": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_float, c_int, c_int, c_void_p]),
+    "b200c_bn_shuffle_mask_bytes": (c_size_t, [c_int, c_int]),
+    "b200c_bn_forward_shuffle": (c_int, [c_void_p, c_int] + [c_void_p] * 9 + [c_float, c_float] + [c_void_p] * 9
+                                 + [c_float, c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_backward_shuffle": (c_int, [c_void_p] * 17 + [c_int, c_int, c_void_p, c_void_p]),
+    "b200c_bn_infer_shuffle": (c_int, [c_void_p, c_int] + [c_void_p] * 5 + [c_float] + [c_void_p] * 5
+                               + [c_float, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b200c_se_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200c_se_pool": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p]),
     "b200c_se_scale": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p]),

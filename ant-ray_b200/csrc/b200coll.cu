@@ -1870,6 +1870,80 @@ extern "C" int b200c_bn_infer_slice(const void* x, void* y, int ldy, const void*
   return B200C_OK;
 }
 
+// ShuffleNetV2's block end (norm_shuffle.cuh): the form (exactly one of x1 and u), the shape (n, hw >= 1, m = n * hw
+// >= min_m, channels 1..kMaxChannels / 2 since the two-batch-norm form takes the dual scratch, n * 2 * channels * hw
+// below 2^31) and x1's sample stride (at least channels * hw, its last element below 2^31).
+static int check_shuffle(const char* site, int min_m, const void* x1, int x1_stride, const void* u, int n, int hw, int c) {
+  if (!x1 == !u) return fail(B200C_EINVAL, "%s: exactly one of x1 and u must be given", site);
+  if (n < 1 || hw < 1 || (int64_t)n * hw < min_m || c < 1 || c > bn::kMaxChannels / 2 || (int64_t)n * 2 * c * hw > INT32_MAX)
+    return fail(B200C_EINVAL, "%s: bad shape n=%d hw=%d channels=%d", site, n, hw, c);
+  if (x1 && (x1_stride < (int64_t)c * hw || (int64_t)(n - 1) * x1_stride + (int64_t)c * hw > INT32_MAX))
+    return fail(B200C_EINVAL, "%s: x1's sample stride %d is below channels * hw or reaches past 2^31 elements", site, x1_stride);
+  return B200C_OK;
+}
+
+extern "C" size_t b200c_bn_shuffle_mask_bytes(int m, int channels) {
+  return m < 1 || channels < 1 || channels > bn::kMaxChannels / 2 || (int64_t)m * channels > INT32_MAX ? 0 : bn::shuffle_mask_bytes(m, channels);
+}
+
+extern "C" int b200c_bn_forward_shuffle(const void* x1, int x1_stride, const void* u, uint8_t* mask_u, const float* weight_u,
+                                        const float* bias_u, float* running_mean_u, float* running_var_u, int64_t* num_batches_tracked_u,
+                                        float* save_mean_u, float* save_invstd_u, float momentum_u, float eps_u, const void* t,
+                                        uint8_t* mask, const float* weight, const float* bias, float* running_mean, float* running_var,
+                                        int64_t* num_batches_tracked, float* save_mean, float* save_invstd, float momentum, float eps,
+                                        void* y, int n, int hw, int channels, void* scratch, b200c_stream_t stream) {
+  if (!t || !mask || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !y || !scratch ||
+      (u && (!mask_u || !weight_u || !bias_u || !running_mean_u || !running_var_u || !save_mean_u || !save_invstd_u)))
+    return fail(B200C_EINVAL, "batch norm shuffle forward: null buffer");
+  int rc = check_shuffle("batch norm shuffle", 2, x1, x1_stride, u, n, hw, channels);
+  if (rc) return rc;
+  const int m = n * hw;
+  const bn::FwdArgs a{t, nullptr, y, mask, true, weight, bias, running_mean, running_var,
+                      reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  const bn::FwdArgs b{u, nullptr, nullptr, mask_u, true, weight_u, bias_u, running_mean_u, running_var_u,
+                      reinterpret_cast<long long*>(num_batches_tracked_u), save_mean_u, save_invstd_u, m, channels, momentum_u, eps_u, scratch};
+  RT(bn::forward_shuffle(a, u ? &b : nullptr, x1, x1_stride, hw, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+// dy is read two channels at a time (4 bytes), so it sits on the 4-byte grid.
+extern "C" int b200c_bn_backward_shuffle(const void* dy, const void* u, const uint8_t* mask_u, void* du, const float* weight_u,
+                                         const float* save_mean_u, const float* save_invstd_u, float* grad_weight_u, float* grad_bias_u,
+                                         const void* t, const uint8_t* mask, void* dt, const float* weight, const float* save_mean,
+                                         const float* save_invstd, float* grad_weight, float* grad_bias, int m, int channels,
+                                         void* scratch, b200c_stream_t stream) {
+  if (!dy || !t || !mask || !dt || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias || !scratch ||
+      (u && (!mask_u || !du || !weight_u || !save_mean_u || !save_invstd_u || !grad_weight_u || !grad_bias_u)))
+    return fail(B200C_EINVAL, "batch norm shuffle backward: null buffer");
+  if (m < 2 || channels < 1 || channels > bn::kMaxChannels / 2 || (int64_t)m * 2 * channels > INT32_MAX)
+    return fail(B200C_EINVAL, "batch norm shuffle: bad shape m=%d channels=%d", m, channels);
+  if (reinterpret_cast<uintptr_t>(dy) % 4) return fail(B200C_EINVAL, "batch norm shuffle: dy is off the 4-byte grid");
+  const bn::BwdArgs a{dy, nullptr, nullptr, mask, t, nullptr, dt, true, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                      m, channels, scratch};
+  const bn::BwdArgs b{dy, nullptr, nullptr, mask_u, u, nullptr, du, true, weight_u, save_mean_u, save_invstd_u, nullptr, grad_weight_u,
+                      grad_bias_u, m, channels, scratch};
+  RT(bn::backward_shuffle(a, u ? &b : nullptr, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_shuffle(const void* x1, int x1_stride, const void* u, const void* weight_u, const void* bias_u,
+                                      const void* running_mean_u, const void* running_var_u, float eps_u, const void* t,
+                                      const void* weight, const void* bias, const void* running_mean, const void* running_var, float eps,
+                                      void* y, int param_bf16, int n, int hw, int channels, b200c_stream_t stream) {
+  if (!t || !weight || !bias || !running_mean || !running_var || !y || (u && (!weight_u || !bias_u || !running_mean_u || !running_var_u)))
+    return fail(B200C_EINVAL, "batch norm infer shuffle: null buffer");
+  int rc = check_shuffle("batch norm infer shuffle", 1, x1, x1_stride, u, n, hw, channels);
+  if (!rc) rc = check_infer("batch norm infer shuffle", param_bf16, n * hw, channels);
+  if (rc) return rc;
+  RT(bn::infer_shuffle({t, u, y, {weight, bias, running_mean, running_var, eps}, {weight_u, bias_u, running_mean_u, running_var_u, eps_u},
+                        u != nullptr, param_bf16 != 0, n * hw, channels, 0, 0},
+                       x1, x1_stride, hw, (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // squeeze-and-excitation (se_kernels.cuh, launched by inst_se.cu): one kernel per call
 // ------------------------------------------------------------------------------------------------

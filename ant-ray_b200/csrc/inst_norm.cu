@@ -1,5 +1,5 @@
 // Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh,
-// norm_slice.cuh); argument checking lives in b200coll.cu.
+// norm_slice.cuh, norm_shuffle.cuh); argument checking lives in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
@@ -10,6 +10,7 @@
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
 #include "norm_res.cuh"
+#include "norm_shuffle.cuh"
 #include "norm_slice.cuh"
 
 namespace b200c {
@@ -282,6 +283,16 @@ cudaError_t load_kernels() {
   load(&bn_slice::k_slice_bwd_elemt);
   load(&bn_slice::k_slice_infer<float>);
   load(&bn_slice::k_slice_infer<bf16>);
+  load(&bn_shuffle::k_shuffle_transform<false>);
+  load(&bn_shuffle::k_shuffle_transform<true>);
+  load(&bn_shuffle::k_shuffle_bwd_reduce<false>);
+  load(&bn_shuffle::k_shuffle_bwd_reduce<true>);
+  load(&bn_shuffle::k_shuffle_bwd_elemt<false>);
+  load(&bn_shuffle::k_shuffle_bwd_elemt<true>);
+  load(&bn_shuffle::k_shuffle_infer<false, float>);
+  load(&bn_shuffle::k_shuffle_infer<true, float>);
+  load(&bn_shuffle::k_shuffle_infer<false, bf16>);
+  load(&bn_shuffle::k_shuffle_infer<true, bf16>);
   for (int src = 0; src < kGradSrcs; src++) {
     load(bwd_reduce_kernel(src, false));
     load(bwd_reduce_kernel(src, true));
@@ -438,7 +449,8 @@ static float* dual_sum_xmu2(void* scratch, int c) { return dual_staging(scratch,
 
 // `a` is the tail's batch norm (y, mask), `b` the downsample branch's (its x, weight, bias, statistics); b's y and
 // mask are unused.
-cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
+// The statistics of both: k_bn_stats_dual, plane z taking k_bn_stats's launch shape for its own input.
+static cudaError_t launch_stats_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
   Scratch s = carve(a.scratch, a.c);
   dim3 block, grid;
   reduce_config(a.m, a.c, &block, &grid);
@@ -455,8 +467,13 @@ cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
               (float)((double)b.m / (double)(b.m - 1)), b.eps};
   ks<<<grid, block, smem, st>>>(static_cast<const bf16*>(a.x), static_cast<const bf16*>(b.x), oa, ob, s.staging,
                              dual_staging(a.scratch, a.c), s.semaphores, a.m, a.c);
-  cudaError_t e = cudaGetLastError();
+  return cudaGetLastError();
+}
+
+cudaError_t forward_dual(const FwdArgs& a, const FwdArgs& b, cudaStream_t st) {
+  const cudaError_t e = launch_stats_dual(a, b, st);
   if (e != cudaSuccess) return e;
+  dim3 block, grid;
   const void* ptrs[3] = {a.x, a.y, b.x};
   const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
   ew_config(a.m, a.c, vec, &block, &grid);
@@ -809,6 +826,78 @@ static cudaError_t launch_infer_slice(const InferArgs& a, int ldy, cudaStream_t 
 
 cudaError_t infer_slice(const InferArgs& a, int ldy, cudaStream_t st) {
   return a.param_bf16 ? launch_infer_slice<bf16>(a, ldy, st) : launch_infer_slice<float>(a, ldy, st);
+}
+
+// ---- ShuffleNetV2's block end (norm_shuffle.cuh) ----
+// The statistics are the local site's (k_bn_stats on t) or, with u, k_bn_stats_dual on (t, u) in the dual scratch;
+// the transform and eval launches cover the [m][B] rows with kTile x kTile tiles; the backward reduce takes
+// reduce_config's launch for [m][B] and the elementwise kernel ew_config's with one channel per thread.
+size_t shuffle_mask_bytes(int m, int c) { return (size_t)m * bn_shuffle::mask_row_bytes(c); }
+
+static dim3 shuffle_tiles(int m, int c) { return dim3(ceil_div(m, bn_shuffle::kTile), ceil_div(c, bn_shuffle::kTile), 1); }
+
+cudaError_t forward_shuffle(const FwdArgs& a, const FwdArgs* b, const void* x1, int x1_stride, int hw, cudaStream_t st) {
+  const cudaError_t e = b ? launch_stats_dual(a, *b, st) : launch_stats(a, nullptr, st);
+  if (e != cudaSuccess) return e;
+  const bn_shuffle::Geometry g{a.m, a.c, hw, static_cast<const bf16*>(x1), x1_stride};
+  const bn_shuffle::SavedStats sa{a.save_mean, a.save_invstd, a.weight, a.bias};
+  const bf16* t = static_cast<const bf16*>(a.x);
+  bf16* y = static_cast<bf16*>(a.y);
+  uint8_t* mask = static_cast<uint8_t*>(a.mask);
+  if (b) {
+    const bn_shuffle::SavedStats sb{b->save_mean, b->save_invstd, b->weight, b->bias};
+    bn_shuffle::k_shuffle_transform<true><<<shuffle_tiles(a.m, a.c), kEwThreads, 0, st>>>(t, static_cast<const bf16*>(b->x), y, mask,
+                                                                                           static_cast<uint8_t*>(b->mask), sa, sb, g);
+  } else {
+    bn_shuffle::k_shuffle_transform<false><<<shuffle_tiles(a.m, a.c), kEwThreads, 0, st>>>(t, nullptr, y, mask, nullptr, sa, sa, g);
+  }
+  return cudaGetLastError();
+}
+
+// t's sums go to the local layout (grad_bias holds Σg, sums + c Σg(x - mean)), u's to the dual scratch's second
+// staging plane and its sum_xmu2; both backward kernels read dy from a.dy.
+cudaError_t backward_shuffle(const BwdArgs& a, const BwdArgs* b, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  auto site = [](const BwdArgs& x, float* sum_xmu, float* staging) {
+    return bn_shuffle::BwdSite{static_cast<const bf16*>(x.x), static_cast<const uint8_t*>(x.mask), x.save_mean, x.save_invstd, x.weight,
+                               x.grad_weight, x.grad_bias, sum_xmu, staging, static_cast<bf16*>(x.dx)};
+  };
+  const bn_shuffle::BwdSite sa = site(a, s.sums + a.c, s.staging);
+  const bn_shuffle::BwdSite sb = b ? site(*b, dual_sum_xmu2(a.scratch, a.c), dual_staging(a.scratch, a.c)) : sa;
+  const bf16* dy = static_cast<const bf16*>(a.dy);
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  if (b) bn_shuffle::k_shuffle_bwd_reduce<true><<<grid, block, 0, st>>>(dy, sa, sb, s.semaphores, a.m, a.c);
+  else bn_shuffle::k_shuffle_bwd_reduce<false><<<grid, block, 0, st>>>(dy, sa, sb, s.semaphores, a.m, a.c);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  ew_config(a.m, a.c, 1, &block, &grid);
+  const float norm_fct = (float)(1.0 / a.m);
+  if (b) bn_shuffle::k_shuffle_bwd_elemt<true><<<grid, block, 0, st>>>(dy, sa, sb, norm_fct, a.m, a.c);
+  else bn_shuffle::k_shuffle_bwd_elemt<false><<<grid, block, 0, st>>>(dy, sa, sb, norm_fct, a.m, a.c);
+  return cudaGetLastError();
+}
+
+template <typename P>
+static cudaError_t launch_infer_shuffle(const InferArgs& a, const void* x1, int x1_stride, int hw, cudaStream_t st) {
+  auto stats = [](const InferParams& q) {
+    return bn_shuffle::RunningStats<P>{static_cast<const P*>(q.running_mean), static_cast<const P*>(q.running_var),
+                                       static_cast<const P*>(q.weight), static_cast<const P*>(q.bias), q.eps};
+  };
+  const bn_shuffle::Geometry g{a.m, a.c, hw, static_cast<const bf16*>(x1), x1_stride};
+  const bn_shuffle::RunningStats<P> sa = stats(a.bn);
+  const bf16* t = static_cast<const bf16*>(a.x);
+  bf16* y = static_cast<bf16*>(a.y);
+  if (a.dual)
+    bn_shuffle::k_shuffle_infer<true, P><<<shuffle_tiles(a.m, a.c), kEwThreads, 0, st>>>(t, static_cast<const bf16*>(a.identity), y, sa,
+                                                                                          stats(a.ds), g);
+  else
+    bn_shuffle::k_shuffle_infer<false, P><<<shuffle_tiles(a.m, a.c), kEwThreads, 0, st>>>(t, nullptr, y, sa, sa, g);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_shuffle(const InferArgs& a, const void* x1, int x1_stride, int hw, cudaStream_t st) {
+  return a.param_bf16 ? launch_infer_shuffle<bf16>(a, x1, x1_stride, hw, st) : launch_infer_shuffle<float>(a, x1, x1_stride, hw, st);
 }
 
 }  // namespace bn

@@ -149,5 +149,17 @@ cudaError_t forward_slice(const FwdArgs& a, int ldy, cudaStream_t s);
 cudaError_t backward_slice(const BwdArgs& a, int lddy, cudaStream_t s);
 cudaError_t infer_slice(const InferArgs& a, int ldy, cudaStream_t s);
 
+// ShuffleNetV2's block end, channel_shuffle(torch.cat((x1 or relu(bn_u(u)), relu(bn_t(t))), 1), 2) (norm_shuffle.cuh):
+// t and u are bf16 [m][c] rows (m = n * hw), y the contiguous NCHW [n][2c][hw] output, x1 NCHW planes x1_stride
+// elements apart per sample.  Each mask takes shuffle_mask_bytes(m, c).  A local training site: the forward reads `a`
+// (t's batch norm: x, y, mask, parameters, statistics, scratch) and with `b` u's (x, mask, parameters, statistics;
+// the dual scratch) instead of x1 (2 kernels); the backward reads a.dy, the channels-last [m][2c] gradient of y, and
+// each batch norm's x, mask, weight and statistics, and writes dx, grad_weight and grad_bias (2 kernels).  The eval
+// site reads InferArgs x (t), y and bn, and with `dual` identity (u) and ds instead of x1 (1 kernel).
+size_t shuffle_mask_bytes(int m, int c);
+cudaError_t forward_shuffle(const FwdArgs& a, const FwdArgs* b, const void* x1, int x1_stride, int hw, cudaStream_t s);
+cudaError_t backward_shuffle(const BwdArgs& a, const BwdArgs* b, cudaStream_t s);
+cudaError_t infer_shuffle(const InferArgs& a, const void* x1, int x1_stride, int hw, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

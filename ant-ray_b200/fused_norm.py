@@ -1,6 +1,6 @@
-"""Fused batch norm for the training step and eval forward of ResNets, DenseNets, Inception v3, GoogLeNet and
-torchvision's Conv2dNormActivation blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh,
-norm_cat.cuh, norm_slice.cuh), and the
+"""Fused batch norm for the training step and eval forward of ResNets, DenseNets, Inception v3, GoogLeNet, ShuffleNetV2
+and torchvision's Conv2dNormActivation blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh,
+norm_res.cuh, norm_cat.cuh, norm_slice.cuh, norm_shuffle.cuh), and the
 squeeze-and-excitation of EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
@@ -87,6 +87,19 @@ BasicConv2d, its batch norm or a GoogLeNet branch Sequential has a hook, a globa
 gradients recorded, the module runs its parent's forward, and where only the operands or the sites fail, it runs the
 batch norms and ReLUs as modules and torch.cat.  The convolutions run in torchvision's order before any branch's last
 batch norm, so the backward adds the module input's branch gradients in eager torch's order.
+
+ShuffleNetV2: `fuse_model` also swaps torchvision's ShuffleNetV2 `InvertedResidual` and `ShuffleNetV2`.  A block walks
+its branches module by module: branch2's first batch norm and ReLU is a bn_relu site, each batch norm after a depthwise
+convolution a bn_res site without identity, and the block's end, `channel_shuffle(torch.cat((x1 or branch1(x),
+branch2(x2)), 1), 2)`, is one block-end site (`bn_relu_shuffle`, norm_shuffle.cuh) over the branches' last batch norms
+and ReLUs that writes the shuffled, contiguous NCHW output directly: no branch output or concatenation is written, and
+the backward reads the output's gradient in place and gives x1 the gradient eager torch's view / transpose / reshape
+chain gives it.  The model's stem is a bn_relu_maxpool site and conv5 a bn_relu site.  Any branch width runs there (58
+and 116 are not multiples of 8).  A block runs there when its branch operands are bf16 channels-last CUDA tensors of
+one shape with at most 65536 channels, a stride-1 block's input is contiguous NCHW, and every site is an eval or a
+local site by the rules above; where a branch Sequential, a tail batch norm or its ReLU has a hook, a global hook is
+registered, or in eval with gradients recorded, the block runs its parent's forward, and where only the operands or the
+sites fail, the modules, torch.cat and channel_shuffle.  Block ends are never sync sites.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -827,6 +840,135 @@ def bn_relu_concat(branches):
     return torch.cat([F.relu(b[0](b[1]), inplace=True) if isinstance(b, tuple) else b for b in branches], 1)
 
 
+# the most channels a ShuffleNetV2 block end takes per branch: its two-batch-norm form runs in the dual scratch
+_MAX_SHUFFLE_CHANNELS = 65536
+
+
+def _shuffle_operands_ok(x1, sites):
+    """Whether a ShuffleNetV2 block end can run on the shuffle kernels: every site's input passes _activation with the
+    second one's shape and device, at most 65536 channels, an output of fewer than 2^31 elements, and a ready x1 is
+    bf16 of the same shape and device laid out as NCHW planes (what x.chunk(2, 1)[0] of a contiguous x is)."""
+    t = sites[-1][1]
+    if t.dim() != 4:
+        return False
+    n, c, h, w = t.shape
+    if c > _MAX_SHUFFLE_CHANNELS or 2 * t.numel() >= 2 ** 31:
+        return False
+    if any(not _activation(x) or x.shape != t.shape or x.device != t.device for _, x, _ in sites):
+        return False
+    if x1 is None:
+        return True
+    return (x1.dtype == torch.bfloat16 and x1.device == t.device and x1.shape == t.shape and x1.stride()[1:] == (h * w, w, 1)
+            and c * h * w <= x1.stride(0) < 2 ** 31)
+
+
+def _shuffle_first_grad(dy, b):
+    """The gradient eager torch's backward of `channel_shuffle(torch.cat((x1, z), 1), 2)` hands x1 for the output's
+    gradient dy: the view/transpose/reshape chain's, narrowed by CatBackward.  Its last reshape copies into a contiguous
+    [N, 2B, H, W] tensor unless B == 1 or dy's channel stride is 0 (an expanded gradient), where it is a view of dy; so
+    x1's gradient is channels 0..B-1 of such a tensor, of which only those channels are written here."""
+    n, _, h, w = dy.shape
+    if b == 1 or dy.stride(1) == 0:
+        return dy.reshape(n, b, 2, h, w).transpose(1, 2).reshape(n, 2 * b, h, w).narrow(1, 0, b)
+    return torch.empty(dy.shape, dtype=dy.dtype, device=dy.device).narrow(1, 0, b).copy_(dy[:, 0::2])
+
+
+class _FusedBatchNormShuffle(torch.autograd.Function):
+    """channel_shuffle(torch.cat((a, relu(bn_t(t))), 1), 2) in training mode, a being x1 (bn_u and u None) or
+    relu(bn_u(u)): the end of a ShuffleNetV2 block, one autograd node.  The forward writes the contiguous NCHW output
+    and each batch norm's mask bits (b200c_bn_forward_shuffle), never a branch output or the concatenation; the backward
+    reads dy channels-last (b200c_bn_backward_shuffle) and gives x1 the gradient eager torch gives it
+    (_shuffle_first_grad), values and strides."""
+
+    @staticmethod
+    def forward(ctx, bn_t, bn_u, x1, t, weight, bias, u, weight_u, bias_u):
+        lib = _native_lib()
+        n, c, h, w = t.shape
+        m = n * h * w
+        two = u is not None
+        y = torch.empty((n, 2 * c, h, w), dtype=torch.bfloat16, device=t.device)
+        mask_bytes = lib.b200c_bn_shuffle_mask_bytes(m, c)
+        mask = torch.empty(mask_bytes, dtype=torch.uint8, device=t.device)
+        stats, params, stream, scratch = _forward_args(t, bn_t, weight, bias, dual=two)
+        mask_u = stats_u = None
+        if two:
+            mask_u = torch.empty(mask_bytes, dtype=torch.uint8, device=t.device)
+            stats_u, params_u, _, _ = _forward_args(u, bn_u, weight_u, bias_u, dual=True)
+            first = (None, 0, u.data_ptr(), mask_u.data_ptr(), *params_u, bn_u.momentum, bn_u.eps)
+        else:
+            first = (x1.data_ptr(), x1.stride(0), None, None, *(None,) * 7, 0.0, 0.0)
+        N.check(lib.b200c_bn_forward_shuffle(*first, t.data_ptr(), mask.data_ptr(), *params, bn_t.momentum, bn_t.eps, y.data_ptr(),
+                                             n, h * w, c, scratch, stream))
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(t, mask, weight, stats, u, mask_u, weight_u, stats_u)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return (None,) * 9
+        t, mask, weight, stats, u, mask_u, weight_u, stats_u = ctx.saved_tensors
+        n, c, h, w = t.shape
+        two = u is not None
+        g = _rows_of(dy)
+        dt, grad_weight, grad_bias, stream, scratch = _backward_args(t, dual=two)
+        mean = stats.data_ptr()
+        first = (None,) * 8
+        if two:
+            du, grad_weight_u, grad_bias_u, _, _ = _backward_args(u, dual=True)
+            mean_u = stats_u.data_ptr()
+            first = (u.data_ptr(), mask_u.data_ptr(), du.data_ptr(), weight_u.data_ptr(), mean_u, mean_u + 4 * c,
+                     grad_weight_u.data_ptr(), grad_bias_u.data_ptr())
+        N.check(_native_lib().b200c_bn_backward_shuffle(g.data_ptr(), *first, t.data_ptr(), mask.data_ptr(), dt.data_ptr(),
+                                                        weight.data_ptr(), mean, mean + 4 * c, grad_weight.data_ptr(),
+                                                        grad_bias.data_ptr(), n * h * w, c, scratch, stream))
+        if two:
+            return None, None, None, dt, grad_weight, grad_bias, du, grad_weight_u, grad_bias_u
+        dx1 = _shuffle_first_grad(dy, c) if ctx.needs_input_grad[2] else None
+        return None, None, dx1, dt, grad_weight, grad_bias, None, None, None
+
+
+def bn_relu_shuffle(first, second):
+    """channel_shuffle(torch.cat((a, relu(bn(t))), 1), 2), the end of torchvision's ShuffleNetV2 block, with eager torch's
+    bits and strides.  `second` is a batch-norm site `(bn, t, mods)`, `first` either one `(bn, u, mods)` (a stride-2
+    block's branch1, a = relu(bn(u))) or the ready tensor a = x1 (a stride-1 block's x.chunk(2, 1)[0]); `mods` are the
+    other modules whose calls the site replaces, whose hooks `_site` checks.  The output is contiguous NCHW, as
+    channel_shuffle's .contiguous() leaves it.
+
+    Every site is decided by `_site` (never a sync site), with x1 among the inputs an eval site must not record a
+    gradient for.  Where every site is an eval site the block end is one b200c_bn_infer_shuffle launch; where every site
+    is a local training site, one _FusedBatchNormShuffle node.  Anything else (operands _shuffle_operands_ok refuses, a
+    site that runs its modules, or eval and training mixed) runs the batch norms and ReLUs as modules, torch.cat and
+    torchvision's channel_shuffle."""
+    sites = [first, second] if isinstance(first, tuple) else [second]
+    x1 = None if isinstance(first, tuple) else first
+    kinds = set()
+    if _shuffle_operands_ok(x1, sites):
+        kinds = {_site(bn, x, mods, sync=False, inputs=() if x1 is None else (x1,)) for bn, x, mods in sites}
+    bn_t, t = second[0], second[1]
+    bn_u, u = (first[0], first[1]) if x1 is None else (None, None)
+    if kinds == {_EVAL} and (u is None or bn_u.weight.dtype == bn_t.weight.dtype):
+        n, c, h, w = t.shape
+        y = torch.empty((n, 2 * c, h, w), dtype=torch.bfloat16, device=t.device)
+        p = _infer_params(bn_t)
+        if u is None:
+            lead = (x1.data_ptr(), x1.stride(0), None, None, None, None, None, 0.0)
+        else:
+            lead = (None, 0, u.data_ptr(), *_infer_params(bn_u)[:4], bn_u.eps)
+        N.check(_native_lib().b200c_bn_infer_shuffle(*lead, t.data_ptr(), *p[:4], bn_t.eps, y.data_ptr(), p[4], n, h * w, c,
+                                                     _raw_stream(t.device.index)))
+        return y
+    if kinds == {_LOCAL}:
+        if u is None:
+            return _FusedBatchNormShuffle.apply(bn_t, None, x1, t, bn_t.weight, bn_t.bias, None, None, None)
+        return _FusedBatchNormShuffle.apply(bn_t, bn_u, None, t, bn_t.weight, bn_t.bias, u, bn_u.weight, bn_u.bias)
+    from torchvision.models.shufflenetv2 import channel_shuffle
+
+    a = x1 if u is None else F.relu(bn_u(u), inplace=True)
+    return channel_shuffle(torch.cat((a, F.relu(bn_t(t), inplace=True)), 1), 2)
+
+
 # activations with native batch-norm sites of their own, by their b200c_act_t (ReLU runs on bn_relu's sites)
 _ACT_CODES = {nn.ReLU6: N.ACT_RELU6, nn.SiLU: N.ACT_SILU, nn.Hardswish: N.ACT_HARDSWISH}
 
@@ -1366,6 +1508,81 @@ else:
                    _inception.InceptionE: FusedInceptionE, _googlenet.Inception: FusedInception}
 
 
+try:
+    from torchvision.models import shufflenetv2
+except ImportError:  # without torchvision there is nothing to rewrite
+    _SHUFFLE_SWAP = {}
+else:
+
+    _BN_CLASSES = (nn.BatchNorm2d, nn.SyncBatchNorm)
+
+    def _is_seq(seq, classes):
+        """Whether `seq` is exactly an nn.Sequential of modules of `classes`, in order (a batch norm BatchNorm2d or
+        SyncBatchNorm)."""
+        if type(seq) is not nn.Sequential or len(seq) != len(classes):
+            return False
+        return all(isinstance(m, _BN_CLASSES) if cls is nn.BatchNorm2d else type(m) is cls for m, cls in zip(seq, classes))
+
+    # torchvision's branches: branch1 (stride 2) depthwise conv, bn, 1x1 conv, bn, ReLU; branch2 1x1 conv, bn, ReLU,
+    # depthwise conv, bn, 1x1 conv, bn, ReLU
+    _BRANCH1 = (nn.Conv2d, nn.BatchNorm2d, nn.Conv2d, nn.BatchNorm2d, nn.ReLU)
+    _BRANCH2 = (nn.Conv2d, nn.BatchNorm2d, nn.ReLU, nn.Conv2d, nn.BatchNorm2d, nn.Conv2d, nn.BatchNorm2d, nn.ReLU)
+
+    def _shuffle_forward(block, x):
+        """A ShuffleNetV2 block's output with its branches walked module by module and its end one bn_relu_shuffle, or
+        None where the parent's forward must run: eval with gradients recorded, a branch that is not exactly
+        torchvision's, or a hook that the walk would skip (on a branch Sequential, a tail batch norm or its ReLU, or a
+        global one).  Every module the walk calls runs its own hooks."""
+        if not block.training and torch.is_grad_enabled():
+            return None
+        b1, b2 = block.branch1, block.branch2
+        if not _is_seq(b2, _BRANCH2) or not _is_seq(b1, _BRANCH1 if block.stride > 1 else ()):
+            return None
+        tails = (b2, b2[6], b2[7]) + ((b1, b1[3], b1[4]) if block.stride > 1 else ())
+        if _skips_hooks(*tails):
+            return None
+        if block.stride == 1:
+            x1, x2 = x.chunk(2, dim=1)
+            first = x1
+        else:
+            x2 = x
+            first = (b1[3], b1[2](bn_res(b1[1], b1[0](x))), (b1[4], b1))
+        out = bn_relu(b2[1], b2[2], b2[0](x2))
+        out = b2[5](bn_res(b2[4], b2[3](out)))
+        return bn_relu_shuffle(first, (b2[6], out, (b2[7], b2)))
+
+    class FusedShuffleInvertedResidual(shufflenetv2.InvertedResidual):
+        """ShuffleNetV2's block whose branches run module by module: each first batch norm and ReLU of branch2 a bn_relu
+        site, each batch norm after a depthwise convolution a bn_res site, and the branch ends with torch.cat and
+        channel_shuffle one bn_relu_shuffle site that writes the shuffled output directly."""
+
+        def forward(self, x):
+            out = _shuffle_forward(self, x)
+            return super().forward(x) if out is None else out
+
+    def _stem_ok(seq):
+        """Whether ShuffleNetV2's conv1 or conv5 `seq` is exactly nn.Sequential(Conv2d, batch norm, ReLU) with no hook on
+        it or its parts."""
+        return _is_seq(seq, (nn.Conv2d, nn.BatchNorm2d, nn.ReLU)) and not any(map(_hooked, (seq, *seq)))
+
+    class FusedShuffleNetV2(shufflenetv2.ShuffleNetV2):
+        """ShuffleNetV2 whose conv1, batch norm, ReLU and max-pool stem is one bn_relu_maxpool site and whose conv5 batch
+        norm and ReLU is a bn_relu site; the stages, the mean and fc run as torchvision runs them.  Hooks on conv1,
+        conv5 or their parts, a global hook, and eval with gradients recorded run the parent's forward (whose blocks
+        still fuse)."""
+
+        def forward(self, x):
+            if (not self.training and torch.is_grad_enabled()) or not (_stem_ok(self.conv1) and _stem_ok(self.conv5)) or _global_hooks():
+                return super().forward(x)
+            c1, c5 = self.conv1, self.conv5
+            x = bn_relu_maxpool(c1[1], c1[2], self.maxpool, c1[0](x))
+            x = self.stage4(self.stage3(self.stage2(x)))
+            x = bn_relu(c5[1], c5[2], c5[0](x))
+            return self.fc(x.mean([2, 3]))
+
+    _SHUFFLE_SWAP = {shufflenetv2.InvertedResidual: FusedShuffleInvertedResidual, shufflenetv2.ShuffleNetV2: FusedShuffleNetV2}
+
+
 # Torch sums a tensor of fewer elements than this (2^31 bytes of bf16) in one launch of its reduce kernel, whose order
 # the squeeze-excitation kernels restate; a larger one it splits into 32-bit-indexed pieces.
 _SE_MAX_NUMEL = 2 ** 30
@@ -1551,7 +1768,10 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module w
     sites (`bn_relu_cat`).  Every module whose class is exactly torchvision's Inception v3 or GoogLeNet BasicConv2d,
     InceptionA to InceptionE or GoogLeNet's Inception gets the fused subclass: BasicConv2d's batch norm and ReLU run as
     a bn_relu site, and each Inception module's branches write their last batch norm and ReLU into their channels of the
-    module's output (`bn_relu_concat`).  Parameters, buffers, state_dict keys, hooks and the
+    module's output (`bn_relu_concat`).  Every module whose class is exactly torchvision's ShuffleNetV2 or its
+    InvertedResidual gets the fused subclass: the stem is one bn_relu_maxpool site, conv5 a bn_relu site, and each
+    block's branches run module by module into one block-end site that writes the shuffled output directly
+    (`bn_relu_shuffle`).  Parameters, buffers, state_dict keys, hooks and the
     object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
     training and in eval (see `fuse_resnet` for inference).
 
@@ -1564,7 +1784,7 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module w
         for mod in model.modules():
             if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
                 mod.__class__ = FusedConv2dNormActivation
-    swap = {**_RES_SWAP, **_DENSE_SWAP, **_SLICE_SWAP}
+    swap = {**_RES_SWAP, **_DENSE_SWAP, **_SLICE_SWAP, **_SHUFFLE_SWAP}
     for mod in model.modules():
         cls = swap.get(type(mod))
         if cls is not None:

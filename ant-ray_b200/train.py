@@ -127,8 +127,9 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     reference returns the bare model there).  The returned module carries `.b200_grad_state`.  On a CUDA device a
     torchvision ResNet, every torchvision Conv2dNormActivation ending in ReLU6, SiLU or Hardswish (MobileNetV2 / V3,
     EfficientNet), the inverted-residual blocks with their projection batch norm and squeeze-and-excitation, a
-    torchvision DenseNet (whose concatenating batch norms then read the feature maps in place), and torchvision's
-    Inception v3 and GoogLeNet (whose Inception modules' branches then write into their concatenation in place), is first
+    torchvision DenseNet (whose concatenating batch norms then read the feature maps in place), torchvision's
+    Inception v3 and GoogLeNet (whose Inception modules' branches then write into their concatenation in place), and
+    torchvision's ShuffleNetV2 (whose blocks' branch ends then write the shuffled block output directly), is first
     rewritten in place by `fused_norm.fuse_model`, and with more than one rank the
     model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
     communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten blocks'

@@ -479,6 +479,42 @@ int b200c_bn_backward_slice(const void* dy, int lddy, const uint8_t* mask, const
 int b200c_bn_infer_slice(const void* x, void* y, int ldy, const void* weight, const void* bias, const void* running_mean,
                          const void* running_var, int param_bf16, float eps, int m, int channels, b200c_stream_t stream);
 
+/* ---- fused batch norms and ReLU into ShuffleNetV2's shuffled block output ----
+ * The end of torchvision's ShuffleNetV2 InvertedResidual, channel_shuffle(torch.cat((a, relu(bn(t))), 1), 2), with a
+ * either the block input's first half x1 (stride 1: one batch norm) or relu(bn_u(u)) (stride 2: a second batch norm
+ * on u), written straight into its bf16 output y, contiguous NCHW [n][2 * channels][hw]: channel 2c is a's channel c,
+ * channel 2c + 1 is relu(bn(t))'s.  t and u are channels-last bf16 [m][channels], m = n * hw, any channels in
+ * 1..65536 with n * 2 * channels * hw below 2^31; x1 is NCHW planes, element (n, c, p) at x1 + n * x1_stride + c * hw +
+ * p.  Exactly one of x1 and u is given.  Every result has the bits of eager torch's modules, cat and channel_shuffle
+ * (bf16 autocast); no branch output or concatenation is written.
+ *
+ * Each batch norm's ReLU predicate is kept as bits in b200c_bn_shuffle_mask_bytes(m, channels) bytes (ceil(channels /
+ * 8) per row; 0 for a bad shape); the layout is private to these calls.  A site's scratch is b200c_bn_scratch_bytes
+ * (one batch norm) or b200c_bn_dual_scratch_bytes (two) of channels.
+ *
+ * b200c_bn_forward_shuffle: training forward, m >= 2: statistics, running statistics and num_batches_tracked (may be
+ *   null) of each batch norm, y and the masks.  2 launches.
+ * b200c_bn_backward_shuffle: from dy, y's gradient as channels-last bf16 [m][2 * channels] on the 4-byte grid, each
+ *   batch norm's mask, input, weight and saved statistics: dt (and du), grad_weight and grad_bias.  u null: the
+ *   one-batch-norm form, whose x1 gradient is dy's even channels.  2 launches.
+ * b200c_bn_infer_shuffle: eval, m >= 1, weight, bias and running statistics all fp32 (param_bf16 0) or all bf16 (1):
+ *   y alone.  1 launch. */
+size_t b200c_bn_shuffle_mask_bytes(int m, int channels);
+int b200c_bn_forward_shuffle(const void* x1, int x1_stride, const void* u, uint8_t* mask_u, const float* weight_u, const float* bias_u,
+                             float* running_mean_u, float* running_var_u, int64_t* num_batches_tracked_u, float* save_mean_u,
+                             float* save_invstd_u, float momentum_u, float eps_u, const void* t, uint8_t* mask, const float* weight,
+                             const float* bias, float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                             float* save_invstd, float momentum, float eps, void* y, int n, int hw, int channels, void* scratch,
+                             b200c_stream_t stream);
+int b200c_bn_backward_shuffle(const void* dy, const void* u, const uint8_t* mask_u, void* du, const float* weight_u, const float* save_mean_u,
+                              const float* save_invstd_u, float* grad_weight_u, float* grad_bias_u, const void* t, const uint8_t* mask,
+                              void* dt, const float* weight, const float* save_mean, const float* save_invstd, float* grad_weight,
+                              float* grad_bias, int m, int channels, void* scratch, b200c_stream_t stream);
+int b200c_bn_infer_shuffle(const void* x1, int x1_stride, const void* u, const void* weight_u, const void* bias_u, const void* running_mean_u,
+                           const void* running_var_u, float eps_u, const void* t, const void* weight, const void* bias,
+                           const void* running_mean, const void* running_var, float eps, void* y, int param_bf16, int n, int hw,
+                           int channels, b200c_stream_t stream);
+
 /* ---- squeeze-and-excitation (torchvision's SqueezeExcitation without its squeeze path) ----
  * Over channels-last bf16 activations x, y, dy, dx of n samples, hw = H * W rows per sample and `channels` channels
  * ([n][hw][channels]), and bf16 per-sample vectors pooled, s, ds, gp of [n][channels]; bit-identical to eager torch:

@@ -12,7 +12,19 @@ iterations of a 128-row grid), and at (16383, 131072), the most channels:
 - eval sites at the first shape: b200c_bn_infer with an identity (fp32 parameters), and b200c_bn_infer_act (Hardswish)
   and b200c_bn_infer_res with an identity (bf16 parameters);
 - concatenation sites (b200c_bn_forward_cat / b200c_bn_backward_cat / b200c_bn_infer_cat) at both shapes: segments of
-  (8, 16, 40) channels at the first, 64 segments of 2048 at the second.
+  (8, 16, 40) channels at the first, 64 segments of 2048 at the second;
+- slice sites (b200c_bn_forward_slice / b200c_bn_backward_slice / b200c_bn_infer_slice): the whole [33554431][64]
+  output (ldy = lddy = 64, m * ldy = 2^31 - 64), and at (16383, 131072) the slice at c0 = 8 of rows of ldy = lddy =
+  131080 channels, which ends at the row's last channel (m * ldy = 2^31 - 8), with a pattern in the channels before it.
+The shuffle sites (b200c_bn_forward_shuffle / b200c_bn_backward_shuffle) admit n * 2B * hw up to 2^31 - 1 and index
+y, dy and x1 with size_t, the masks by rows of ceil(B / 8) bytes.  Both forms run at (n, B, h, w) = (8192, 65535, 1,
+2): the most channels with B odd (2048 channel tiles, the last partial; 8192-byte mask rows with one padding bit; the
+dual scratch at its largest); and at (377812, 58, 7, 7): 18512788 rows, whose 32-row tiles cross sample boundaries up
+to the top of the index range.  The one-batch-norm form runs at B = 1, h * w = 49 and n = (2^31 - 1) // 98: the
+longest backward-reduce walk (block (1, 512), 128 rows of blocks, about 16,000 rows per thread) and one mask byte with
+7 padding bits per row.  x1 is the first half of each sample of the block input, y's planes are compared with torch's
+batch norm and ReLU and with x1, each mask with its bit rule, and the saved statistics with float64 sums taken over
+slices of rows.
 Every output is filled with all-ones bits (a NaN) before its call, so an element no thread writes shows.
 
 The squeeze-and-excitation calls admit n * c * hw up to 2^31 - 1, where torch splits its own reduction (so no torch
@@ -26,15 +38,19 @@ Each tensor is 4 GiB.  Comparisons stay on the device (torch.equal of int16 view
 and the work runs in phases that free what they no longer need.  Each test prints its peak allocation.  On an NVIDIA
 H100 80GB HBM3 (700 W power limit) they peaked at 30.3 and 30.5 GiB for the ReLU sites, 30.0 and 30.2 GiB for the
 SiLU sites, 30.1 and 30.2 GiB for the stochastic-depth sites, 18.0 GiB for each eval test, 30.0 and 30.2 GiB for the
-concatenation sites, and 14.0, 14.0, 14.0 and 24.0 GiB for the squeeze-and-excitation sites.  The tests skip, saying
+concatenation sites, 26.0 and 26.2 GiB for the slice sites, 17.2 and 24.5 GiB for the 65535-channel shuffle sites
+(one and two batch norms), 17.1 and 24.3 GiB for the 58-channel ones, 18.0 GiB for the one-channel one, and 14.0,
+14.0, 14.0 and 24.0 GiB for the squeeze-and-excitation sites.  The tests skip, saying
 so, where the GPU has less than NEED free."""
 import ctypes
+import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
 from ant_ray_b200 import _native as N
+from gpu_common import BnLaunch, bn_launch_config
 from test_fused_se_cpu import se_reduce_config
 from test_gpu_bn_act_res_abi import row_noise
 from test_gpu_fused_norm import GUARD, check_scratch, check_stats_against_float64, make_bn
@@ -81,8 +97,24 @@ def check_mask(mask, y):
         assert torch.equal(mask[i // 8:(i + CHUNK) // 8], want), f"mask bytes {i // 8}.. differ"
 
 
-def scratch(c):
-    need = int(N.load().b200c_bn_scratch_bytes(c))
+def check_shuffle_mask(mask, y):
+    """The shuffle sites' mask of one batch norm whose output rows are y [m][B]: bit c % 8 of byte r * ceil(B / 8) +
+    c / 8 is !(y[r, c] <= 0), and the bits of each row's padding channels are 0."""
+    m, c = y.shape
+    mb = -(-c // 8)
+    assert mask.shape == (m * mb,), "mask length"
+    weights = (1 << torch.arange(8, device="cuda", dtype=torch.int32)).view(1, 1, 8)
+    rows = max(1, CHUNK // (8 * mb))
+    for i in range(0, m, rows):
+        j = min(m, i + rows)
+        bits = torch.zeros(j - i, 8 * mb, dtype=torch.int32, device="cuda")
+        bits[:, :c] = ~(y[i:j].float() <= 0)
+        want = (bits.view(j - i, mb, 8) * weights).sum(2).to(torch.uint8)
+        assert torch.equal(mask.view(m, mb)[i:j], want), f"mask rows {i}.. differ"
+
+
+def scratch(c, dual=False):
+    need = int(N.load().b200c_bn_dual_scratch_bytes(c) if dual else N.load().b200c_bn_scratch_bytes(c))
     buf = torch.empty(need + GUARD, dtype=torch.uint8, device="cuda")
     buf[:need].zero_()
     buf[need:].fill_(0xA5)
@@ -346,6 +378,186 @@ def test_largest_cat_site_matches_torch(room, m, chans):
     with torch.no_grad():
         want = torch.relu_(bn.eval()(x4))
     same(y, want.view(m, c), "eval y")
+
+
+# ---- slice sites --------------------------------------------------------------------------------------------------
+OUT_PATTERN = 0x3F5A   # a bf16 outside the slice, which no call writes
+
+
+@pytest.mark.parametrize("m,c,ldy,c0", [(*SITES[0], 64, 0), (*SITES[1], 131080, 8)], ids=["whole_output", "last_slice"])
+def test_largest_slice_site_matches_torch(room, m, c, ldy, c0):
+    # y is out[:, c0:c0 + c] of an [m][ldy] output and ends at the row's last channel; dy has the same row stride
+    assert c0 + c == ldy and 2 ** 31 - 64 <= m * ldy <= 2 ** 31 - 1
+    lib = N.load()
+    s = torch.cuda.current_stream().cuda_stream
+    bn = make_bn(c, 40)
+    w, b = bn.weight.detach(), bn.bias.detach()
+    x = seeded(m, c, 41, 2.0, 0.5)
+    buf, need = scratch(c)
+
+    # forward: the native site into a patterned output, then torch's batch norm and ReLU, compared and freed
+    rm, rv, nbt = bn.running_mean.clone(), bn.running_var.clone(), bn.num_batches_tracked.clone()
+    mean, invstd = nan_filled(c, dtype=torch.float32), nan_filled(c, dtype=torch.float32)
+    out, mask = torch.empty(m, ldy, dtype=torch.bfloat16, device="cuda"), nan_filled(m * c // 8, dtype=torch.uint8)
+    out.view(torch.int16).fill_(OUT_PATTERN)
+    N.check(lib.b200c_bn_forward_slice(x.data_ptr(), out.data_ptr() + 2 * c0, ldy, mask.data_ptr(), w.data_ptr(), b.data_ptr(),
+                                       rm.data_ptr(), rv.data_ptr(), nbt.data_ptr(), mean.data_ptr(), invstd.data_ptr(), m, c, 0.1, 1e-5,
+                                       buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    assert int(nbt) == int(bn.num_batches_tracked) + 1
+    check_stats_against_float64(x, {"mean": mean, "invstd": invstd})
+    rm_t, rv_t = bn.running_mean.clone(), bn.running_var.clone()
+    x4 = x.view(m, c, 1, 1)   # NCHW strides with stride(1) == 1: torch's channels-last kernels
+    y_t, mean_t, invstd_t = torch.native_batch_norm(x4, w, b, rm_t, rv_t, True, 0.1, 1e-5)
+    torch.relu_(y_t)
+    for got, want, what in ((mean, mean_t, "save_mean"), (invstd, invstd_t, "save_invstd"), (rm, rm_t, "running_mean"),
+                            (rv, rv_t, "running_var"), (out[:, c0:], y_t.view(m, c), "y")):
+        same(got, want, what)
+    assert bool((out[:, :c0].view(torch.int16) == OUT_PATTERN).all()), "a write outside the slice"
+    check_mask(mask, y_t.view(m, c))
+    del out
+
+    # backward: the native call from dy's slice, then torch's g (which needs y, then freed) and dx
+    dy = seeded(m, ldy, 42, 1.0, 0.0)
+    dx = nan_filled(m, c)
+    dw, db = nan_filled(c, dtype=torch.float32), nan_filled(c, dtype=torch.float32)
+    N.check(lib.b200c_bn_backward_slice(dy.data_ptr() + 2 * c0, ldy, mask.data_ptr(), x.data_ptr(), dx.data_ptr(), w.data_ptr(),
+                                        mean.data_ptr(), invstd.data_ptr(), dw.data_ptr(), db.data_ptr(), m, c, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    g_t = torch.ops.aten.threshold_backward(dy[:, c0:], y_t.view(m, c), 0).reshape(m, c, 1, 1)
+    del dy, y_t, mask
+    dx_t, dw_t, db_t = torch.ops.aten.native_batch_norm_backward(g_t, x4, w, rm_t, rv_t, mean_t, invstd_t, True, 1e-5,
+                                                                 [True, True, True])
+    same(dx, dx_t.view(m, c), "dx")
+    same(dw, dw_t, "dweight")
+    same(db, db_t, "dbias")
+    del dx, dx_t, g_t
+
+    # eval: fp32 parameters into a fresh pattern, eager torch's eval-mode module and ReLU
+    out = torch.empty(m, ldy, dtype=torch.bfloat16, device="cuda")
+    out.view(torch.int16).fill_(OUT_PATTERN)
+    N.check(lib.b200c_bn_infer_slice(x.data_ptr(), out.data_ptr() + 2 * c0, ldy, w.data_ptr(), b.data_ptr(), bn.running_mean.data_ptr(),
+                                     bn.running_var.data_ptr(), 0, 1e-5, m, c, s))
+    with torch.no_grad():
+        want = torch.relu_(bn.eval()(x4))
+    same(out[:, c0:], want.view(m, c), "eval y")
+    assert bool((out[:, :c0].view(torch.int16) == OUT_PATTERN).all()), "an eval write outside the slice"
+
+
+# ---- shuffle sites ------------------------------------------------------------------------------------------------
+# (n, B, h, w, two batch norms): the most channels with B odd (2048 channel tiles, the last partial, 8192-byte mask rows
+# with one padding bit, the dual scratch at its largest); 18512788 rows of 58 channels, whose 32-row tiles cross
+# sample boundaries up to the top of the index range; and B = 1, the longest backward-reduce walk (block (1, 512), 128
+# rows of blocks) with one mask byte of 7 padding bits per row.  h * w > 1 everywhere: with h = w = 1 torch's choice of
+# kernel would follow its layout guess.
+SHUFFLE_SITES = [(8192, 65535, 1, 2, False), (8192, 65535, 1, 2, True), (377812, 58, 7, 7, False), (377812, 58, 7, 7, True),
+                 ((2 ** 31 - 1) // 98, 1, 7, 7, False)]
+
+
+def check_stats_by_rows(x, mean, invstd):
+    """check_stats_against_float64's bounds, with the float64 sums taken over slices of rows: one channel of a billion
+    rows has no float64 copy beside the site."""
+    m, c = x.shape
+    cfg = bn_launch_config(m, c)
+    k = -(-m // (cfg.block_y * cfg.grid_y)) + 2 * math.log2(m)
+    u = 2.0 ** -24
+    rows = max(1, CHUNK // c)
+    total, amax = torch.zeros(c, dtype=torch.float64, device="cuda"), torch.zeros(c, dtype=torch.float64, device="cuda")
+    for i in range(0, m, rows):
+        x64 = x[i:i + rows].double()
+        total += x64.sum(0)
+        amax = torch.maximum(amax, x64.abs().amax(0))
+    mean64 = total / m
+    dev, sq = torch.zeros_like(total), torch.zeros_like(total)
+    for i in range(0, m, rows):
+        x64 = x[i:i + rows].double()
+        dev += ((x64 - mean64) ** 2).sum(0)
+        sq += (x64 ** 2).sum(0)
+    var_got = 1 / invstd.double() ** 2 - 1e-5
+    assert bool(((mean.double() - mean64).abs() <= 4 * k * u * amax).all()), "save_mean"
+    assert bool(((var_got - dev / m).abs() <= 8 * k * u * sq / m).all()), "save_invstd"
+
+
+@pytest.mark.parametrize("n,c,h,w,two", SHUFFLE_SITES, ids=["65535_one", "65535_two", "58_one", "58_two", "1_one"])
+def test_largest_shuffle_site_matches_torch(room, n, c, h, w, two):
+    hw = h * w
+    m = n * hw
+    assert hw > 1 and 2 ** 31 - 2 ** 15 <= n * 2 * c * hw <= 2 ** 31 - 1
+    cfg = bn_launch_config(m, c)
+    print(f"backward reduce {cfg}")
+    if c == 1:
+        assert cfg == BnLaunch(1, 512, 1, 128)
+    lib = N.load()
+    s = torch.cuda.current_stream().cuda_stream
+    nb = 2 if two else 1
+    bns = [make_bn(c, 50 + i) for i in range(nb)]
+    xs = [seeded(m, c, 52 + i, 1.5, -0.2) for i in range(nb)]   # t, then u: channels-last [m][B] rows
+    x = None if two else seeded(n, 2 * c * hw, 54, 2.0, 0.5)    # the block input, whose first half is x1
+    buf, need = scratch(c, two)
+
+    # forward: the native site, then torch's batch norms and ReLU, compared plane by plane
+    mb = int(lib.b200c_bn_shuffle_mask_bytes(m, c))
+    assert mb == m * -(-c // 8)
+    y = nan_filled(n * 2 * c * hw)
+    st, ref = [], []
+    for bn in bns:
+        st.append({"mask": nan_filled(mb, dtype=torch.uint8), "rm": bn.running_mean.clone(), "rv": bn.running_var.clone(),
+                   "nbt": bn.num_batches_tracked.clone(), "mean": nan_filled(c, dtype=torch.float32),
+                   "invstd": nan_filled(c, dtype=torch.float32)})
+
+    def fwd(bn, o):
+        return (o["mask"].data_ptr(), bn.weight.data_ptr(), bn.bias.data_ptr(), o["rm"].data_ptr(), o["rv"].data_ptr(), o["nbt"].data_ptr(),
+                o["mean"].data_ptr(), o["invstd"].data_ptr(), 0.1, 1e-5)
+
+    lead = (None, 0, xs[1].data_ptr(), *fwd(bns[1], st[1])) if two else (x.data_ptr(), 2 * c * hw, None, *(None,) * 8, 0.0, 0.0)
+    N.check(lib.b200c_bn_forward_shuffle(*lead, xs[0].data_ptr(), *fwd(bns[0], st[0]), y.data_ptr(), n, hw, c, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    planes = y.view(n, c, 2, hw)   # [..., 1, :] relu(bn_t(t)), [..., 0, :] the lead
+    for i, (bn, o) in enumerate(zip(bns, st)):
+        assert int(o["nbt"]) == int(bn.num_batches_tracked) + 1
+        check_stats_by_rows(xs[i], o["mean"], o["invstd"])
+        rm_t, rv_t = bn.running_mean.clone(), bn.running_var.clone()
+        y_t, mean_t, invstd_t = torch.native_batch_norm(xs[i].view(m, c, 1, 1), bn.weight.detach(), bn.bias.detach(), rm_t, rv_t,
+                                                        True, 0.1, 1e-5)
+        torch.relu_(y_t)
+        for got, want, what in ((o["mean"], mean_t, "save_mean"), (o["invstd"], invstd_t, "save_invstd"), (o["rm"], rm_t, "running_mean"),
+                                (o["rv"], rv_t, "running_var"), (planes[:, :, 1 - i], y_t.view(n, hw, c).permute(0, 2, 1), "y")):
+            same(got, want, f"{what} of batch norm {i}")
+        check_shuffle_mask(o["mask"], y_t.view(m, c))
+        ref.append((y_t.view(m, c), rm_t, rv_t, mean_t, invstd_t))
+    if not two:
+        same(planes[:, :, 0], x.view(n, 2, c, hw)[:, 0], "y's x1 planes")
+    del y, planes, x
+
+    # backward: the native call, then per batch norm torch's g (which needs y, then freed) and dx
+    dy = seeded(m, 2 * c, 55, 1.0, 0.0)
+    for o in st:
+        o.update(dx=nan_filled(m, c), dw=nan_filled(c, dtype=torch.float32), db=nan_filled(c, dtype=torch.float32))
+
+    def bwd(x_, bn, o):
+        return (x_.data_ptr(), o["mask"].data_ptr(), o["dx"].data_ptr(), bn.weight.data_ptr(), o["mean"].data_ptr(), o["invstd"].data_ptr(),
+                o["dw"].data_ptr(), o["db"].data_ptr())
+
+    u_part = bwd(xs[1], bns[1], st[1]) if two else (None,) * 8
+    N.check(lib.b200c_bn_backward_shuffle(dy.data_ptr(), *u_part, *bwd(xs[0], bns[0], st[0]), m, c, buf.data_ptr(), s))
+    torch.cuda.synchronize()
+    check_scratch(buf, need)
+    gs = [torch.ops.aten.threshold_backward(dy.view(m, c, 2)[:, :, 1 - i], ref[i][0], 0).reshape(m, c, 1, 1) for i in range(nb)]
+    del dy
+    for i, (bn, o) in enumerate(zip(bns, st)):
+        y_t, rm_t, rv_t, mean_t, invstd_t = ref[i]
+        ref[i] = None
+        del y_t, o["mask"]
+        dx_t, dw_t, db_t = torch.ops.aten.native_batch_norm_backward(gs[i], xs[i].view(m, c, 1, 1), bn.weight.detach(), rm_t, rv_t,
+                                                                     mean_t, invstd_t, True, 1e-5, [True, True, True])
+        gs[i] = None
+        same(o["dx"], dx_t.view(m, c), f"dx of batch norm {i}")
+        same(o["dw"], dw_t, f"dweight of batch norm {i}")
+        same(o["db"], db_t, f"dbias of batch norm {i}")
+        del dx_t
 
 
 # ---- squeeze-and-excitation sites ---------------------------------------------------------------------------------

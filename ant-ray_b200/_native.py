@@ -118,6 +118,9 @@ SYMBOLS = {
     "b200c_bn_infer": (c_int, [c_void_p] * 7 + [c_int, c_float, c_int, c_int, c_void_p]),
     "b200c_bn_infer_dual": (c_int, [c_void_p] * 7 + [c_float] + [c_void_p] * 4 + [c_float, c_int, c_int, c_int, c_void_p]),
     "b200c_bn_infer_pool": (c_int, [c_void_p] * 6 + [c_int, c_float] + [c_int] * 4 + [c_void_p]),
+    "b200c_bn_forward_pool2": (c_int, [c_void_p] * 10 + [c_int] * 4 + [c_float, c_float, c_void_p, c_void_p]),
+    "b200c_bn_backward_pool2": (c_int, [c_void_p] * 9 + [c_int] * 4 + [c_void_p, c_void_p]),
+    "b200c_bn_infer_pool2": (c_int, [c_void_p] * 6 + [c_int, c_float] + [c_int] * 4 + [c_void_p]),
     "b200c_bn_forward_act": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "b200c_bn_backward_act": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200c_bn_infer_act": (c_int, [c_void_p] * 6 + [c_int, c_float, c_int, c_int, c_int, c_void_p]),

@@ -1645,6 +1645,85 @@ extern "C" int b200c_bn_infer_pool(const void* x, void* y, const void* weight, c
   return run_infer({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, h, w}, stream);
 }
 
+// VGG's stage end, max_pool2d(relu(bn(x)), 2, 2) (norm_pool2.cuh): n images of h x w rows, h and w at least 2 (torch's
+// max_pool2d refuses an output of zero rows or columns), channels 1..kMaxChannels, n * h * w * channels below 2^31, and
+// every bf16 operand on its 2-byte grid and every fp32 one on its 4-byte grid (the kernels run 8 channels per thread
+// where all of them are also on the 16-byte grid and channels % 8 == 0, else 1).
+static int check_pool2(const char* site, int n, int h, int w, int c, int* m) {
+  if (n < 1 || h < 2 || w < 2 || c < 1 || c > bn::kMaxChannels || (int64_t)n * h * w * c > INT32_MAX)
+    return fail(B200C_EINVAL, "%s: bad shape n=%d h=%d w=%d channels=%d", site, n, h, w, c);
+  *m = n * h * w;
+  return B200C_OK;
+}
+
+static int check_grid(const char* site, std::initializer_list<const void*> bf16s, std::initializer_list<const void*> fp32s) {
+  for (const void* q : bf16s)
+    if (reinterpret_cast<uintptr_t>(q) % 2) return fail(B200C_EINVAL, "%s: a bf16 operand is off the 2-byte grid", site);
+  for (const void* q : fp32s)
+    if (reinterpret_cast<uintptr_t>(q) % 4) return fail(B200C_EINVAL, "%s: an fp32 operand is off the 4-byte grid", site);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_forward_pool2(const void* x, void* y, uint8_t* argmax, const float* weight, const float* bias,
+                                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                                      float* save_invstd, int n, int h, int w, int channels, float momentum, float eps, void* scratch,
+                                      b200c_stream_t stream) {
+  const char* site = "batch norm pool2 forward";
+  if (!x || !y || !argmax || !weight || !bias || !running_mean || !running_var || !save_mean || !save_invstd || !scratch)
+    return fail(B200C_EINVAL, "%s: null buffer", site);
+  int m = 0;
+  int rc = check_pool2(site, n, h, w, channels, &m);
+  if (!rc) rc = check_grid(site, {x, y}, {weight, bias, running_mean, running_var, save_mean, save_invstd});
+  if (!rc && reinterpret_cast<uintptr_t>(num_batches_tracked) % 8)
+    rc = fail(B200C_EINVAL, "%s: num_batches_tracked is off the 8-byte grid", site);
+  if (rc) return rc;
+  bn::FwdArgs a{x, nullptr, y, nullptr, true, weight, bias, running_mean, running_var,
+                reinterpret_cast<long long*>(num_batches_tracked), save_mean, save_invstd, m, channels, momentum, eps, scratch};
+  a.argmax = argmax;
+  a.pool_h = h;
+  a.pool_w = w;
+  RT(bn::forward_pool2(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_backward_pool2(const void* dy, const uint8_t* argmax, const void* x, void* dx, const float* weight,
+                                       const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
+                                       int h, int w, int channels, void* scratch, b200c_stream_t stream) {
+  const char* site = "batch norm pool2 backward";
+  if (!dy || !argmax || !x || !dx || !weight || !save_mean || !save_invstd || !grad_weight || !grad_bias || !scratch)
+    return fail(B200C_EINVAL, "%s: null buffer", site);
+  int m = 0;
+  int rc = check_pool2(site, n, h, w, channels, &m);
+  if (!rc) rc = check_grid(site, {dy, x, dx}, {weight, save_mean, save_invstd, grad_weight, grad_bias});
+  if (rc) return rc;
+  bn::BwdArgs a{dy, nullptr, nullptr, nullptr, x, nullptr, dx, true, weight, save_mean, save_invstd, nullptr, grad_weight, grad_bias,
+                m, channels, scratch};
+  a.argmax = argmax;
+  a.pool_h = h;
+  a.pool_w = w;
+  RT(bn::backward_pool2(a, (cudaStream_t)stream));
+  g_launches.fetch_add(2);
+  return B200C_OK;
+}
+
+extern "C" int b200c_bn_infer_pool2(const void* x, void* y, const void* weight, const void* bias, const void* running_mean,
+                                    const void* running_var, int param_bf16, float eps, int n, int h, int w, int channels,
+                                    b200c_stream_t stream) {
+  const char* site = "batch norm infer pool2";
+  if (!x || !y || !weight || !bias || !running_mean || !running_var) return fail(B200C_EINVAL, "%s: null buffer", site);
+  int m = 0;
+  int rc = check_pool2(site, n, h, w, channels, &m);
+  if (!rc) rc = check_infer(site, param_bf16, m, channels);
+  if (!rc) rc = param_bf16 ? check_grid(site, {x, y, weight, bias, running_mean, running_var}, {})
+                           : check_grid(site, {x, y}, {weight, bias, running_mean, running_var});
+  if (rc) return rc;
+  RT(bn::infer_pool2({x, nullptr, y, {weight, bias, running_mean, running_var, eps}, {}, false, param_bf16 != 0, m, channels, h, w},
+                     (cudaStream_t)stream));
+  g_launches.fetch_add(1);
+  return B200C_OK;
+}
+
 // A batch norm followed by ReLU6, SiLU or Hardswish (norm_act.cuh): the local site's checks, an activation the kernels
 // have, and (the eval site too) at most kMaxChannels channels.
 static int check_act(const char* site, int act, int c) {

@@ -1,5 +1,5 @@
 // Launchers of the fused batch-norm kernels (norm_kernels.cuh, norm_infer.cuh, norm_act.cuh, norm_res.cuh, norm_cat.cuh,
-// norm_slice.cuh, norm_shuffle.cuh); argument checking lives in b200coll.cu.
+// norm_slice.cuh, norm_shuffle.cuh, norm_pool2.cuh); argument checking lives in b200coll.cu.
 #include <algorithm>
 #include <initializer_list>
 #include <type_traits>
@@ -9,6 +9,7 @@
 #include "norm_infer.cuh"
 #include "norm_kernels.cuh"
 #include "norm_launch.h"
+#include "norm_pool2.cuh"
 #include "norm_res.cuh"
 #include "norm_shuffle.cuh"
 #include "norm_slice.cuh"
@@ -264,6 +265,31 @@ static ResInferKernel<P> res_infer_kernel(int vec, bool add) {
   });
 }
 
+// VGG's stage end (norm_pool2.cuh): the training and eval pooling kernels take 8 channels per thread or 1, the backward
+// reduce kBwdVec or 1.
+using Pool2FwdKernel = void (*)(const bf16*, bf16*, uint8_t*, const float*, const float*, const float*, const float*, bn_pool2::Dims,
+                                int, int);
+using Pool2BwdReduceKernel = void (*)(const bf16*, const bf16*, const uint8_t*, const float*, const float*, float*, float*, float*,
+                                      float*, volatile float*, int*, bn_pool2::Dims, int, int);
+using Pool2BwdElemtKernel = void (*)(const bf16*, const uint8_t*, const bf16*, bf16*, const float*, const float*, const float*,
+                                     const float*, const float*, float, bn_pool2::Dims, int, int);
+template <typename P>
+using Pool2InferKernel = void (*)(const bf16*, bf16*, const P*, const P*, const P*, const P*, float, bn_pool2::Dims, int, int);
+
+static Pool2FwdKernel pool2_fwd_kernel(int vec) {
+  return with_const<1, kEwVec>(vec, [](auto v) -> Pool2FwdKernel { return bn_pool2::k_pool2_fwd<decltype(v)::value>; });
+}
+static Pool2BwdReduceKernel pool2_bwd_reduce_kernel(int vec) {
+  return with_const<1, kBwdVec>(vec, [](auto v) -> Pool2BwdReduceKernel { return bn_pool2::k_pool2_bwd_reduce<decltype(v)::value>; });
+}
+static Pool2BwdElemtKernel pool2_bwd_elemt_kernel(int vec) {
+  return with_const<1, kEwVec>(vec, [](auto v) -> Pool2BwdElemtKernel { return bn_pool2::k_pool2_bwd_elemt<decltype(v)::value>; });
+}
+template <typename P>
+static Pool2InferKernel<P> pool2_infer_kernel(int vec) {
+  return with_const<1, kEwVec>(vec, [](auto v) -> Pool2InferKernel<P> { return bn_pool2::k_pool2_infer<decltype(v)::value, P>; });
+}
+
 // Loads every batch-norm kernel into the context (b200coll.cu's load_kernels explains why a loopback world must not
 // load a kernel lazily while a peer's collective waits): every key value goes through the functions above.
 cudaError_t load_kernels() {
@@ -293,6 +319,14 @@ cudaError_t load_kernels() {
   load(&bn_shuffle::k_shuffle_infer<true, float>);
   load(&bn_shuffle::k_shuffle_infer<false, bf16>);
   load(&bn_shuffle::k_shuffle_infer<true, bf16>);
+  for (int vec : {1, kEwVec}) {
+    load(pool2_fwd_kernel(vec));
+    load(pool2_bwd_elemt_kernel(vec));
+    load(pool2_infer_kernel<float>(vec));
+    load(pool2_infer_kernel<bf16>(vec));
+  }
+  load(pool2_bwd_reduce_kernel(1));
+  load(pool2_bwd_reduce_kernel(kBwdVec));
   for (int src = 0; src < kGradSrcs; src++) {
     load(bwd_reduce_kernel(src, false));
     load(bwd_reduce_kernel(src, true));
@@ -898,6 +932,74 @@ static cudaError_t launch_infer_shuffle(const InferArgs& a, const void* x1, int 
 
 cudaError_t infer_shuffle(const InferArgs& a, const void* x1, int x1_stride, int hw, cudaStream_t st) {
   return a.param_bf16 ? launch_infer_shuffle<bf16>(a, x1, x1_stride, hw, st) : launch_infer_shuffle<float>(a, x1, x1_stride, hw, st);
+}
+
+// ---- VGG's stage end (norm_pool2.cuh) ----
+// The statistics are launch_stats'.  The pooling kernels run one thread per pooled row and 8 (or 1) channels, the
+// backward reduce reduce_config's launch for [m][C] with kBwdVec (or 1) channels per hardware thread, and the backward
+// elementwise kernel ew_config's launch for [m][C].
+static bn_pool2::Dims pool2_dims(int h, int w) { return bn_pool2::Dims{h, w, h / 2, w / 2}; }
+static int pool2_rows(int m, int h, int w) { return m / (h * w) * (h / 2) * (w / 2); }
+
+cudaError_t forward_pool2(const FwdArgs& a, cudaStream_t st) {
+  cudaError_t e = launch_stats(a, nullptr, st);
+  if (e != cudaSuccess) return e;
+  const int rows = pool2_rows(a.m, a.pool_h, a.pool_w);
+  const void* ptrs[3] = {a.x, a.y, a.argmax};
+  const int vec = vec_ok(a.c, ptrs, 3) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(rows, a.c, vec, &block, &grid);
+  const Pool2FwdKernel k = pool2_fwd_kernel(vec);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), static_cast<uint8_t*>(a.argmax), a.save_mean,
+                            a.save_invstd, a.weight, a.bias, pool2_dims(a.pool_h, a.pool_w), rows, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t backward_pool2(const BwdArgs& a, cudaStream_t st) {
+  Scratch s = carve(a.scratch, a.c);
+  const bn_pool2::Dims d = pool2_dims(a.pool_h, a.pool_w);
+  const bf16* dy = static_cast<const bf16*>(a.dy);
+  const bf16* x = static_cast<const bf16*>(a.x);
+  const uint8_t* argmax = static_cast<const uint8_t*>(a.argmax);
+  const void* ptrs[4] = {a.x, a.dy, a.argmax, a.dx};
+  dim3 block, grid;
+  reduce_config(a.m, a.c, &block, &grid);
+  const int rvec = vec_ok(a.c, ptrs, 3) ? kBwdVec : 1;
+  block.x /= rvec;
+  const Pool2BwdReduceKernel r = pool2_bwd_reduce_kernel(rvec);
+  if (!r) return kNoKernel;
+  r<<<grid, block, 0, st>>>(x, dy, argmax, a.save_mean, a.save_invstd, s.sums, s.sums + a.c, a.grad_weight, a.grad_bias, s.staging,
+                            s.semaphores, d, a.m, a.c);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const int vec = vec_ok(a.c, ptrs, 4) ? kEwVec : 1;
+  ew_config(a.m, a.c, vec, &block, &grid);
+  const Pool2BwdElemtKernel k = pool2_bwd_elemt_kernel(vec);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(dy, argmax, x, static_cast<bf16*>(a.dx), a.save_mean, a.save_invstd, a.weight, s.sums, s.sums + a.c,
+                            (float)(1.0 / a.m), d, a.m, a.c);
+  return cudaGetLastError();
+}
+
+template <typename P>
+static cudaError_t launch_infer_pool2(const InferArgs& a, cudaStream_t st) {
+  auto p = [](const void* q) { return static_cast<const P*>(q); };
+  const InferParams& b = a.bn;
+  const int rows = pool2_rows(a.m, a.pool_h, a.pool_w);
+  const void* ptrs[2] = {a.x, a.y};
+  const int vec = vec_ok(a.c, ptrs, 2) ? kEwVec : 1;
+  dim3 block, grid;
+  ew_config(rows, a.c, vec, &block, &grid);
+  const Pool2InferKernel<P> k = pool2_infer_kernel<P>(vec);
+  if (!k) return kNoKernel;
+  k<<<grid, block, 0, st>>>(static_cast<const bf16*>(a.x), static_cast<bf16*>(a.y), p(b.running_mean), p(b.running_var), p(b.weight),
+                            p(b.bias), b.eps, pool2_dims(a.pool_h, a.pool_w), rows, a.c);
+  return cudaGetLastError();
+}
+
+cudaError_t infer_pool2(const InferArgs& a, cudaStream_t st) {
+  return a.param_bf16 ? launch_infer_pool2<bf16>(a, st) : launch_infer_pool2<float>(a, st);
 }
 
 }  // namespace bn

@@ -161,5 +161,12 @@ cudaError_t forward_shuffle(const FwdArgs& a, const FwdArgs* b, const void* x1, 
 cudaError_t backward_shuffle(const BwdArgs& a, const BwdArgs* b, cudaStream_t s);
 cudaError_t infer_shuffle(const InferArgs& a, const void* x1, int x1_stride, int hw, cudaStream_t s);
 
+// VGG's stage end, max_pool2d(relu(bn(x)), 2, 2) (norm_pool2.cuh): FwdArgs, BwdArgs and InferArgs as at the stem (pool_h
+// by pool_w images, h, w >= 2), with n * (h / 2) * (w / 2) pooled rows and one argmax byte per pooled element.  The
+// backward writes no g (BwdArgs.dy_masked is unused).  2 kernels per training direction, 1 in eval.
+cudaError_t forward_pool2(const FwdArgs& a, cudaStream_t s);
+cudaError_t backward_pool2(const BwdArgs& a, cudaStream_t s);
+cudaError_t infer_pool2(const InferArgs& a, cudaStream_t s);
+
 }  // namespace bn
 }  // namespace b200c

@@ -1,6 +1,6 @@
-"""Fused batch norm for the training step and eval forward of ResNets, DenseNets, Inception v3, GoogLeNet, ShuffleNetV2
-and torchvision's Conv2dNormActivation blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh,
-norm_res.cuh, norm_cat.cuh, norm_slice.cuh, norm_shuffle.cuh), and the
+"""Fused batch norm for the training step and eval forward of ResNets, DenseNets, Inception v3, GoogLeNet, ShuffleNetV2,
+VGG-BN and torchvision's Conv2dNormActivation blocks (libb200coll.so, norm_kernels.cuh, norm_infer.cuh, norm_act.cuh,
+norm_res.cuh, norm_cat.cuh, norm_slice.cuh, norm_shuffle.cuh, norm_pool2.cuh), and the
 squeeze-and-excitation of EfficientNet and MobileNetV3 blocks (se_kernels.cuh).
 
 Every batch norm of a torchvision ResNet is followed by a ReLU, by `+= identity` and a ReLU (a block's tail), or
@@ -100,6 +100,18 @@ one shape with at most 65536 channels, a stride-1 block's input is contiguous NC
 local site by the rules above; where a branch Sequential, a tail batch norm or its ReLU has a hook, a global hook is
 registered, or in eval with gradients recorded, the block runs its parent's forward, and where only the operands or the
 sites fail, the modules, torch.cat and channel_shuffle.  Block ends are never sync sites.
+
+VGG-BN: `fuse_model` also swaps torchvision's `VGG`, whose forward walks `features` group by group.  Each stage's end,
+Conv2d, batch norm, ReLU and nn.MaxPool2d(2, 2), is one stage-end site (`bn_relu_maxpool`, norm_pool2.cuh) that writes
+only the pooled output and one argmax byte per pooled element, which also stands in for the ReLU's mask; relu(bn(x)) is
+never written or saved, and the backward rebuilds the batch norm's output gradient from the pooled gradient and those
+bytes.  Every other Conv2d, batch norm and ReLU is a bn_relu site, and any other module runs as a module, so a VGG
+without batch norm computes torchvision's ops.  A stage end runs there when the max-pool is exactly nn.MaxPool2d(2, 2)
+(padding 0, dilation 1, floor mode, no indices) without a hook, the input has at least 2 rows and 2 columns (torch
+raises below that), and the batch norm is an eval or a local site by the rules above; a sync batch norm there runs its
+own module forward, as at the stem.  Where `features` is not an nn.Sequential or has a hook, a global hook is
+registered, or in eval with gradients recorded, the model runs its parent's forward; a hook on a batch norm, ReLU or
+max-pool makes that group call its modules.
 
 Sync batch norm: `sync_batch_norm(model, comm)` gives every `nn.SyncBatchNorm` of the world group the subclass
 `FusedSyncBatchNorm`, which records a peer-memory communicator.  Where such a module runs with a communicator of
@@ -212,6 +224,12 @@ def _pooled_like(x):
     """An empty channels-last output of the stem's nn.MaxPool2d(3, 2, 1) over x."""
     n, c, h, w = x.shape
     return torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+
+
+def _pooled2_like(x):
+    """An empty channels-last output of VGG's nn.MaxPool2d(2, 2) over x: floor(h / 2) x floor(w / 2)."""
+    n, c, h, w = x.shape
+    return torch.empty((n, c, h // 2, w // 2), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
 
 
 class _FusedBatchNorm(torch.autograd.Function):
@@ -366,6 +384,38 @@ class _FusedBatchNormPool(torch.autograd.Function):
         return dx, grad_weight, grad_bias, None
 
 
+class _FusedBatchNormPool2(torch.autograd.Function):
+    """maxpool(relu(bn(x))) in training mode, maxpool being nn.MaxPool2d(2, 2): the end of a VGG stage.  The forward
+    writes the pooled output and one argmax byte per pooled element, never relu(bn(x)) itself; the backward takes the
+    pooled output's gradient and rebuilds the batch norm's output gradient from it and the argmax bytes."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, bn):
+        n, c, h, w = x.shape
+        y = _pooled2_like(x)
+        argmax = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)
+        stats, params, stream, scratch = _forward_args(x, bn, weight, bias)
+        N.check(_native_lib().b200c_bn_forward_pool2(x.data_ptr(), y.data_ptr(), argmax.data_ptr(), *params, n, h, w, c,
+                                                     bn.momentum, bn.eps, scratch, stream))
+        ctx.save_for_backward(x, argmax, weight, stats)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None, None
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        x, argmax, weight, stats = ctx.saved_tensors
+        n, c, h, w = x.shape
+        dx, grad_weight, grad_bias, stream, scratch = _backward_args(x)
+        mean = stats.data_ptr()
+        N.check(_native_lib().b200c_bn_backward_pool2(dy.data_ptr(), argmax.data_ptr(), x.data_ptr(), dx.data_ptr(), weight.data_ptr(),
+                                                      mean, mean + 4 * c, grad_weight.data_ptr(), grad_bias.data_ptr(), n, h, w, c,
+                                                      scratch, stream))
+        return dx, grad_weight, grad_bias, None
+
+
 # eager torch's backward of each activation, g of (dy, t)
 _ACT_BACKWARD = {N.ACT_RELU6: lambda dy, t: torch.ops.aten.hardtanh_backward(dy, t, 0.0, 6.0),
                  N.ACT_SILU: torch.ops.aten.silu_backward, N.ACT_HARDSWISH: torch.ops.aten.hardswish_backward}
@@ -515,10 +565,11 @@ def _infer_params(bn):
             int(bn.weight.dtype == torch.bfloat16))
 
 
-def _infer(bn, x, launch, pooled=False):
-    """The output y of an eval site's one native launch: like x, or with `pooled` the stem's pooled output.
-    `launch(y, params, stream)` makes the C-ABI call from y's pointer, _infer_params(bn) and the current stream."""
-    y = _pooled_like(x) if pooled else torch.empty_like(x)
+def _infer(bn, x, launch, like=torch.empty_like):
+    """The output y of an eval site's one native launch, `like(x)`: like x, or a pooled output (_pooled_like,
+    _pooled2_like).  `launch(y, params, stream)` makes the C-ABI call from y's pointer, _infer_params(bn) and the
+    current stream."""
+    y = like(x)
     N.check(launch(y.data_ptr(), _infer_params(bn), _raw_stream(x.device.index)))
     return y
 
@@ -1023,16 +1074,35 @@ def _pool_fusable(pool):
             and two(pool.dilation, 1) and not pool.ceil_mode and not pool.return_indices and not _hooked(pool))
 
 
+def _pool2_fusable(pool):
+    """Whether the VGG stage-end kernels can replace `pool`'s call: `pool` is exactly nn.MaxPool2d(2, 2) (padding 0,
+    dilation 1, floor mode, no indices) without a hook of its own (the site's `_site` checks the global ones)."""
+    two = lambda v, k: v in (k, (k, k))  # noqa: E731
+    return (type(pool) is nn.MaxPool2d and two(pool.kernel_size, 2) and two(pool.stride, 2) and two(pool.padding, 0)
+            and two(pool.dilation, 1) and not pool.ceil_mode and not pool.return_indices and not _hooked(pool))
+
+
 def bn_relu_maxpool(bn, relu, pool, x):
-    """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) and the batch norm can run as an
-    eval or a local training site; otherwise bn_relu and the module call."""
+    """pool(relu(bn(x))), fused into one site when `pool` is nn.MaxPool2d(3, 2, 1) (the ResNet stem) or nn.MaxPool2d(2,
+    2) (a VGG stage end) and the batch norm can run as an eval or a local training site; otherwise bn_relu and the
+    module call."""
     site = _site(bn, x, (relu,), sync=False) if type(relu) is nn.ReLU and _pool_fusable(pool) else None
     if site is _EVAL:
         n, c, h, w = x.shape
         return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_pool(x.data_ptr(), y, *p, bn.eps, n, h, w, c, s),
-                      pooled=True)
+                      like=_pooled_like)
     if site is _LOCAL:
         return _FusedBatchNormPool.apply(x, bn.weight, bn.bias, bn)
+    # VGG's stage end; an h or w below 2 is left to torch's max_pool2d, which raises for it
+    site = None
+    if type(relu) is nn.ReLU and _pool2_fusable(pool) and x.dim() == 4 and min(x.shape[2:]) >= 2:
+        site = _site(bn, x, (relu,), sync=False)
+    if site is _EVAL:
+        n, c, h, w = x.shape
+        return _infer(bn, x, lambda y, p, s: _native_lib().b200c_bn_infer_pool2(x.data_ptr(), y, *p, bn.eps, n, h, w, c, s),
+                      like=_pooled2_like)
+    if site is _LOCAL:
+        return _FusedBatchNormPool2.apply(x, bn.weight, bn.bias, bn)
     return pool(bn_relu(bn, relu, x))
 
 
@@ -1583,6 +1653,50 @@ else:
     _SHUFFLE_SWAP = {shufflenetv2.InvertedResidual: FusedShuffleInvertedResidual, shufflenetv2.ShuffleNetV2: FusedShuffleNetV2}
 
 
+try:
+    from torchvision.models import vgg
+except ImportError:  # without torchvision there is nothing to rewrite
+    _VGG_SWAP = {}
+else:
+
+    def _vgg_features(features, x):
+        """VGG's `features` walked group by group: Conv2d, batch norm and ReLU followed by a max-pool is one
+        bn_relu_maxpool site, without one a bn_relu site; every other module (and so every module of a VGG without
+        batch norm) is called as a module."""
+        mods = list(features)
+        i = 0
+        while i < len(mods):
+            if (i + 2 < len(mods) and type(mods[i]) is nn.Conv2d and isinstance(mods[i + 1], (nn.BatchNorm2d, nn.SyncBatchNorm))
+                    and type(mods[i + 2]) is nn.ReLU):
+                conv, bn, relu = mods[i:i + 3]
+                if i + 3 < len(mods) and type(mods[i + 3]) is nn.MaxPool2d:
+                    x = bn_relu_maxpool(bn, relu, mods[i + 3], conv(x))
+                    i += 4
+                else:
+                    x = bn_relu(bn, relu, conv(x))
+                    i += 3
+            else:
+                x = mods[i](x)
+                i += 1
+        return x
+
+    class FusedVGG(vgg.VGG):
+        """VGG whose `features` run group by group: each stage's last Conv2d, batch norm, ReLU and max-pool a
+        bn_relu_maxpool site, every other Conv2d, batch norm and ReLU a bn_relu site, anything else its module; avgpool,
+        flatten and the classifier run as torchvision runs them.  A `features` that is not an nn.Sequential or has a
+        hook of its own, a global hook, and eval with gradients recorded run the parent's forward."""
+
+        def forward(self, x):
+            f = self.features
+            if (not self.training and torch.is_grad_enabled()) or type(f) is not nn.Sequential or _hooked(f) or _global_hooks():
+                return super().forward(x)
+            x = self.avgpool(_vgg_features(f, x))
+            x = torch.flatten(x, 1)
+            return self.classifier(x)
+
+    _VGG_SWAP = {vgg.VGG: FusedVGG}
+
+
 # Torch sums a tensor of fewer elements than this (2^31 bytes of bf16) in one launch of its reduce kernel, whose order
 # the squeeze-excitation kernels restate; a larger one it splits into 32-bit-indexed pieces.
 _SE_MAX_NUMEL = 2 ** 30
@@ -1771,7 +1885,9 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module w
     module's output (`bn_relu_concat`).  Every module whose class is exactly torchvision's ShuffleNetV2 or its
     InvertedResidual gets the fused subclass: the stem is one bn_relu_maxpool site, conv5 a bn_relu site, and each
     block's branches run module by module into one block-end site that writes the shuffled output directly
-    (`bn_relu_shuffle`).  Parameters, buffers, state_dict keys, hooks and the
+    (`bn_relu_shuffle`).  Every module whose class is exactly torchvision's VGG gets the fused subclass: each stage's
+    last batch norm, ReLU and 2 x 2 max-pool is one bn_relu_maxpool site and every other batch norm and ReLU a bn_relu
+    site (a VGG without batch norm runs torchvision's ops).  Parameters, buffers, state_dict keys, hooks and the
     object itself are unchanged, and a second call changes nothing.  Every fused site has eager torch's bits, in
     training and in eval (see `fuse_resnet` for inference).
 
@@ -1784,7 +1900,7 @@ an MBConv or MobileNetV3 block becomes a FusedSqueezeExcitation.  Every module w
         for mod in model.modules():
             if type(mod) is Conv2dNormActivation and len(mod) == 3 and type(mod[2]) in _ACT_CODES:
                 mod.__class__ = FusedConv2dNormActivation
-    swap = {**_RES_SWAP, **_DENSE_SWAP, **_SLICE_SWAP, **_SHUFFLE_SWAP}
+    swap = {**_RES_SWAP, **_DENSE_SWAP, **_SLICE_SWAP, **_SHUFFLE_SWAP, **_VGG_SWAP}
     for mod in model.modules():
         cls = swap.get(type(mod))
         if cls is not None:

@@ -129,7 +129,8 @@ def prepare_model(model: torch.nn.Module, move_to_device: Union[bool, torch.devi
     EfficientNet), the inverted-residual blocks with their projection batch norm and squeeze-and-excitation, a
     torchvision DenseNet (whose concatenating batch norms then read the feature maps in place), torchvision's
     Inception v3 and GoogLeNet (whose Inception modules' branches then write into their concatenation in place), and
-    torchvision's ShuffleNetV2 (whose blocks' branch ends then write the shuffled block output directly), is first
+    torchvision's ShuffleNetV2 (whose blocks' branch ends then write the shuffled block output directly), and
+    torchvision's VGG (whose stage ends then run batch norm, ReLU and the 2 x 2 max-pool as one site), is first
     rewritten in place by `fused_norm.fuse_model`, and with more than one rank the
     model's `nn.SyncBatchNorm` layers over the world group run on peer memory (`fused_norm.sync_batch_norm`, the
     communicator kept as `.b200_norm_comm`); SyncBatchNorm over a subgroup stays on torch.  The rewritten blocks'

@@ -361,6 +361,32 @@ int b200c_bn_backward_pool(const void* dy, const uint8_t* argmax, const void* x,
                            const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
                            int h, int w, int channels, void* scratch, b200c_stream_t stream);
 
+/* VGG-BN's stage end, maxpool(relu(bn(x))) with torch's nn.MaxPool2d(2, stride=2) (floor mode), over n images of h x w
+ * rows (m = n * h * w), bit-identical to eager torch's batch norm, ReLU and channels-last max_pool2d.  Scratch,
+ * statistics and their contract are those of b200c_bn_forward (b200c_bn_scratch_bytes(channels)).  h >= 2, w >= 2,
+ * channels 1..131072 and n * h * w * channels below 2^31; bf16 operands sit on the 2-byte grid and fp32 ones on the
+ * 4-byte grid (8 channels per thread where channels % 8 == 0 and every operand is on the 16-byte grid).  Every
+ * argument is checked before the first launch.
+ * Forward: y receives the pooled output, n * (h / 2) * (w / 2) channels-last rows (an odd h or w leaves its last row
+ * or column out of every window), and `argmax` one byte per pooled element: the position ((row & 1) * 2 + (column &
+ * 1)) in its window of the element it selected (rows first, the first maximum and the last NaN win), or 255 where the
+ * maximum is <= 0 and the ReLU passes no gradient.  relu(bn(x)) itself is not written.  2 kernels.
+ * Backward: from dy (the gradient of y, channels-last), argmax and x writes dx, grad_weight and grad_bias.  An element's
+ * batch-norm output gradient is its window's dy as it is where the window selected it, else +0; it is rebuilt by both
+ * kernels and never written.  2 kernels.
+ * b200c_bn_infer_pool2: eval, y = max_pool2d(relu(bn(x)), 2, 2) from the running statistics, fp32 (param_bf16 0) or
+ * bf16 (1) parameters, as b200c_bn_infer; writes the pooled rows only (no argmax).  1 kernel. */
+int b200c_bn_forward_pool2(const void* x, void* y, uint8_t* argmax, const float* weight, const float* bias,
+                           float* running_mean, float* running_var, int64_t* num_batches_tracked, float* save_mean,
+                           float* save_invstd, int n, int h, int w, int channels, float momentum, float eps, void* scratch,
+                           b200c_stream_t stream);
+int b200c_bn_backward_pool2(const void* dy, const uint8_t* argmax, const void* x, void* dx, const float* weight,
+                            const float* save_mean, const float* save_invstd, float* grad_weight, float* grad_bias, int n,
+                            int h, int w, int channels, void* scratch, b200c_stream_t stream);
+int b200c_bn_infer_pool2(const void* x, void* y, const void* weight, const void* bias, const void* running_mean,
+                         const void* running_var, int param_bf16, float eps, int n, int h, int w, int channels,
+                         b200c_stream_t stream);
+
 /* ---- fused batch norm (eval) over channels-last bf16 activations ----
  * An eval-mode batch norm with its running statistics and what follows it in a ResNet, in one kernel, bit-identical
  * to eager torch's batch_norm (train = false: invstd = rsqrt(float(running_var) + eps), then w * (x - mean) * invstd

@@ -3,7 +3,8 @@
 (mobilenet_v2, mobilenet_v3_large, efficientnet_b0, efficientnet_v2_s, regnet_y_400mf), in DenseNet's dense layers
 (densenet121, densenet161, densenet169, densenet201, by `--models` only) or in Inception's BasicConv2d blocks
 (inception_v3 at 299 x 299 and googlenet, aux heads on, by `--models` only) or in ShuffleNetV2's blocks
-(shufflenet_v2_x0_5, x1_0, x1_5, x2_0, by `--models` only), with and without
+(shufflenet_v2_x0_5, x1_0, x1_5, x2_0, by `--models` only) or in VGG-BN's stages (vgg11_bn, vgg16_bn, by `--models`
+only), with and without
 `fused_norm.fuse_model`.  The builds (`--builds`): "fused" (fuse_model), "unfused" (the untouched model), "act_only"
 (fuse_model without the inverted-residual blocks' projection sites: only the Conv2dNormActivation sites are fused) and
 "no_se" (fuse_model with the squeeze-excitation modules back on torchvision's class).
@@ -43,6 +44,8 @@ MODELS = ["mobilenet_v2", "mobilenet_v3_large", "efficientnet_b0", "efficientnet
 # first match wins
 FAMILIES = [
     ("bn_shuffle", r"b200c::bn_shuffle::k_shuffle"),   # ShuffleNetV2's block ends, every direction but the statistics
+    ("bn_pool2", r"b200c::bn_pool2::k_pool2"),       # VGG's stage ends, every direction but the statistics
+    ("torch_max_pool", r"max_pool"),                  # torch's max_pool2d forward and backward
     ("bn_cat", r"b200c::bn_cat::k_cat"),             # DenseNet's concatenation sites, every direction
     ("bn_slice", r"b200c::bn_slice::k_slice"),       # Inception's slice sites, every direction but the statistics
     ("torch_cat", r"CatArrayBatchedCopy"),
